@@ -1,7 +1,8 @@
 """Loader of the UNMODIFIED reference for the baseline legs of bench.py (and nothing else).
 
-The reference's pure-Python forward path is staged byte-identical under the git-ignored `baseline/_ref/` by
-`tools/stage_reference.py` (it travels to the GPU box with the gpurun snapshot; `/root/reference` does not exist there).
+The reference's pure-Python forward path is staged byte-identical under the git-ignored `oracle/_ref/reference/` by
+`oracle/stage_reference.py` (called from `__graft_entry__.build()` where a reference checkout is present), so it is
+available wherever the built tree is, including machines without the reference checkout.
 This module puts that tree on sys.path and builds `spann3r.model.Spann3R` (`spann3r/model.py:214-226`) on the synthetic
 checkpoint the product is benchmarked on.  Baseline infrastructure: nothing under `spann3r_b200/` imports it.
 """
@@ -13,8 +14,9 @@ import sys
 import tempfile
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-_CANDIDATES = (os.path.join(HERE, "_ref"), "/root/reference")
-CUROPE_DIR = os.path.join(HERE, "_ref_curope")
+_REF_OUT = os.path.join(os.path.dirname(HERE), "oracle", "_ref")   # written by oracle/stage_reference.py
+_CANDIDATES = (os.path.join(_REF_OUT, "reference"),)
+CUROPE_DIR = os.path.join(_REF_OUT, "curope")
 _REF_TOP = ("spann3r", "dust3r", "croco", "models", "curope")
 
 
@@ -41,16 +43,16 @@ def _purge():
 
 
 def load(with_curope: bool = False):
-    """Import (or re-import) the reference's `spann3r.model`.  with_curope: put the sm_100 build of the reference's own
-    CUDA RoPE extension (tools/stage_reference.py --curope) on the path, so that `croco/models/pos_embed.py:106-111`
+    """Import (or re-import) the reference's `spann3r.model`.  with_curope: put the local build of the reference's own
+    CUDA RoPE extension (oracle/stage_reference.py --curope) on the path, so that `croco/models/pos_embed.py:106-111`
     binds RoPE2D to cuRoPE2D instead of the PyTorch fallback.  The choice is made at import time, hence the purge."""
     r = root()
     if r is None:
-        raise ImportError("the reference is not staged: run `python tools/stage_reference.py` where /root/reference exists")
+        raise ImportError("the reference is not staged: run `python -m oracle.stage_reference` where a reference checkout exists")
     _purge()
     if with_curope:
         if not curope_available():
-            raise ImportError("baseline/_ref_curope/curope.so not built (tools/stage_reference.py --curope)")
+            raise ImportError("oracle/_ref/curope/curope.so not built (python -m oracle.stage_reference --curope)")
         sys.path.insert(0, CUROPE_DIR)
     sys.path.insert(0, r)
     import spann3r.model as ref_model   # noqa: the reference

@@ -9,9 +9,16 @@ One "step" = one whole 10-frame 512x384 sequence (BASELINE config[1]) through `S
 batch 1 per GPU, spatial memory reset per sequence).  N > 1: one process per GPU (torchrun), every rank runs its
 own independent sequences (weak scaling, no data-path collective -- SURVEY.md §8e); time = max over ranks.
 Rank 0 prints ONE JSON line.  Keys beyond the base contract: `roofline` (dominant kernel = the split-bf16
-tcgen05 GEMM/conv engine, CUDA-event timed per launch in a separate profiling pass), `cpu_baseline` (the oracle
+wgmma GEMM/conv engine, CUDA-event timed per launch in a separate profiling pass), `cpu_baseline` (the oracle
 port of the reference on the host cores, bounded sample), `e2e` (same metric with pinned-host inputs copied H2D
 and predictions copied D2H inside the timed region), `gpu_launches`, `clocks`.
+
+--dump-outputs DIR: after the timed steps, what `Spann3R.forward` returned in the last timed step is written in float32:
+`preds` as DIR/frame<i>_<key>.npy and the second view of every pair in `preds_all` as DIR/pair<i>_res2_<key>.npy (the
+first view of each pair is preds[i] itself).  At most 64 MB in all: when the arrays are larger (bigger --batch or
+--frames), every array keeps the same fixed sample of its pixels -- n of the N = batch*H*W rows, the indices
+sorted(numpy.random.default_rng(0).choice(N, n, replace=False)) -- and its file name ends in _sample<n>of<N>.  The inputs
+depend only on the arguments (seeded synthetic checkpoint and frames), so two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -36,13 +43,13 @@ def _peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return dict(bf16_sustained=float(d.get("bf16_tflops_sustained", 1454.1)), hbm=float(d.get("hbm_gbs", 6578.3)),
+        return dict(bf16_sustained=float(d.get("bf16_tflops_sustained", 989.0)), hbm=float(d.get("hbm_gbs", 3350.0)),
                     src="measured (MEASURED_PEAKS.json, bf16 sustained)")
-    return dict(bf16_sustained=1400.0, hbm=6650.0, src="fallback (B200_PROFILING.md)")
+    return dict(bf16_sustained=989.0, hbm=3350.0, src="NVIDIA H100 SXM data sheet (dense BF16, HBM3), not reached")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed regions (B200_PROFILING.md recipe).  The process is started
+    """nvidia-smi clocks / throttle reasons during the timed regions (read-only queries).  The process is started
     BEFORE the warm-up (nvidia-smi needs ~0.3 s to deliver its first row; a 5-step run is over by then) and only the rows that
     arrive inside [mark_begin, mark_end] -- the device-timed loop -- are reported; it is stopped before the e2e loop."""
 
@@ -105,13 +112,13 @@ def _host_threads():
 
 
 def _reference_model(sd):
-    """(model, kind): the UNMODIFIED reference `spann3r.model.Spann3R` from the staged copy under baseline/_ref
-    (tools/stage_reference.py) on the synthetic checkpoint -> kind "reference"; None when it is not staged."""
+    """(model, kind): the UNMODIFIED reference `spann3r.model.Spann3R` from the staged copy under oracle/_ref
+    (oracle/stage_reference.py, run by build()) on the synthetic checkpoint -> kind "reference"; None when it is not staged."""
     try:
         from baseline import ref_loader
         from spann3r_b200 import synth
         if ref_loader.root() is None:
-            return None, "reference not staged under baseline/_ref"
+            return None, "reference not staged under oracle/_ref"
         import contextlib
         import io
         with contextlib.redirect_stdout(io.StringIO()):     # the reference prints while constructing
@@ -153,7 +160,7 @@ def _cpu_reference_leg(sd, model_ref, budget_s, max_steps):
             if steps >= max_steps or time.time() - t0 > budget_s:
                 break
     dt = (time.time() - t0) / steps
-    what = "UNMODIFIED reference Spann3R.forward (baseline/_ref)" if kind == "reference" else "oracle port"
+    what = "UNMODIFIED reference Spann3R.forward (oracle/_ref)" if kind == "reference" else "oracle port"
     return {"value": FRAMES / dt, "unit": "frames/s", "cores": cores, "kind": kind, "seconds_per_step": dt, "steps": steps,
             "sample": f"{steps} x the full {FRAMES}-frame {WIDTH}x{HEIGHT} sequence (the headline config), {what}, torch CPU fp32, "
                       f"{cores} threads (OMP_NUM_THREADS={cores})"}
@@ -187,7 +194,7 @@ def run_reference(args):
 def _eager_gpu_legs(mref, why, sd, frames_dev, model, dev, F_):
     """The reference as PyTorch eager on THIS GPU, same frames, batch 1 (SURVEY.md §8d(i)): the staged unmodified
     `Spann3R.forward` with (a) its shipped TF32 default and the PyTorch RoPE fallback it uses when curope is not built,
-    (b) strict fp32, (c) TF32 + the reference's OWN curope extension built for sm_100 (tools/stage_reference.py --curope,
+    (b) strict fp32, (c) TF32 + the reference's OWN curope extension built for this GPU (oracle/stage_reference.py --curope,
     one-token patch) -- the reference's best shot.  Falls back to the oracle port when the reference is not staged.
     Also returns the parity of the CUDA path against the reference's strict-fp32 GPU run on these frames."""
     fr = [{"img": f["img"][:1].contiguous()} for f in frames_dev]
@@ -202,7 +209,7 @@ def _eager_gpu_legs(mref, why, sd, frames_dev, model, dev, F_):
             pg = getattr(mod, "position_getter", None)      # a plain object hanging off PatchEmbed, not an nn.Module
             if pg is not None and hasattr(pg, "cache_positions"):
                 pg.cache_positions = {}
-        what = "UNMODIFIED reference Spann3R.forward (baseline/_ref), PyTorch eager (cuBLAS/cuDNN), batch 1, same frames"
+        what = "UNMODIFIED reference Spann3R.forward (oracle/_ref), PyTorch eager (cuBLAS/cuDNN), batch 1, same frames"
 
         def fwd(f):
             with torch.no_grad(), contextlib.redirect_stdout(io.StringIO()):
@@ -244,7 +251,7 @@ def _eager_gpu_legs(mref, why, sd, frames_dev, model, dev, F_):
         try:
             from baseline import ref_loader
             if not ref_loader.curope_available():
-                raise ImportError("baseline/_ref_curope/curope.so not built")
+                raise ImportError("oracle/_ref/curope/curope.so not built")
             if ref_loader.CUROPE_DIR not in sys.path:
                 sys.path.insert(0, ref_loader.CUROPE_DIR)
             from models.curope.curope2d import cuRoPE2D   # noqa: the reference's own module (staged), now importable
@@ -258,7 +265,7 @@ def _eager_gpu_legs(mref, why, sd, frames_dev, model, dev, F_):
             torch.backends.cudnn.allow_tf32 = True
             v, out2 = timed()
             eager["tf32_default_curope"] = {"value": v, "unit": "frames/s", "rope_modules_switched": len(old),
-                                            "what": "same, RoPE = the reference's own curope CUDA extension built for sm_100 "
+                                            "what": "same, RoPE = the reference's own curope CUDA extension built for this GPU "
                                                     "(kernels.cu:101 one-token patch): the reference's best shot"}
         except Exception as ex:
             eager["tf32_default_curope"] = {"unavailable": repr(ex)[:200]}
@@ -267,6 +274,34 @@ def _eager_gpu_legs(mref, why, sd, frames_dev, model, dev, F_):
             for name, r in locals().get("old", {}).items():
                 mods[name].rope = r
     return eager, parity
+
+
+DUMP_BUDGET = 64 * 1000 * 1000   # bytes of array data written by --dump-outputs
+
+
+def _dump_outputs(out_dir, preds, preds_all):
+    """See the module docstring (--dump-outputs).  The headline config writes 60 MB without sampling."""
+    import numpy as np
+    arrays = {}
+    for i, p in enumerate(preds):
+        for k, v in p.items():
+            arrays[f"frame{i}_{k}"] = v
+    for i, (_, r2) in enumerate(preds_all):
+        for k, v in r2.items():
+            arrays[f"pair{i}_res2_{k}"] = v
+    arrays = {n: v.detach().float() for n, v in arrays.items() if torch.is_tensor(v) and v.is_floating_point()}
+    total = sum(v.numel() * 4 for v in arrays.values())
+    keep = min(1.0, 0.99 * DUMP_BUDGET / max(total, 1))      # 1 % left for the .npy headers
+    os.makedirs(out_dir, exist_ok=True)
+    for name, v in arrays.items():
+        x = v.cpu().numpy()
+        if keep < 1.0:     # pts3d [b, H, W, 3] / conf [b, H, W]: rows = pixels
+            rows = x.reshape(-1, *x.shape[3:]) if x.ndim >= 3 else x.reshape(-1)
+            N = rows.shape[0]
+            n = max(1, int(N * keep))
+            idx = np.sort(np.random.default_rng(0).choice(N, n, replace=False))
+            x, name = rows[idx], f"{name}_sample{n}of{N}"
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(x))
 
 
 def main():
@@ -293,6 +328,8 @@ def main():
                     "random-init checkpoint, SURVEY.md §8d: report both)")
     ap.add_argument("--batch", type=int, default=1,
                     help="sequences advanced in lockstep per GPU (BASELINE config[2] runs 8 per GPU); the headline is 1")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned as DIR/*.npy (float32, at most 64 MB; see above)")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -356,14 +393,17 @@ def main():
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for i in range(K):
-        model(resident[i % n_distinct])
+        last_preds, last_preds_all = model(resident[i % n_distinct])
     e1.record()
     barrier()
     ms = max_over_ranks(e0.elapsed_time(e1))
+    if args.dump_outputs and rank == 0:
+        _dump_outputs(args.dump_outputs, last_preds, last_preds_all)
+    del last_preds, last_preds_all
     launches = eng.take_launches()
     flops_issued = eng.take_flops()
-    # the sampler stops HERE: nvidia-smi polling the driver every 100 ms costs the e2e loop below a third of its throughput
-    # (135 vs 196 frames/s, profiles/r2q_bench.json vs r2m_bench.json) -- its queries serialise with the pinned-memory copies
+    # the sampler stops HERE: nvidia-smi polling the driver every 100 ms slows the e2e loop below -- its queries serialise
+    # with the pinned-memory copies
     sampler.mark_end()
     clocks = sampler.stop() if rank == 0 else None
     value = world * BATCH * F_ * K / (ms / 1e3)
@@ -411,7 +451,7 @@ def main():
         except Exception:
             traffic = None
     roofline = {
-        "bound": "tensor", "kernel": "gemm_bf16x3_kernel (split-bf16 tcgen05 GEMM / implicit-GEMM conv)",
+        "bound": "tensor", "kernel": "gemm_bf16x3_kernel (split-bf16 wgmma GEMM / implicit-GEMM conv)",
         "achieved": gemm_tflops, "peak": pk["bf16_sustained"], "unit": "TFLOP/s", "frac": gemm_tflops / pk["bf16_sustained"],
         "traffic": traffic, "traffic_source": traffic_src, "peak_source": pk["src"],
         "note": "achieved = algorithmic 2MNK FLOPs / CUDA-event time summed over all GEMM/conv launches of one sequence; "
@@ -434,8 +474,7 @@ def main():
         sd_base = sd
         mref, why = _reference_model(sd_base)
         # GPU legs FIRST: a CPU forward leaves the host's OpenMP pool spinning, which depresses whatever is timed on the GPU
-        # right after it (measured: the CUDA arm's own e2e drops from 195 to 138 frames/s under a 64-thread pool,
-        # profiles/r2k_e2e_threads.txt) -- the reference's eager-GPU numbers must not pay for its own CPU leg
+        # right after it -- the reference's eager-GPU numbers must not pay for its own CPU leg
         if want_eager:
             try:
                 eager, parity_ref = _eager_gpu_legs(mref, why, sd_base, resident[0], model, dev, F_)
@@ -517,7 +556,7 @@ def main():
             "config": {"workload": f"{F_}-frame {WIDTH}x{HEIGHT} sequence per step, batch {BATCH} per GPU, ViT-L enc / ViT-B dec + DPT, "
                                    f"random-init {'raw' if args.raw_checkpoint else 'sharpened'} checkpoint (SURVEY.md §8d config 2)",
                        "parallelism": f"{world} independent replicas (one sequence stream per GPU, no collective)",
-                       "l2": "per-step working set (2.6 GB packed weights + activations) >> 126 MB L2; inputs alternate between "
+                       "l2": "per-step working set (2.6 GB packed weights + activations) >> 50 MB L2; inputs alternate between "
                              "2 distinct sequences"},
             "e2e": {"value": e2e, "unit": "frames/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,
                     "ms_per_step": ms_e2e / K},

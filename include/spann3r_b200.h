@@ -1,4 +1,4 @@
-/* spann3r_b200 -- C ABI of the B200-native Spann3R forward path (libspann3r_b200.so).
+/* spann3r_b200 -- C ABI of the H100-native (sm_90a) Spann3R forward path (libspann3r_b200.so).
  *
  * The reference (HengyiWang/spann3r) is Python over PyTorch; its only native boundary is the
  * pybind module `curope` (croco/models/curope/curope.cpp:49-69).  This header is the boundary a
@@ -8,7 +8,7 @@
  * the caller must free except the opaque engine handle.
  *
  * Number format.  Every weight GEMM / convolution on the path consumes fp32 values carried as two
- * bf16 planes (hi = bf16(x), lo = bf16(x - hi)) and issues three tcgen05 MMAs per product
+ * bf16 planes (hi = bf16(x), lo = bf16(x - hi)) and issues three wgmma tensor-core MMAs per product
  * (DESIGN.md section 3).  "planes" below always means such a (hi, lo) pair of identical layout.
  *
  * Each entry point cites the reference code it replaces (paths relative to the reference root).
@@ -34,7 +34,7 @@ int s3r_version(void);
 int s3r_abi_sizeof(int which /* 0 gemm_desc, 1 model_w, 2 bank */);
 /* last error text of the calling thread ("" if none) */
 const char* s3r_last_error(void);
-/* 1 if a CUDA device of compute capability 10.x is visible, else 0 (never falls back to CPU) */
+/* 1 if a CUDA device of compute capability 9.0 (H100, sm_90a) is visible, else 0 (never falls back to CPU) */
 int s3r_device_ok(void);
 
 /* ---- op level ------------------------------------------------------------------------------ */
@@ -109,8 +109,8 @@ typedef struct s3r_gemm_desc {
    * sums of the rows it writes.  All NULL / 0 = plain GEMM. */
   const float* ln_stats; int ln_np; float ln_eps; const float* ln_cs; int a_swap;
   float* stats_out;
-  /* diagnostics: 16 x uint64 %globaltimer stamps of CTA 0 (entry, prologue done, dependency wait done, first operands
-   * landed, accumulator ready, epilogue done, exit, ...; tools/trace_gemm.py); NULL = off.  1-CTA kernel only. */
+  /* diagnostics: %globaltimer stamps of CTA 0 in slots 0..6 of a 16 x uint64 buffer (entry, prologue done, dependency
+   * wait done, first operands landed, accumulator ready, epilogue done, exit; tools/trace_gemm.py); NULL = off. */
   uint64_t* trace;
   /* merged projections: a_swap applies to output columns >= swap_col0 only (0 = all; a multiple of 256), and EPI_QKV
    * roles 3 / 4 (columns 3*q_c .. 5*q_c) are a second K / V^T pair written to k2_out / vt2_out -- the decoder's
@@ -118,10 +118,10 @@ typedef struct s3r_gemm_desc {
   int swap_col0; float* k2_out; float* vt2_out;
 } s3r_gemm_desc;
 int s3r_gemm(const s3r_gemm_desc* d, void* stream);
-/* tile width the planner would pick (64/128/256), for tests */
+/* tile width the planner would pick (64/128), for tests */
 int s3r_gemm_tile_n(const s3r_gemm_desc* d);
 
-/* Fused multi-head attention core, head dim 64: O = softmax(Q K^T) V per (batch*head) on tf32 tcgen05.
+/* Fused multi-head attention core, head dim 64: O = softmax(Q K^T) V per (batch*head) on tf32 wgmma.
  *   q [bh, nq, 64], k [bh, nk, 64] (already RoPE'd / scaled by the QKV epilogue), vt [bh, 64, nk_pad];
  *   output [b*nq, heads*64] as planes and/or fp32 (row stride ldo).
  * croco/models/blocks.py:106-110 (self), :162-166 (cross). */
@@ -259,10 +259,9 @@ int s3r_engine_memory_read(s3r_engine* e, const s3r_bank* bank, const float* fea
  * of (seed, (b * N + row) * len + column): reproducible, regenerated for the backward pass / tests by s3r_dropout_mask */
 int s3r_engine_memory_read_train(s3r_engine* e, const s3r_bank* bank, const float* feat, float thresh, float drop_p,
                                  uint64_t seed, float* out, void* stream);
-/* Tuning knobs of the tile planner, read when an engine builds its plans (first pass of a stage): "gemm2" (CTA-pair GEMM
- * tiles: 0 off, 1 planner, 128 / 256 forced), "gemm2_64" (256 x 64 pair tiles for the one-wave N = 768 / 1024 GEMMs),
- * "prefetch_b" (weight tiles staged before the programmatic-dependent-launch wait), "attn_pair".  Defaults = the measured
- * best; the call exists so that two engines of one process can be planned differently and timed alternately. */
+/* Tuning knobs of the GEMM planner, read when an engine builds its plans (first pass of a stage): "prefetch_b" (weight
+ * tiles staged before the programmatic-dependent-launch wait; default 1).  The call exists so that two engines of one
+ * process can be planned differently and timed alternately. */
 int s3r_set_option(const char* name, int value);
 /* out[i] = 0 or 1/(1-p): the keep-scale the training-mode read applies to flat element i = (b * N + row) * len + column */
 int s3r_dropout_mask(float* out, int64_t n, uint64_t seed, float p, void* stream);

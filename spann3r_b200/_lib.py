@@ -1,7 +1,7 @@
 """ctypes binding of libspann3r_b200.so (include/spann3r_b200.h).
 
 This is the ONLY compute backend of the package: if the library is missing or the device is not
-sm_100, every op raises -- there is no CPU, eager-PyTorch or Triton fallback.
+an sm_90 (H100) GPU, every op raises -- there is no CPU, eager-PyTorch or Triton fallback.
 """
 from __future__ import annotations
 
@@ -119,7 +119,7 @@ def check(status: int, what: str = ""):
 
 def require_device():
     if not torch.cuda.is_available() or not lib().s3r_device_ok():
-        raise S3RError("spann3r_b200 needs a CUDA device of compute capability 10.x (B200); no fallback exists")
+        raise S3RError("spann3r_b200 needs a CUDA device of compute capability 9.0 (H100); no fallback exists")
 
 
 def ptr(t):

@@ -1,10 +1,10 @@
-"""`nn.Linear` forward AND backward on the tcgen05 GEMM engine -- the first native piece of the training backward
+"""`nn.Linear` forward AND backward on the wgmma GEMM engine -- the first native piece of the training backward
 (SURVEY.md §8f rank 1).
 
 `_recompute.py` (the PyTorch recompute that `train.py` differentiates) routes every Linear through `linear()` below.  With the
 switch off (default) that is `F.linear` and PyTorch autograd.  With it on, the three GEMMs of a Linear -- y = x W^T + b in the
 recompute, dx = dy W (dgrad) and dW = dy^T x (wgrad) in the backward -- run as split-bf16 (`bf16x3`, ~fp32-accurate) launches of
-`s3r_gemm` through the C ABI: the same `gemm2_bf16x3_kernel` / `gemm_bf16x3_kernel` the forward path uses, operands re-laid-out by
+`s3r_gemm` through the C ABI: the same `gemm_bf16x3_kernel` the forward path uses, operands re-laid-out by
 plain data movement (transpose, zero-pad of the contraction to a multiple of 8, split into planes).  Linears carry ~85 % of the
 backward's FLOPs; attention, LayerNorm, GELU, the DPT convolutions and the elementwise glue remain PyTorch autograd.
 
@@ -30,7 +30,7 @@ def _pad8(t: torch.Tensor) -> torch.Tensor:
 
 
 def gemm_nt(a: torch.Tensor, b: torch.Tensor, bias: torch.Tensor | None = None) -> torch.Tensor:
-    """a [rows, K] @ b[N, K]^T (+ bias) -> fp32 [rows, N] on the split-bf16 tcgen05 engine (N % 32 == 0)."""
+    """a [rows, K] @ b[N, K]^T (+ bias) -> fp32 [rows, N] on the split-bf16 wgmma engine (N % 32 == 0)."""
     assert a.dim() == 2 and b.dim() == 2 and a.shape[1] == b.shape[1] and b.shape[0] % 32 == 0, (tuple(a.shape), tuple(b.shape))
     a, b = _pad8(a.float()).contiguous(), _pad8(b.float()).contiguous()
     out, _, _ = _lib.linear(_lib.split(a), _lib.split(b), bias=None if bias is None else bias.float().contiguous())

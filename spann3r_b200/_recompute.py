@@ -1,6 +1,6 @@
 """PyTorch RECOMPUTE of the four engine stages -- used ONLY by the backward pass of training mode (`train.py`).
 
-This is NOT a forward path: `Spann3R.forward` always runs the sm_100a kernels (training mode included), and nothing here
+This is NOT a forward path: `Spann3R.forward` always runs the sm_90a kernels (training mode included), and nothing here
 is reachable from eval-mode code.  The native dgrad / wgrad kernels of SURVEY.md §8f rank 1 are not written yet; until
 they are, `torch.autograd.Function.backward` of every stage re-evaluates that stage with these differentiable
 restatements (activation checkpointing at stage granularity) and lets PyTorch autograd produce the gradients -- labelled
@@ -20,7 +20,7 @@ ENC_HEADS, DEC_HEADS, VAL_HEADS = 16, 12, 16
 
 
 def _lin(P, n, x):
-    # F.linear + PyTorch autograd by default; with the switch on, forward / dgrad / wgrad on the tcgen05 GEMM engine
+    # F.linear + PyTorch autograd by default; with the switch on, forward / dgrad / wgrad on the wgmma GEMM engine
     return _native_linear.linear(x, P[n + ".weight"], P[n + ".bias"])
 
 

@@ -1,7 +1,7 @@
-"""In-tree build of libspann3r_b200.so (sm_100a only) with nvcc.
+"""In-tree build of libspann3r_b200.so (sm_90a, H100, only) with nvcc.
 
 `python -m spann3r_b200.build` or `__graft_entry__.build()`.  nvcc cross-compiles without a GPU;
-the resulting .so is git-ignored but travels to the GPU box with the gpurun snapshot.
+the resulting .so is git-ignored and rebuilt whenever a source or header is newer.
 """
 from __future__ import annotations
 
@@ -18,7 +18,7 @@ OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libspann3r_b200.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
 ]
 
@@ -39,8 +39,8 @@ def _newer(src_list, target) -> bool:
 
 def build(force: bool = False, verbose: bool = True, defines=(), lib: str = LIB, obj_dir: str = OBJ) -> str:
     """defines / lib / obj_dir: build an A/B variant next to the shipped library, e.g.
-    `python -m spann3r_b200.build --variant NAME -DSOME_MACRO=1` -> ab/libspann3r_b200_NAME.so (git-ignored,
-    travels with gpurun; select it with S3R_LIB=...).  The default build takes no defines."""
+    `python -m spann3r_b200.build --variant NAME -DSOME_MACRO=1` -> ab/libspann3r_b200_NAME.so (git-ignored;
+    select it with S3R_LIB=...).  The default build takes no defines."""
     return _build(force, verbose, tuple(defines), lib, obj_dir)
 
 
@@ -65,7 +65,7 @@ def _build(force, verbose, defines, LIB, OBJ) -> str:
 
     with cf.ThreadPoolExecutor(max_workers=min(8, len(srcs))) as ex:
         objs = list(ex.map(compile_one, srcs))
-    cmd = [nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"]
+    cmd = [nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

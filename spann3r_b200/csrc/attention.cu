@@ -1,4 +1,4 @@
-// Fused multi-head attention core for head dim 64 on tcgen05 (kind::tf32), sm_100a.
+// Fused multi-head attention core for head dim 64 on Hopper wgmma (tf32), sm_90a.
 //
 //   O[b, q, h*64:(h+1)*64] = softmax_k( Q[b,h,q,:] . K[b,h,k,:] ) V[b,h,k,:]
 //
@@ -7,20 +7,16 @@
 // (2-D RoPE), Q pre-scaled by 64^-0.5, V transposed, all rounded to tf32 by the QKV-projection GEMM
 // epilogue (gemm.cu, EPI_QKV), so RoPE never exists as a separate op or tensor.
 //
-// One CTA per (128-query tile, batch*head), 384 threads: warp 0 TMA (Q once, K / V^T per 128-key block into a
-// 3-stage ring), warp 1 MMA issuer, warpgroups 1 and 2 = two softmax groups that take alternate KV blocks
-// (see the kernel comment).  S, P and O live in TMEM; P is the TMEM A operand of the PV MMA.
+// One CTA per (128-query tile, batch*head), 384 threads: warpgroup 0 = TMA producer (Q once, K / V^T per 128-key
+// block into a 3-stage ring), warpgroups 1 and 2 each own 64 query rows for ALL KV blocks: S = Q K^T into registers
+// (wgmma, A and B from shared memory), exact online softmax in registers, O += P V with P as the register A operand.
 // Output: split-bf16 planes (A operand of the following projection GEMM) and/or fp32.
 #include "common.cuh"
 #include "kernels.cuh"
+#include "wgmma.cuh"
 
 #include <cstdlib>
 #include <cstring>
-
-// Registers left to the TMA / MMA warpgroup after setmaxnreg.dec.  40 is the verified build; 64 (128 x 64 + 256 x 224 = the
-// whole 64 K file) was built and run on a B200 in round 2 to remove the pair-tile variant's ~0.2 KB spill: the kernel
-// faults ("unspecified launch failure", gpurun_out/r2a_ab_attn64.err), so the knob is gone and the spill stays.
-#define S3R_ATTN_PRODUCER_REGS 40
 
 namespace s3r {
 
@@ -31,72 +27,27 @@ constexpr int D = 64;
 constexpr int Q_BYTES = BQ * D * 4;       // 32 KB (2 swizzle atoms of [128 x 32 f32])
 constexpr int K_BYTES = BKV * D * 4;      // 32 KB
 constexpr int V_BYTES = D * BKV * 4;      // 32 KB (4 atoms of [64 x 32 f32])
-// PAIR = false: one 128-query tile per CTA, the two softmax groups take alternate KV blocks (merged at the end);
-// PAIR = true: two query tiles per CTA, group g owns tile g for ALL KV blocks -- K/V are loaded once per 256 queries
-// and there is no merge (many-wave launches: the batched encoder).
-template <bool PAIR>
-struct Cfg {
-  static constexpr int QB = PAIR ? 2 * Q_BYTES : Q_BYTES;
-  static constexpr int KV_STAGES = PAIR ? 2 : 3;
-  static constexpr int SMEM = QB + KV_STAGES * (K_BYTES + V_BYTES) + 1024 + 256;
-};
-constexpr uint32_t TMEM_COLS = 512;       // group g: S/P at [g*192, +128), O at [g*192+128, +64)
-constexpr int kThreads = 384;             // warpgroup 0: warp 0 TMA, warp 1 MMA (2, 3 idle); warpgroups 1, 2: softmax
+constexpr int KV_STAGES = 3;
+constexpr int SMEM = Q_BYTES + KV_STAGES * (K_BYTES + V_BYTES) + 1024 + 256;
+constexpr int kThreads = 384;             // warpgroup 0: warp 0 TMA (1..3 idle); warpgroups 1, 2: MMA + softmax
+constexpr int kConsumerWarps = 8;
 }  // namespace attn
 
-// TMEM <- registers (this warp's 32 lanes x 32 columns)
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};\n" ::"r"(taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-      "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]),
-      "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]),
-      "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-// D[tmem] (+)= A[tmem] * B[smem]^T, tf32: A = 128 lanes x 8 columns (one fp32 column per K element)
-__device__ __forceinline__ void umma_tf32_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
-
-// One CTA per (128-query tile, batch*head).  The KV blocks alternate between two softmax warpgroups (even blocks ->
-// group 0, odd -> group 1), each with its own S/P and O regions in TMEM and its own running (max, sum, o[64]) state;
-// while one group runs its softmax the tensor core serves the other group's QK^T / PV, and the two partial results
-// are merged once at the end (flash-decoding style).  P never touches shared memory: the softmax threads overwrite
-// their S row in TMEM with tf32 probabilities (tcgen05.st) and the PV MMA takes its A operand from TMEM.
-template <bool PAIR>
 __global__ void __launch_bounds__(attn::kThreads, 1) attention_kernel(const __grid_constant__ AttnArgs args) {
   using namespace attn;
-  constexpr int KV_STAGES = Cfg<PAIR>::KV_STAGES;
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment by pointer arithmetic on the __shared__ array (an integer round trip would lose the address
   // space and turn every access through `smem` into a generic LD / ST)
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* sQ = smem;
-  uint8_t* sKV = sQ + Cfg<PAIR>::QB;                      // stage s: K at s*(K+V), V after K
+  uint8_t* sKV = sQ + Q_BYTES;                      // stage s: K at s*(K+V), V after K
   uint64_t* bars = reinterpret_cast<uint64_t*>(sKV + KV_STAGES * (K_BYTES + V_BYTES));
-  uint64_t* q_full = bars;            // 1
-  uint64_t* kv_full = bars + 1;       // 3
-  uint64_t* kv_empty = bars + 4;      // 3
-  uint64_t* s_full = bars + 7;        // 2 (per group)
-  uint64_t* p_full = bars + 9;        // 2 (per group, 128 arrivals)
-  uint64_t* o_full = bars + 11;       // 2 (per group)
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 13);
+  uint64_t* q_full = bars;                          // 1
+  uint64_t* kv_full = bars + 1;                     // KV_STAGES
+  uint64_t* kv_empty = bars + 1 + KV_STAGES;        // KV_STAGES
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int q0 = (PAIR ? 2 : 1) * blockIdx.x * BQ;       // PAIR: group g's tile starts at q0 + g * BQ
+  const int q0 = blockIdx.x * BQ;
   const int bh = blockIdx.y;
   const int nblk = (args.nk + BKV - 1) / BKV;
 
@@ -107,34 +58,21 @@ __global__ void __launch_bounds__(attn::kThreads, 1) attention_kernel(const __gr
     mbar_init(q_full, 1);
     for (int i = 0; i < KV_STAGES; ++i) {
       mbar_init(&kv_full[i], 1);
-      mbar_init(&kv_empty[i], 1);
-    }
-    for (int g = 0; g < 2; ++g) {
-      mbar_init(&s_full[g], 1);
-      mbar_init(&p_full[g], 128);
-      mbar_init(&o_full[g], 1);
+      mbar_init(&kv_empty[i], kConsumerWarps);
     }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<TMEM_COLS>(tmem_ptr_smem);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_ptr_smem;
   pdl_launch_dependents();
   pdl_wait();
 
-  // register re-balancing: the TMA / MMA warpgroup needs few registers, each softmax thread holds a 128-key row
   if (warp < 4) {
-  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(S3R_ATTN_PRODUCER_REGS));
-  if (warp == 0) {
-    if (lane == 0) {
-      mbar_arrive_expect_tx(q_full, Cfg<PAIR>::QB);
-#pragma unroll
-      for (int t = 0; t < (PAIR ? 2 : 1); ++t) {
-        tma_load_3d(sQ + t * Q_BYTES, &args.tmQ, q_full, 0, q0 + t * BQ, bh);
-        tma_load_3d(sQ + t * Q_BYTES + Q_BYTES / 2, &args.tmQ, q_full, 32, q0 + t * BQ, bh);
-      }
+    // register re-balancing: the TMA warpgroup needs few registers, each consumer thread holds S, P and O fragments
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (warp == 0 && lane == 0) {
+      mbar_arrive_expect_tx(q_full, Q_BYTES);
+      tma_load_3d(sQ, &args.tmQ, q_full, 0, q0, bh);
+      tma_load_3d(sQ + Q_BYTES / 2, &args.tmQ, q_full, 32, q0, bh);
       for (int j = 0; j < nblk; ++j) {
         const int st = j % KV_STAGES;
         const uint32_t ph = (j / KV_STAGES) & 1;
@@ -148,242 +86,137 @@ __global__ void __launch_bounds__(attn::kThreads, 1) attention_kernel(const __gr
         for (int a = 0; a < 4; ++a) tma_load_3d(v + a * (V_BYTES / 4), &args.tmV, &kv_full[st], j * BKV + a * 32, 0, bh);
       }
     }
-  } else if (warp == 1) {
-    // MMA issuer: the whole warp runs the uniform control flow, one elected lane issues, and the TMEM / smem bases go
-    // through a shuffle so the compiler can prove them uniform -- otherwise every tcgen05.mma sits in an
-    // ELECT / R2UR.BROADCAST / BRA.U.ANY waterfall loop (~80 cycles each, see gemm.cu).
-    {
-      constexpr uint32_t idesc_s = umma_idesc(kFmtTF32, BQ, BKV);
-      constexpr uint32_t idesc_o = umma_idesc(kFmtTF32, BQ, D);
-      const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem_base, 0);
-      const uint32_t aQ = __shfl_sync(0xffffffffu, smem_u32(sQ), 0);
-      const uint32_t aKV = __shfl_sync(0xffffffffu, smem_u32(sKV), 0);
-      // S_g = Q_g K_j^T into group g's S/P columns.  !PAIR: one query tile, g = j & 1.  PAIR: group g's own tile.
-      auto issue_s = [&](int g, int j) {
-        const int st = j % KV_STAGES;
-        mbar_wait(&kv_full[st], (j / KV_STAGES) & 1);
-        tc_fence_after_sync();
-        if (elect_one()) {
-          const uint32_t aK = aKV + st * (K_BYTES + V_BYTES);
-          const uint32_t aQg = aQ + (PAIR ? g * Q_BYTES : 0);
-          const uint32_t tmem_s = tmem_u + g * 192;
-#pragma unroll
-          for (int a = 0; a < 2; ++a) {
-            const uint64_t dq = umma_desc_sw128_kmajor(aQg + a * (Q_BYTES / 2));
-            const uint64_t dk = umma_desc_sw128_kmajor(aK + a * (K_BYTES / 2));
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk) umma_tf32(tmem_s, dq + 2 * kk, dk + 2 * kk, idesc_s, (a | kk) != 0);
-          }
-          umma_commit(&s_full[g]);
-        }
-        __syncwarp();
-      };
-      // O_g (+)= P_g V_j (P from TMEM); `first` = group g's first block; `release` frees the KV stage afterwards
-      auto issue_pv = [&](int g, int j, bool first, bool release, uint32_t p_parity) {
-        const int st = j % KV_STAGES;
-        mbar_wait(&p_full[g], p_parity);
-        tc_fence_after_sync();
-        if (elect_one()) {
-          const uint32_t aV = aKV + st * (K_BYTES + V_BYTES) + K_BYTES;
-          const uint32_t tmem_p = tmem_u + g * 192, tmem_o = tmem_p + 128;
-#pragma unroll
-          for (int a = 0; a < 4; ++a) {
-            const uint64_t dv = umma_desc_sw128_kmajor(aV + a * (V_BYTES / 4));
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk)
-              umma_tf32_ts(tmem_o, tmem_p + a * 32 + kk * 8, dv + 2 * kk, idesc_o, !first || (a | kk) != 0);
-          }
-          umma_commit(&o_full[g]);
-          if (release) umma_commit(&kv_empty[st]);
-        }
-        __syncwarp();
-      };
-      mbar_wait(q_full, 0);
-      if constexpr (!PAIR) {
-        issue_s(0, 0);
-        if (nblk > 1) issue_s(1, 1);
-        for (int j = 0; j < nblk; ++j) {
-          issue_pv(j & 1, j, j < 2, true, (j >> 1) & 1);
-          if (j + 2 < nblk) issue_s(j & 1, j + 2);   // same group's next block: its S/P columns are free once PV_j retires
-        }
-      } else {
-        issue_s(0, 0);
-        issue_s(1, 0);
-        for (int j = 0; j < nblk; ++j) {
-          issue_pv(0, j, j == 0, false, j & 1);
-          if (j + 1 < nblk) issue_s(0, j + 1);       // needs K_{j+1} (2-stage ring) and group 0's S/P columns (in-order pipe)
-          issue_pv(1, j, j == 0, true, j & 1);        // both groups' P.V of block j issued -> the stage can be refilled
-          if (j + 1 < nblk) issue_s(1, j + 1);
-        }
-      }
-    }
-  }
-  } else {
-    // ------------------------------------------------------------------ softmax groups, thread = query row
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 224;");
-    const int g = (warp - 4) >> 2;
-    const int quad = warp & 3;
-    const int r = quad * 32 + lane;
-    const uint32_t lane_sel = (uint32_t)(quad * 32) << 16;
-    const uint32_t ts = tmem_base + lane_sel + g * 192;     // S / P
-    const uint32_t to = ts + 128;                           // O
-    // Exact online softmax with a lazily updated reference (FA4-style): p = exp(s - ref), where ref only moves when
-    // a block's row max exceeds it by more than 8 (p <= e^8 stays far from overflow); l and the TMEM-resident O
-    // accumulator are rescaled in the same step, so the result is exact regardless of the threshold.
-    constexpr float kLog2e = 1.4426950408889634f;
-    float ref = -INFINITY, l = 0.f;
-    int it = 0;
-    for (int j = PAIR ? 0 : g; j < nblk; j += (PAIR ? 1 : 2), ++it) {   // PAIR: every block, for this group's own tile
-      mbar_wait(&s_full[g], it & 1);
-      tc_fence_after_sync();
-      const int kbase = j * BKV;
-      uint32_t s0[32], s1[32], s2[32], s3[32];   // the whole 128-key row of S: read from TMEM exactly once
-      tmem_ld_32x32(ts, s0);
-      tmem_ld_32x32(ts + 32, s1);
-      tmem_ld_32x32(ts + 64, s2);
-      tmem_ld_32x32(ts + 96, s3);
-      tmem_ld_wait();
-      if (kbase + BKV > args.nk) {   // ragged last block: keys beyond nk do not exist
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          if (kbase + i >= args.nk) s0[i] = 0xff800000u;
-          if (kbase + 32 + i >= args.nk) s1[i] = 0xff800000u;
-          if (kbase + 64 + i >= args.nk) s2[i] = 0xff800000u;
-          if (kbase + 96 + i >= args.nk) s3[i] = 0xff800000u;
-        }
-      }
-      float bmax = -INFINITY;
-#pragma unroll
-      for (int i = 0; i < 32; ++i) {
-        bmax = fmaxf(bmax, fmaxf(fmaxf(__uint_as_float(s0[i]), __uint_as_float(s1[i])),
-                                 fmaxf(__uint_as_float(s2[i]), __uint_as_float(s3[i]))));
-      }
-      if (it == 0) {
-        ref = bmax;
-      } else if (__any_sync(0xffffffffu, bmax > ref + 8.0f)) {   // rare: move the reference, rescale l and O
-        const float new_ref = (bmax > ref + 8.0f) ? bmax : ref;
-        const float alpha = exp2f((ref - new_ref) * kLog2e);
-        mbar_wait(&o_full[g], (it - 1) & 1);   // this group's previous P.V has retired
-        tc_fence_after_sync();
-#pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          uint32_t raw[32];
-          tmem_ld_32x32(to + c * 32, raw);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 32; ++i) raw[i] = __float_as_uint(__uint_as_float(raw[i]) * alpha);
-          tmem_st_32x32(to + c * 32, raw);
-        }
-        l *= alpha;
-        ref = new_ref;
-      }
-      const float nref2 = -ref * kLog2e;
-      float psum = 0.f;
-      auto expo = [&](uint32_t (&x)[32]) {
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          const float e = exp2f(fmaf(__uint_as_float(x[i]), kLog2e, nref2));   // exp(s - ref); exp(-inf) = 0
-          const uint32_t rb = (__float_as_uint(e) + 0x1000u) & 0xffffe000u;     // round to tf32 (the MMA truncates)
-          psum += __uint_as_float(rb);
-          x[i] = rb;
-        }
-      };
-      expo(s0); tmem_st_32x32(ts, s0);          // P overwrites S in place
-      expo(s1); tmem_st_32x32(ts + 32, s1);
-      expo(s2); tmem_st_32x32(ts + 64, s2);
-      expo(s3); tmem_st_32x32(ts + 96, s3);
-      tmem_st_wait();
-      l += psum;
-      tc_fence_before_sync();
-      mbar_arrive(&p_full[g]);
-    }
-    float m = ref;
-    float o[D];
-    if (it >= 1) {
-      mbar_wait(&o_full[g], (it - 1) & 1);
-      tc_fence_after_sync();
-#pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        uint32_t raw[32];
-        tmem_ld_32x32(to + c * 32, raw);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 32; ++i) o[c * 32 + i] = __uint_as_float(raw[i]);
-      }
-    } else {
-#pragma unroll
-      for (int i = 0; i < D; ++i) o[i] = 0.f;
-    }
-    named_bar_sync(1, 256);   // both groups have seen their last o_full: every MMA that reads the KV ring has retired
-    bool writer = true;
-    int qt0 = q0;                                      // first query row of the tile this thread's group writes
-    constexpr int LD = D + 4;
-    float* stg;
-    if constexpr (!PAIR) {
-      // ---- merge the two groups' partial results through shared memory (the KV ring is drained by now) ----
-      float* mg = reinterpret_cast<float*>(sKV);        // [66][128]: o[0..63], m, l  (column = query row)
-      if (g == 1) {
-#pragma unroll
-        for (int i = 0; i < D; ++i) mg[i * 128 + r] = o[i];
-        mg[64 * 128 + r] = m;
-        mg[65 * 128 + r] = l;
-      }
-      named_bar_sync(1, 256);
-      writer = (g == 0);
-      if (writer) {
-        const float m1 = mg[64 * 128 + r], l1 = mg[65 * 128 + r];
-        const float mm = fmaxf(m, m1);
-        const float w0 = __expf(m - mm), w1 = (l1 > 0.f) ? __expf(m1 - mm) : 0.f;
-        const float inv = 1.0f / (l * w0 + l1 * w1);
-#pragma unroll
-        for (int i = 0; i < D; ++i) o[i] = (o[i] * w0 + mg[i * 128 + r] * w1) * inv;
-      }
-      stg = reinterpret_cast<float*>(sKV + 40 * 1024) + quad * 32 * LD;   // behind the merge buffer
-    } else {
-      // each group owns a complete softmax over all keys for its tile: normalise and write
-      const float inv = 1.0f / l;
-#pragma unroll
-      for (int i = 0; i < D; ++i) o[i] *= inv;
-      qt0 = q0 + g * BQ;
-      stg = reinterpret_cast<float*>(sKV) + (g * 4 + quad) * 32 * LD;
-    }
-    if (writer) {
-      // Transposed store (see gemm_epilogue.cuh): thread = row would touch 32 different cache lines per 16-byte
-      // access; stage the warp's 32 x 64 tile in the drained KV ring and write it so that 16 consecutive lanes cover
-      // one row's 256 bytes.
-      {
-        float4* sp = reinterpret_cast<float4*>(stg + lane * LD);
-#pragma unroll
-        for (int i = 0; i < D / 4; ++i) sp[i] = make_float4(o[4 * i], o[4 * i + 1], o[4 * i + 2], o[4 * i + 3]);
-      }
-      __syncwarp();
-      const int b = bh / args.heads, h = bh - b * args.heads;
-      const int cq = (lane & 15) * 4;
-#pragma unroll 4
-      for (int it2 = 0; it2 < 16; ++it2) {
-        const int rr = it2 * 2 + (lane >> 4);
-        const int q = qt0 + quad * 32 + rr;
-        if (q < args.nq) {
-          const float4 x = *reinterpret_cast<const float4*>(stg + rr * LD + cq);
-          const long long off = ((long long)b * args.nq + q) * args.ldo + h * D + cq;
-          if (args.o_f32) *reinterpret_cast<float4*>(args.o_f32 + off) = x;
-          if (args.o_hi) {
-            uint32_t h0, l0, h1, l1;
-            split2_bf16(x.x, x.y, h0, l0);
-            split2_bf16(x.z, x.w, h1, l1);
-            *reinterpret_cast<uint2*>(args.o_hi + off) = make_uint2(h0, h1);
-            *reinterpret_cast<uint2*>(args.o_lo + off) = make_uint2(l0, l1);
-          }
-        }
-      }
-    }
+    return;
   }
 
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after_sync();
-    tmem_dealloc<attn::TMEM_COLS>(tmem_base);
+  // ------------------------------------------------------------------ consumers
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+  const int wg = (warp - 4) >> 2;        // rows [64 wg, 64 wg + 64) of the query tile
+  const int wq = warp & 3;               // this warp: rows 16 wq + g and 16 wq + g + 8 of them
+  const int g = lane >> 2, t4 = lane & 3;
+  const uint32_t aQ = __shfl_sync(0xffffffffu, smem_u32(sQ), 0) + wg * (64 * 128);
+  const uint32_t aKV = __shfl_sync(0xffffffffu, smem_u32(sKV), 0);
+  constexpr float kLog2e = 1.4426950408889634f;
+
+  float o[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;   // rows g and g + 8: running max, partial row sums
+  // P fragment sources: key 8kk + t4 of a row is column 2 (t4 / 2) + (t4 & 1) of lane 4g + t4 / 2, key 8kk + t4 + 4 the
+  // same column of lane 4g + 2 + t4 / 2
+  const int src_lo = (lane & ~3) | (t4 >> 1), src_hi = src_lo + 2;
+  const bool odd = (t4 & 1) != 0;
+
+  mbar_wait(q_full, 0);
+  for (int j = 0; j < nblk; ++j) {
+    const int st = j % KV_STAGES;
+    mbar_wait(&kv_full[st], (j / KV_STAGES) & 1);
+    const uint32_t aK = aKV + st * (K_BYTES + V_BYTES);
+    const uint32_t aV = aK + K_BYTES;
+
+    // S = Q K^T: 64 x 128 per warpgroup, 8 K-steps of 8 (two 32-wide swizzle atoms of the head dim)
+    float s[64];
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) {
+      const uint32_t part = (kk >> 2) * (Q_BYTES / 2), ko = (kk & 3) * 2;
+      wgmma_tf32_n128_ss(s, wgmma_desc_sw128_kmajor(aQ + part) + ko, wgmma_desc_sw128_kmajor(aK + part) + ko, kk > 0);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+
+    const int kbase = j * BKV;
+    if (kbase + BKV > args.nk) {   // ragged last block: keys beyond nk do not exist
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {
+        const int c = kbase + 8 * i + 2 * t4;
+        if (c >= args.nk) { s[4 * i] = -INFINITY; s[4 * i + 2] = -INFINITY; }
+        if (c + 1 >= args.nk) { s[4 * i + 1] = -INFINITY; s[4 * i + 3] = -INFINITY; }
+      }
+    }
+    float b0 = -INFINITY, b1 = -INFINITY;
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+      b0 = fmaxf(b0, fmaxf(s[4 * i], s[4 * i + 1]));
+      b1 = fmaxf(b1, fmaxf(s[4 * i + 2], s[4 * i + 3]));
+    }
+#pragma unroll
+    for (int x = 1; x < 4; x <<= 1) {
+      b0 = fmaxf(b0, __shfl_xor_sync(0xffffffffu, b0, x));
+      b1 = fmaxf(b1, __shfl_xor_sync(0xffffffffu, b1, x));
+    }
+    const float n0 = fmaxf(m0, b0), n1 = fmaxf(m1, b1);
+    const float al0 = (j == 0) ? 0.f : exp2f((m0 - n0) * kLog2e);
+    const float al1 = (j == 0) ? 0.f : exp2f((m1 - n1) * kLog2e);
+    m0 = n0;
+    m1 = n1;
+    const float nr0 = -n0 * kLog2e, nr1 = -n1 * kLog2e;
+    float ps0 = 0.f, ps1 = 0.f;
+#pragma unroll
+    for (int i = 0; i < 64; ++i) {
+      const bool r1 = (i & 2) != 0;
+      const float e = exp2f(fmaf(s[i], kLog2e, r1 ? nr1 : nr0));            // exp(s - max); exp(-inf) = 0
+      const uint32_t rb = (__float_as_uint(e) + 0x1000u) & 0xffffe000u;     // round to tf32 (the MMA truncates)
+      s[i] = __uint_as_float(rb);
+      if (r1) ps1 += s[i]; else ps0 += s[i];
+    }
+    l0 = l0 * al0 + ps0;
+    l1 = l1 * al1 + ps1;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      o[4 * i] *= al0; o[4 * i + 1] *= al0;
+      o[4 * i + 2] *= al1; o[4 * i + 3] *= al1;
+    }
+
+    // P (accumulator layout) -> tf32 A fragments: a0 (g, k), a1 (g+8, k), a2 (g, k+4), a3 (g+8, k+4), k = t4
+    uint32_t pa[16][4];
+#pragma unroll
+    for (int kk = 0; kk < 16; ++kk) {
+      const float x0 = __shfl_sync(0xffffffffu, s[4 * kk], src_lo), x1 = __shfl_sync(0xffffffffu, s[4 * kk + 1], src_lo);
+      const float y0 = __shfl_sync(0xffffffffu, s[4 * kk + 2], src_lo), y1 = __shfl_sync(0xffffffffu, s[4 * kk + 3], src_lo);
+      const float z0 = __shfl_sync(0xffffffffu, s[4 * kk], src_hi), z1 = __shfl_sync(0xffffffffu, s[4 * kk + 1], src_hi);
+      const float w0 = __shfl_sync(0xffffffffu, s[4 * kk + 2], src_hi), w1 = __shfl_sync(0xffffffffu, s[4 * kk + 3], src_hi);
+      pa[kk][0] = __float_as_uint(odd ? x1 : x0);
+      pa[kk][1] = __float_as_uint(odd ? y1 : y0);
+      pa[kk][2] = __float_as_uint(odd ? z1 : z0);
+      pa[kk][3] = __float_as_uint(odd ? w1 : w0);
+    }
+    // O += P V: 16 K-steps of 8 keys; V^T is stored as four 32-key swizzle atoms of [64 x 32 f32]
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 16; ++kk)
+      wgmma_tf32_n64_rs(o, pa[kk], wgmma_desc_sw128_kmajor(aV + (kk >> 2) * (V_BYTES / 4)) + (kk & 3) * 2, 1);
+    wgmma_commit();
+    wgmma_wait<0>();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&kv_empty[st]);   // this warp's reads of the stage have retired
+  }
+
+#pragma unroll
+  for (int x = 1; x < 4; x <<= 1) {
+    l0 += __shfl_xor_sync(0xffffffffu, l0, x);
+    l1 += __shfl_xor_sync(0xffffffffu, l1, x);
+  }
+  const float inv0 = 1.0f / l0, inv1 = 1.0f / l1;
+  const int b = bh / args.heads, h = bh - b * args.heads;
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int q = q0 + wg * 64 + wq * 16 + g + 8 * r;
+    if (q >= args.nq) continue;
+    const float inv = r ? inv1 : inv0;
+    const long long row = ((long long)b * args.nq + q) * args.ldo + h * D;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const float x = o[4 * i + 2 * r] * inv, y = o[4 * i + 2 * r + 1] * inv;
+      const long long off = row + 8 * i + 2 * t4;
+      if (args.o_f32) *reinterpret_cast<float2*>(args.o_f32 + off) = make_float2(x, y);
+      if (args.o_hi) {
+        uint32_t hh, ll;
+        split2_bf16(x, y, hh, ll);
+        *reinterpret_cast<uint32_t*>(args.o_hi + off) = hh;
+        *reinterpret_cast<uint32_t*>(args.o_lo + off) = ll;
+      }
+    }
   }
 }
 
@@ -418,29 +251,24 @@ int attn_plan_init(AttnPlan* plan, const float* q, const float* k, const float* 
     if (r) return r;
   }
   a.nq = nq; a.nk = nk; a.heads = heads;
-  // many-wave launches (the batched encoder: 960 CTAs on 148 SMs) take two query tiles per CTA
-  const int q_tiles = (nq + BQ - 1) / BQ;
-  const int pair_on = options().attn_pair;
-  plan->pair = (pair_on && q_tiles % 2 == 0 && (long long)q_tiles * BH >= 3 * 148) ? 1 : 0;
-  plan->grid = dim3(plan->pair ? q_tiles / 2 : q_tiles, BH);
+  plan->grid = dim3((nq + BQ - 1) / BQ, BH);
   plan->flops = 4.0 * BH * (double)nq * nk * 64;
   return 0;
 }
 
-template <bool PAIR>
-static int attn_launch_t(const AttnPlan& plan, const AttnArgs& a, cudaStream_t st) {
+static int attn_launch_args(const AttnPlan& plan, const AttnArgs& a, cudaStream_t st) {
   using namespace attn;
   static PerDeviceOnce once;
   bool& attr_set = once.cur();
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(attention_kernel<PAIR>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<PAIR>::SMEM);
+    cudaError_t e = cudaFuncSetAttribute(attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
     if (e != cudaSuccess) {
-      set_error("attention: cudaFuncSetAttribute(smem=%d): %s", Cfg<PAIR>::SMEM, cudaGetErrorString(e));
+      set_error("attention: cudaFuncSetAttribute(smem=%d): %s", SMEM, cudaGetErrorString(e));
       return -5;
     }
     attr_set = true;
   }
-  cudaError_t e = launch_pdl(attention_kernel<PAIR>, plan.grid, dim3(kThreads), Cfg<PAIR>::SMEM, st, a);
+  cudaError_t e = launch_pdl(attention_kernel, plan.grid, dim3(kThreads), SMEM, st, a);
   if (e != cudaSuccess) {
     set_error("attention launch failed: %s", cudaGetErrorString(e));
     return -6;
@@ -452,7 +280,7 @@ int attn_launch(const AttnPlan& plan, __nv_bfloat16* o_hi, __nv_bfloat16* o_lo, 
                 cudaStream_t st) {
   AttnArgs a = plan.args;
   a.o_hi = o_hi; a.o_lo = o_lo; a.o_f32 = o_f32; a.ldo = ldo;
-  return plan.pair ? attn_launch_t<true>(plan, a, st) : attn_launch_t<false>(plan, a, st);
+  return attn_launch_args(plan, a, st);
 }
 
 int launch_attention(const float* q, const float* k, const float* vt, int BH, int heads, int nq, int nk, int nk_pad,

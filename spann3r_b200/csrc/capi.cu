@@ -31,10 +31,11 @@ int s3r_device_ok(void) {
     cudaGetLastError();
     return 0;
   }
-  int dev = 0, major = 0;
+  int dev = 0, major = 0, minor = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
-  return major == 10 ? 1 : 0;
+  cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev);
+  return (major == 9 && minor == 0) ? 1 : 0;
 }
 
 int s3r_split(const float* x, int64_t ldx, void* hi, void* lo, int64_t ldp, int col0, int64_t rows, int c, int relu,
@@ -182,12 +183,8 @@ int s3r_conf_score(const float* conf, int64_t n, float* scratch256, float* out, 
 int s3r_set_option(const char* name, int value) {
   s3r::Options& o = s3r::options();
   if (!name) { set_error("s3r_set_option: null name"); return -1; }
-  if (!strcmp(name, "gemm2")) o.gemm2 = value;
-  else if (!strcmp(name, "gemm2_64")) o.gemm2_64 = value;
-  else if (!strcmp(name, "prefetch_b")) o.prefetch_b = value;
-  else if (!strcmp(name, "attn_pair")) o.attn_pair = value;
-  else if (!strcmp(name, "chain")) o.chain = value;
-  else { set_error("s3r_set_option: unknown option '%s' (gemm2, gemm2_64, prefetch_b, attn_pair, chain)", name); return -1; }
+  if (!strcmp(name, "prefetch_b")) o.prefetch_b = value;
+  else { set_error("s3r_set_option: unknown option '%s' (prefetch_b)", name); return -1; }
   return 0;
 }
 

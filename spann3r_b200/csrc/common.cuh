@@ -1,9 +1,9 @@
-// Shared device-side helpers for the sm_100a kernels: mbarrier, TMA, tcgen05/TMEM wrappers
+// Shared device-side helpers for the sm_90a kernels: mbarrier, TMA, wgmma shared-memory descriptors
 // and the split-bf16 ("bf16x3") number format used by every weight GEMM / conv on the path.
 //
 // Number format (DESIGN.md §3): an fp32 value x is carried as two bf16 planes
 //     hi = bf16_rn(x),  lo = bf16_rn(x - hi)          (hi + lo carries ~16 mantissa bits)
-// and a product a*b is issued as three tensor-core MMAs into one fp32 TMEM accumulator
+// and a product a*b is issued as three tensor-core MMAs into one fp32 register accumulator
 //     a_hi*b_hi + a_hi*b_lo + a_lo*b_hi              (the lo*lo term, 2^-16 relative, is dropped)
 // which is what keeps the path inside the 1e-3 fp32 parity bar (SURVEY.md §7.3-#1).
 #pragma once
@@ -112,13 +112,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
-__device__ __forceinline__ void tc_fence_before_sync() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after_sync() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-
 // ----------------------------------------------------------------------------------------------
 // TMA (cp.async.bulk.tensor) loads, completion on an mbarrier
 // ----------------------------------------------------------------------------------------------
@@ -170,93 +163,29 @@ __device__ __forceinline__ void tma_load_4d_u(uint32_t smem, const CUtensorMap* 
 }
 
 // ----------------------------------------------------------------------------------------------
-// TMEM allocation (one warp, power-of-two columns >= 32)
-// ----------------------------------------------------------------------------------------------
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst) {
-  static_assert(kCols == 32 || kCols == 64 || kCols == 128 || kCols == 256 || kCols == 512, "tmem cols");
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-
-// ----------------------------------------------------------------------------------------------
-// UMMA descriptors.  Shared-memory matrix descriptor for a K-major tile whose rows are exactly one
-// 128-byte swizzle span (64 bf16 or 32 tf32) and which is stored as TMA SWIZZLE_128B wrote it:
+// wgmma shared-memory matrix descriptor for a K-major tile whose rows are exactly one 128-byte
+// swizzle span (64 bf16 or 32 tf32) and which is stored as TMA SWIZZLE_128B wrote it:
 //   start_address  = addr >> 4                       bits [0,14)
 //   leading offset = 1 (ignored for swizzled K-major) bits [16,30)
 //   stride offset  = 1024 B >> 4 = 64 (8-row group)   bits [32,46)
-//   version        = 1 (Blackwell)                    bits [46,48)
-//   layout type    = 2 (SWIZZLE_128B)                 bits [61,64)
-// Stepping along K inside the 128-byte span = adding (bytes >> 4) to the start address.
+//   layout type    = 1 (SWIZZLE_128B)                 bits [62,64)
+// Tiles start on 1024-byte boundaries (base offset 0).  Stepping along K inside the 128-byte span = adding
+// (bytes >> 4) to the start address; stepping 64 rows = adding 8 KB.
 // ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint64_t umma_desc_sw128_kmajor(uint32_t smem_addr) {
+__device__ __forceinline__ uint64_t wgmma_desc_sw128_kmajor(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
   d |= (uint64_t)1 << 16;
   d |= (uint64_t)64 << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
-// Instruction descriptor (upper 32 bits of idescE): fp32 accumulate, K-major A and B, dense.
-//   c_format [4,6)=1 (F32)  a_format [7,10)  b_format [10,13)  (0=F16 1=BF16 2=TF32)
-//   n_dim [17,23) = N>>3    m_dim [24,29) = M>>4
-__host__ __device__ constexpr uint32_t umma_idesc(uint32_t fmt, uint32_t M, uint32_t N) {
-  return (1u << 4) | (fmt << 7) | (fmt << 10) | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-constexpr uint32_t kFmtBF16 = 1, kFmtTF32 = 2;
-
-// D[tmem] (+)= A[smem] * B[smem]^T ; issued by ONE thread.
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// all previously issued MMAs of this thread -> arrive(1) on the mbarrier when they complete
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-
-// TMEM -> registers: this warp's 32 lanes x 32 consecutive fp32 columns (thread i = lane i = tile row)
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 // ----------------------------------------------------------------------------------------------
 // Programmatic dependent launch (PDL): every kernel of the library is launched with
 // cudaLaunchAttributeProgrammaticStreamSerialization, signals its dependents at once and waits for
 // its prerequisite grid right before touching global memory, so the launch latency, CTA scheduling,
-// barrier init, TMEM allocation and tensor-map prefetch of kernel i+1 overlap the tail of kernel i.
+// barrier init and tensor-map prefetch of kernel i+1 overlap the tail of kernel i.
 // ----------------------------------------------------------------------------------------------
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }

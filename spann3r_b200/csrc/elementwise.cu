@@ -1,4 +1,4 @@
-// Bandwidth-bound helper kernels of the Spann3R forward path (sm_100a): LayerNorm with split-bf16
+// Bandwidth-bound helper kernels of the Spann3R forward path (sm_90a): LayerNorm with split-bf16
 // re-encode, fp32 -> split-bf16, patch im2col, stride-2 im2col, bilinear x2 upsample (align_corners),
 // and the curope-compatible in-place RoPE shim.  All are plain coalesced / 128-bit vectorised
 // CUDA-core kernels: the data they touch (<= a few MB per call, except the DPT upsamples) lives in
@@ -41,7 +41,7 @@ int launch_split(const float* x, long long ldx, __nv_bfloat16* hi, __nv_bfloat16
   const long long total = rows * (C / 4);
   if (total == 0) return 0;
   int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   launch_pdl(split_kernel, dim3(blocks), dim3(256), 0, st, x, ldx, hi, lo, ldp, col0, rows, C, relu);
   return cudaGetLastError() == cudaSuccess ? 0 : -6;
 }
@@ -179,7 +179,7 @@ int launch_im2col_patch16(const float* img, long long sb, long long sc, long lon
   const long long total = (long long)B * gh * gw * 48;
   if (total == 0) return 0;
   int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   launch_pdl(im2col_patch16_kernel, dim3(blocks), dim3(256), 0, st, img, sb, sc, sy, sx, B, gh, gw, hi, lo);
   return cudaGetLastError() == cudaSuccess ? 0 : -6;
 }
@@ -222,7 +222,7 @@ int launch_im2col_3x3s2(const __nv_bfloat16* ihi, const __nv_bfloat16* ilo, int 
   const long long total = (long long)NB * Ho * Wo * 9 * (C / 8);
   if (total == 0) return 0;
   int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   launch_pdl(im2col_3x3s2_kernel, dim3(blocks), dim3(256), 0, st, ihi, ilo, NB, H, W, C, Ho, Wo, ohi, olo);
   return cudaGetLastError() == cudaSuccess ? 0 : -6;
 }
@@ -344,7 +344,7 @@ int launch_rope2d(float* tokens, const long long* pos, long long BN, int H, int 
   const long long total = BN * H * (D / 2);
   if (total == 0) return 0;
   long long blocks = (total + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   launch_pdl(rope2d_kernel, dim3((int)blocks), dim3(256), 0, st, tokens, pos, BN, H, D, stride_tok, stride_head, base, fwd);
   return cudaGetLastError() == cudaSuccess ? 0 : -6;
 }

@@ -1,4 +1,4 @@
-// Model-level runtime of libspann3r_b200.so: sequences the sm_100a kernels of one frame step of
+// Model-level runtime of libspann3r_b200.so: sequences the sm_90a kernels of one frame step of
 // Spann3R.forward (spann3r/model.py:473-539) -- encoder, twin decoder, key heads, DPT heads, value
 // encoder, spatial-memory read / append -- over an engine-owned activation workspace, with every
 // tensor-map / tile plan built once per shape and replayed (no per-call descriptor encoding, no host
@@ -60,18 +60,13 @@ struct Epi {
 struct PlanCache {
   std::vector<GemmPlan> gemms;
   std::vector<AttnPlan> attns;
-  std::vector<ChainPlan> chains;   // runs of consecutive GEMM plans launched as ONE persistent kernel (gemm_chain.cu)
-  size_t gc = 0, ac = 0, cc = 0;
+  size_t gc = 0, ac = 0;
   bool building = true;
-  bool chain_open = false, use_chain = false;
-  size_t chain_first = 0;
   void begin() {
-    gc = ac = cc = 0;
-    chain_open = false;
+    gc = ac = 0;
     if (building) {   // a previous first pass failed half way (e.g. a plan_init error): start the plan list over
       gemms.clear();
       attns.clear();
-      chains.clear();
     }
   }
   void end() { building = false; }
@@ -161,14 +156,6 @@ struct s3r_engine {
       int r = gemm_plan_init(&pc.gemms.back(), A.hi, A.lo, Bw.hi, Bw.lo, g.groups, g.NB, g.H, g.W, g.Kc, g.taps, g.N,
                              e.epi == EPI_HEADTAIL ? 1128 : g.force_bn, g.lda, g.ldb, g.b_group_rows);
       if (r) return r;
-      const GemmArgs& pa = pc.gemms.back().args;
-      const bool even_rows = ((pa.tiles_w * pa.tiles_h * pa.NB) & 1) == 0;   // CTA pairs need an even number of 128-row tiles
-      if (pc.chain_open && !pc.gemms.back().two_cta && even_rows) {   // every phase of a chain runs on CTA pairs
-        const int bn = pc.gemms.back().bn;
-        r = gemm_plan_init(&pc.gemms.back(), A.hi, A.lo, Bw.hi, Bw.lo, g.groups, g.NB, g.H, g.W, g.Kc, g.taps, g.N, 2000 + bn,
-                           g.lda, g.ldb, g.b_group_rows);
-        if (r) return r;
-      }
       pc.gemms.back().b_static = (g.b_static && options().prefetch_b) ? 1 : 0;   // decided when the plan is built
     }
     if (pc.gc >= pc.gemms.size()) {
@@ -196,81 +183,11 @@ struct s3r_engine {
     a.stats_out = e.stats_out;
     a.b_static = p.b_static;
     flops += p.flops;
-    if (pc.chain_open) return 0;   // launched by chain_end() together with the other phases
     ++launches;
     if (!profiling) return gemm_launch(p, st);
     Timed t; t.a = get_event(); t.b = get_event(); t.flops = p.flops; t.kind = 0;
     cudaEventRecord(t.a, st);
     int r = gemm_launch(p, st);
-    cudaEventRecord(t.b, st);
-    timed.push_back(t);
-    return r;
-  }
-
-  // The GEMM calls between chain_begin() and chain_end() are dependent linear layers on the same rows (phase p+1 consumes
-  // what phase p writes): they become ONE persistent launch with per-row-block dependency counters (gemm_chain.cu).
-  void chain_begin(PlanCache& pc) {
-    if (pc.building) pc.use_chain = options().chain != 0;   // decided when the plans are built, replayed as built
-    if (!pc.use_chain) return;
-    pc.chain_open = true;
-    pc.chain_first = pc.gc;
-  }
-  int chain_end(PlanCache& pc, cudaStream_t st) {
-    if (!pc.chain_open) return 0;
-    pc.chain_open = false;
-    const int n = (int)(pc.gc - pc.chain_first);
-    if (n == 0) return 0;
-    if (pc.building) {
-      const GemmPlan* items[kChainMaxPhases] = {};
-      if (n > kChainMaxPhases) {
-        set_error("engine: chain of %d phases", n);
-        return -8;
-      }
-      bool pairs = true;
-      for (int i = 0; i < n; ++i) {
-        items[i] = &pc.gemms[pc.chain_first + i];
-        pairs = pairs && items[i]->two_cta;
-      }
-      pc.chains.emplace_back();
-      if (pairs) {
-        const int cap = 1 + n * items[0]->args.groups * items[0]->args.tiles_w * items[0]->args.tiles_h * items[0]->args.NB;
-        uint32_t* dct = alloc<uint32_t>(cap);
-        if (status) return status;
-        int r = chain_plan_init(&pc.chains.back(), items, n, dct, cap);
-        if (r) return r;
-      } else {   // an odd number of 128-row tiles (e.g. 4 x 196 tokens): no CTA pairs, the run goes out as separate launches
-        memset(&pc.chains.back(), 0, sizeof(ChainPlan));
-        pc.chains.back().first = (int)pc.chain_first;
-        pc.chains.back().count = n;
-      }
-    }
-    if (pc.cc >= pc.chains.size()) {
-      set_error("engine: chain plan cache out of sync");
-      return -8;
-    }
-    const ChainPlan& cp = pc.chains[pc.cc++];
-    if (cp.count > 0) {
-      for (int i = 0; i < cp.count; ++i) {
-        const GemmPlan& p = pc.gemms[cp.first + i];
-        ++launches;
-        if (!profiling) {
-          if (int r = gemm_launch(p, st)) return r;
-          continue;
-        }
-        Timed t; t.a = get_event(); t.b = get_event(); t.flops = p.flops; t.kind = 0;
-        cudaEventRecord(t.a, st);
-        int r = gemm_launch(p, st);
-        cudaEventRecord(t.b, st);
-        timed.push_back(t);
-        if (r) return r;
-      }
-      return 0;
-    }
-    ++launches;
-    if (!profiling) return chain_launch(cp, st);
-    Timed t; t.a = get_event(); t.b = get_event(); t.flops = cp.flops; t.kind = 0;
-    cudaEventRecord(t.a, st);
-    int r = chain_launch(cp, st);
     cudaEventRecord(t.b, st);
     timed.push_back(t);
     return r;
@@ -309,8 +226,7 @@ struct s3r_engine {
   // ---- ViT blocks on X [nimg*N, D] (in place).  croco/models/blocks.py:127-130 ----
   // LayerNorms are folded into the GEMM that consumes them (s3r_lin.cs): P holds the planes of the block input x and St1
   // its per-row chunk statistics (written by whichever GEMM produced x).  No LayerNorm kernel runs inside a block.
-  // Launch structure per block: [qkv of block 0] then, per block, attention + ONE chain launch (proj -> fc1 -> fc2 -> the
-  // NEXT block's qkv); without the chain option the same GEMMs go out one by one.
+  // Launch structure per block: [qkv of block 0] then, per block, attention, proj, fc1, fc2 and the NEXT block's qkv.
   int vit_qkv(PlanCache& pc, const s3r_block_w& bw, int D, int nimg, bool rope, cudaStream_t st, const int* pos_tab) {
     const int rows = nimg * N;
     Geom g; g.W = rows; g.Kc = D; g.N = 3 * D;
@@ -329,7 +245,6 @@ struct s3r_engine {
     for (int l = 0; l < depth; ++l) {
       const s3r_block_w& bw = blocks[l];
       if ((r = attention(pc, Qb, Kb, Vtb, nimg * heads, heads, N, N, AO, D, st))) return r;
-      chain_begin(pc);
       {
         Geom g; g.W = rows; g.Kc = D; g.N = D;
         Epi e; e.bias = bw.proj.b; e.res1 = Xp; e.ldr1 = D; e.out = Xp; e.ldo = D;
@@ -349,7 +264,6 @@ struct s3r_engine {
         if ((r = gemm(pc, Hb, WP(bw.fc2.w), g, e, st))) return r;
       }
       if (l + 1 < depth && (r = vit_qkv(pc, blocks[l + 1], D, nimg, rope, st, pos_tab))) return r;
-      if ((r = chain_end(pc, st))) return r;
     }
     return 0;
   }
@@ -626,8 +540,8 @@ int s3r_engine_decode(s3r_engine* e, const float* f1, const float* f2, float* de
   // of the layer input (both streams), Sa its chunk statistics: read by qkv (norm1) and -- with the groups swapped,
   // each stream cross-attends to the OTHER stream's layer input -- by kv (norm_y).  Pb / Sb: x after self attention
   // (norm2 -> q), Pc / Sc: x after cross attention (norm3 -> fc1).  fc2 writes the next layer's xin / Sa.
-  // Launch structure: [qkv of layer 0], then per layer: self attention, chain (proj -> q), cross attention, chain (cproj ->
-  // fc1 -> fc2 -> the NEXT layer's qkv): 4 launches per layer instead of 9 (the same GEMMs one by one without the chain option).
+  // Launch structure: [qkv of layer 0], then per layer: self attention, proj, q, cross attention, cproj, fc1, fc2 and the
+  // NEXT layer's qkv.
   auto qkv_launch = [&](int l, Planes xin) {
     // self-attention q, k, v (norm1 folded) and -- same launch, columns >= 2304 reading the OTHER stream's layer
     // input (norm_y folded, group swap) -- the cross-attention k, v
@@ -644,7 +558,6 @@ int s3r_engine_decode(s3r_engine* e, const float* f1, const float* f2, float* de
   for (int l = 0; l < 12; ++l) {
     const s3r_decblock_w& bw = e->w.dec[l];
     if ((r = e->attention(pc, e->Qd, e->Kd, e->Vtd, 2 * B * 12, 12, N, N, e->AOd, 768, st))) return r;
-    e->chain_begin(pc);
     {
       Geom g; g.groups = 2; g.W = (int)R; g.Kc = 768; g.N = 768;
       Epi ep; ep.bias = bw.proj.b; ep.res1 = e->Xd; ep.ldr1 = 768; ep.out = e->Xd; ep.ldo = 768;
@@ -660,9 +573,7 @@ int s3r_engine_decode(s3r_engine* e, const float* f1, const float* f2, float* de
       ep.ln_stats = e->Sb; ep.ln_np = 24; ep.ln_eps = 1e-6f; ep.ln_cs = bw.q.cs;                        // norm2
       if ((r = e->gemm(pc, e->Pb, WP(bw.q.w), g, ep, st))) return r;
     }
-    if ((r = e->chain_end(pc, st))) return r;
     if ((r = e->attention(pc, e->Qd, e->Kd2, e->Vtd2, 2 * B * 12, 12, N, N, e->AOd, 768, st))) return r;
-    e->chain_begin(pc);
     {
       Geom g; g.groups = 2; g.W = (int)R; g.Kc = 768; g.N = 768;
       Epi ep; ep.bias = bw.cproj.b; ep.res1 = e->Xd; ep.ldr1 = 768; ep.out = e->Xd; ep.ldo = 768;
@@ -687,7 +598,6 @@ int s3r_engine_decode(s3r_engine* e, const float* f1, const float* f2, float* de
       xin = xout;
     }
     if (l < 11 && (r = qkv_launch(l + 1, xin))) return r;
-    if ((r = e->chain_end(pc, st))) return r;
     if (dec_all && l < 11) {
       ++e->launches;
       cudaMemcpyAsync(dec_all + (size_t)l * 2 * R * 768, e->Xd, (size_t)2 * R * 768 * sizeof(float),

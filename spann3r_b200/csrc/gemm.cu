@@ -1,4 +1,4 @@
-// Split-bf16 ("bf16x3") GEMM / implicit-GEMM 3x3 convolution on tcgen05 tensor cores, sm_100a.
+// Split-bf16 ("bf16x3") GEMM / implicit-GEMM 3x3 convolution on Hopper wgmma tensor cores, sm_90a.
 //
 //   D[pixel, n] = sum_{tap, k} A[pixel shifted by tap, k] * Wt[n, tap, k]      (fp32 result)
 //
@@ -7,17 +7,17 @@
 // (dust3r/patch_embed.py:19-29, after an im2col kernel), and every Conv2d / ConvTranspose2d of the
 // DPT head (croco/models/dpt_block.py:33-75,121-142,189-218,318-324,356-410).
 //
-// Structure: persistent, warp-specialised, one CTA per SM.
-//   warp 0      TMA producer: per k-block four SWIZZLE_128B boxes (A_hi, A_lo: 128 pixels x 64 ch;
-//               B_hi, B_lo: BN x 64) into a STAGES-deep smem ring; a 3x3 conv is 9 taps whose A box is
-//               the same 4-D tensor map at (w+dx, h+dy) -- out-of-bounds pixels are zero-filled by TMA,
-//               which is exactly the conv's zero padding.
-//   warp 1      MMA issuer (one thread): per k-block 4 K-steps x 3 MMAs (hi*lo, lo*hi, hi*hi) into a
-//               128 x BN fp32 accumulator in TMEM; two accumulator stages so the epilogue of tile i
-//               overlaps the main loop of tile i+1.
-//   warps 2..5  epilogue: tcgen05.ld 32 columns at a time (thread = tile row), fused bias / GELU / ReLU /
-//               residual adds / split-bf16 re-encode for the next GEMM / RoPE + head split for attention /
-//               ConvTranspose pixel shuffle / DPT head tail + postprocess.
+// Structure: persistent, warp-specialised, one CTA per SM, 128 x BN output tiles.
+//   warpgroup 0   TMA producer (one warp; registers handed to the consumers with setmaxnreg): per k-block four
+//                 SWIZZLE_128B boxes (A_hi, A_lo: 128 pixels x 64 ch; B_hi, B_lo: BN x 64) into a STAGES-deep smem
+//                 ring; a 3x3 conv is 9 taps whose A box is the same 4-D tensor map at (w+dx, h+dy) -- out-of-bounds
+//                 pixels are zero-filled by TMA, which is exactly the conv's zero padding.
+//   warpgroups 1, 2  consumers: each owns 64 rows of the tile and issues per k-block 4 K-steps x 3 wgmma (hi*lo,
+//                 lo*hi, hi*hi) into a 64 x BN fp32 register accumulator, one k-block in flight.  The epilogue is run
+//                 by the same 8 warps: the accumulator goes through shared memory 2 x 32 columns at a time into the
+//                 thread = tile row layout of gemm_epilogue.cuh (fused bias / GELU / ReLU / residual adds / split-bf16
+//                 re-encode / RoPE + head split / ConvTranspose pixel shuffle / DPT head tail + postprocess).  The
+//                 producer keeps filling the ring for the next tile meanwhile.
 #include "gemm.cuh"
 
 #include <cmath>
@@ -27,29 +27,37 @@
 
 #include "common.cuh"
 #include "gemm_epilogue.cuh"
+#include "wgmma.cuh"
 
 namespace s3r {
 
 static constexpr int BM = 128;
 static constexpr int BK = 64;
-static constexpr int kEpiWarps = 8;     // 2 per SM sub-partition: the epilogue is a chain of dependent instructions, a second
-                                        // warp per scheduler hides its latencies (tools/trace_gemm.py)
-static constexpr int kNumThreads = 64 + 32 * kEpiWarps;
-static constexpr int kSmemRing = 192 * 1024;
+static constexpr int kEpiWarps = 8;     // the two consumer warpgroups
+static constexpr int kNumThreads = 128 + 32 * kEpiWarps;
+static constexpr int kSmemMax = 227 * 1024;
+static constexpr int kAccLD = 36;       // accumulator staging row stride (floats): 16-byte rows, conflict-free row reads
+static constexpr int kAccBytes = 2 * BM * kAccLD * 4;   // two 32-column chunks (one per column half) of all 128 rows
 
 template <int BN>
 struct GemmCfg {
   static constexpr int A_TILE = BM * BK * 2;  // bytes, one plane
   static constexpr int B_TILE = BN * BK * 2;
   static constexpr int STAGE = 2 * A_TILE + 2 * B_TILE;
-  static constexpr int STAGES = kSmemRing / STAGE;
-  static constexpr int COLV = 2 * 2 * BN * 4;  // per accumulator stage: staged bias + LN-fold column sums of the tile
-  static constexpr int SW = 16;                // epilogue staging width (gemm_epilogue.cuh)
-  static constexpr int STG = kEpiWarps * Stg<SW>::WARP_BYTES;
-  static constexpr int SMEM = STAGES * STAGE + 1024 /*align slack*/ + 256 /*barriers*/ + COLV + STG;
-  static constexpr uint32_t TMEM_COLS = 2 * BN;  // two accumulator stages
+  static constexpr int COLV = 2 * 2 * BN * 4;  // per tile parity: staged bias + LN-fold column sums of the tile
+  static constexpr int HT = 4 * 2 * 32 * 16;   // EPI_HEADTAIL hand-over slots (per lane quadrant, two tile parities)
+  static constexpr int FIXED = 1024 /*align slack*/ + 256 /*barriers*/ + kAccBytes + COLV + HT;
+  static constexpr int STAGES = (kSmemMax - FIXED) / STAGE;
+  static constexpr int SMEM = STAGES * STAGE + FIXED;
+  static_assert(STAGES >= 2, "smem ring");
+  static_assert(Stg<32>::WARP_BYTES == 32 * kAccLD * 4, "a warp's staging tile is its own rows of the accumulator chunk");
 };
 
+template <int BN>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[BN / 2], uint64_t da, uint64_t db, int scale_d) {
+  if constexpr (BN == 64) wgmma_bf16_n64(d, da, db, scale_d);
+  else wgmma_bf16_n128(d, da, db, scale_d);
+}
 
 template <int BN, int EPI>
 __global__ void __launch_bounds__(kNumThreads, 1) gemm_bf16x3_kernel(const __grid_constant__ GemmArgs args) {
@@ -61,10 +69,9 @@ __global__ void __launch_bounds__(kNumThreads, 1) gemm_bf16x3_kernel(const __gri
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + Cfg::STAGES;
-  uint64_t* tmem_full = bars + 2 * Cfg::STAGES;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-  float* colv = reinterpret_cast<float*>(smem + Cfg::STAGES * Cfg::STAGE + 256);   // [2 stages][bias | colsum][BN]
+  float* sacc = reinterpret_cast<float*>(smem + Cfg::STAGES * Cfg::STAGE + 256);   // [2][BM][kAccLD]
+  float* colv = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(sacc) + kAccBytes);   // [2 parities][bias | colsum][BN]
+  float4* hts = reinterpret_cast<float4*>(reinterpret_cast<uint8_t*>(colv) + Cfg::COLV);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -84,19 +91,11 @@ __global__ void __launch_bounds__(kNumThreads, 1) gemm_bf16x3_kernel(const __gri
     tma_prefetch_desc(&args.tmB_lo);
     for (int i = 0; i < Cfg::STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], kEpiWarps);
+      mbar_init(&empty_bar[i], kEpiWarps);
     }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<Cfg::TMEM_COLS>(tmem_ptr_smem);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_ptr_smem;
   pdl_launch_dependents();
   if (trace && threadIdx.x == 0) trace[1] = globaltimer_ns();
   // Weights do not depend on the previous kernel: the producer stages the B tiles of the first ring pass of this CTA's first
@@ -123,11 +122,11 @@ __global__ void __launch_bounds__(kNumThreads, 1) gemm_bf16x3_kernel(const __gri
   pdl_wait();  // everything above overlapped the previous kernel's tail; activations are touched only below
   if (trace && threadIdx.x == 0) trace[2] = globaltimer_ns();
 
-  if (warp == 0) {
-    // ------------------------------------------------------------------ TMA producer
-    // whole warp in uniform control flow, one elected lane issues (same reason as the MMA warp below: no
-    // per-instruction ELECT / R2UR waterfall); tap / channel coordinates advance incrementally, no div / mod per k-block
-    {
+  if (warp < 4) {
+    // ------------------------------------------------------------------ TMA producer (warp 0; warps 1..3 idle)
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (warp == 0) {
+      // whole warp in uniform control flow, one elected lane issues; tap / channel coordinates advance incrementally
       const uint32_t smem_u = __shfl_sync(0xffffffffu, smem_u32(smem), 0);
       const uint32_t full_u = __shfl_sync(0xffffffffu, smem_u32(full_bar), 0);
       int stage = 0;
@@ -175,67 +174,20 @@ __global__ void __launch_bounds__(kNumThreads, 1) gemm_bf16x3_kernel(const __gri
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    // The WHOLE warp runs the (warp-uniform) control flow and one elected lane issues; the TMEM / smem base
-    // addresses go through a shuffle so that the compiler can prove them uniform.  With a plain `if (lane == 0)` and a
-    // TMEM address loaded from shared memory ptxas wraps every tcgen05.mma in an ELECT / R2UR.BROADCAST / BRA.U.ANY
-    // waterfall loop that costs ~80 cycles per MMA -- more than a 128 x 64 or 128 x 128 MMA takes to execute
-    // (tools/fill_probe.py: 517 ns per k-block whatever the tile width); now the 12 MMAs of a k-block are
-    // back-to-back UTCHMMA instructions.
-    {
-      constexpr uint32_t idesc = umma_idesc(kFmtBF16, BM, BN);
-      const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem_base, 0);
-      const uint32_t smem_u = __shfl_sync(0xffffffffu, smem_u32(smem), 0);
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-        const int as = it & 1;
-        const uint32_t aphase = (it >> 1) & 1;
-        mbar_wait(&tmem_empty[as], aphase ^ 1);
-        tc_fence_after_sync();
-        const uint32_t tmem_d = tmem_u + as * BN;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after_sync();
-          if (trace && kb == 0 && it == 0 && lane == 0) trace[3] = globaltimer_ns();
-          if (elect_one()) {
-            const uint32_t sa = smem_u + stage * Cfg::STAGE;
-            const uint64_t da_hi = umma_desc_sw128_kmajor(sa);
-            const uint64_t da_lo = umma_desc_sw128_kmajor(sa + Cfg::A_TILE);
-            const uint64_t db_hi = umma_desc_sw128_kmajor(sa + 2 * Cfg::A_TILE);
-            const uint64_t db_lo = umma_desc_sw128_kmajor(sa + 2 * Cfg::A_TILE + Cfg::B_TILE);
-#pragma unroll
-            for (int kk = 0; kk < BK / 16; ++kk) {
-              const uint64_t ko = (uint64_t)(kk * 32 >> 4);  // 16 bf16 = 32 bytes along K inside the swizzle span
-              umma_bf16(tmem_d, da_hi + ko, db_lo + ko, idesc, (kb | kk) != 0);
-              umma_bf16(tmem_d, da_lo + ko, db_hi + ko, idesc, 1);
-              umma_bf16(tmem_d, da_hi + ko, db_hi + ko, idesc, 1);
-            }
-            umma_commit(&empty_bar[stage]);  // frees the smem slot when these MMAs retire
-          }
-          __syncwarp();
-          if (++stage == Cfg::STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        if (elect_one()) umma_commit(&tmem_full[as]);
-        __syncwarp();
-        if (trace && it == 0 && lane == 0) trace[7] = globaltimer_ns();
-      }
-    }
   } else {
-    // ------------------------------------------------------------------ epilogue (warps 2..9): TMEM lane quadrant
-    // warp & 3, column half (warp - 2) >> 2
-    const int quad = warp & 3;  // TMEM lane quadrant this warp may access
-    const int half = (warp - 2) >> 2;
-    constexpr int CH = BN / 64;  // 32-column chunks per warp
+    // ------------------------------------------------------------------ consumers: MMA, then epilogue
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    const int cw = warp - 4;            // consumer warp 0..7
+    const int wg = cw >> 2;             // MMA: warpgroup wg owns tile rows [64 wg, 64 wg + 64)
+    const int wq = cw & 3;              //      and this warp rows 16 wq + (lane / 4) (+8) of them
+    const int quad = cw & 3;            // epilogue: thread = tile row quad * 32 + lane ...
+    const int half = cw >> 2;           // ... of column half `half`
+    constexpr int CH = BN / 64;         // 32-column chunks per half
+    const uint32_t smem_u = __shfl_sync(0xffffffffu, smem_u32(smem), 0);
+    int stage = 0;
+    uint32_t phase = 0;
     int it = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-      const int as = it & 1;
-      const uint32_t aphase = (it >> 1) & 1;
       const int g = tile / tiles_per_group;
       const int rem = tile - g * tiles_per_group;
       const int mt = rem / n_tiles;
@@ -244,59 +196,104 @@ __global__ void __launch_bounds__(kNumThreads, 1) gemm_bf16x3_kernel(const __gri
       const int th = (mt / args.tiles_w) % args.tiles_h;
       const int nb = mt / (args.tiles_w * args.tiles_h);
 
-      // everything that does not need the accumulator is requested while the main loop of this tile still runs:
-      // the tile's bias / colsum columns (-> smem), the rows' LayerNorm statistics, RoPE positions and output
-      // addresses, and the residual values of the first chunk
-      constexpr int SW = Cfg::SW;
-      float* sb = colv + as * 2 * BN;
+      // everything that does not need the accumulator is requested before the main loop: the tile's bias / colsum
+      // columns (-> smem), the rows' LayerNorm statistics, RoPE positions and output addresses, and the residual values
+      // of the first chunk
+      float* sb = colv + (it & 1) * 2 * BN;
       float* scs = sb + BN;
-      float* stg = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(colv) + Cfg::COLV + (warp - 2) * Stg<SW>::WARP_BYTES);
-      epi_stage_cols<EPI, BN>(args, sb, scs, g, nt, (int)threadIdx.x - 64, 32 * kEpiWarps);
+      epi_stage_cols<EPI, BN>(args, sb, scs, g, nt, (int)threadIdx.x - 128, 32 * kEpiWarps);
       const TileGeom tg = make_geom(args, g, nb, th, tw, nt * BN);
       EpiRow er;
       EpiTRows tr;
-      epi_tile_pre<EPI, SW>(args, tg, quad, lane, er, tr);
+      epi_tile_pre<EPI, 32>(args, tg, quad, lane, er, tr);
       float4 rcur[8], rnxt[8];
       const int cfirst = nt * BN + half * CH * 32;
-      if (cfirst < args.N) epi_prefetch_res<EPI, SW>(args, tr, rcur, cfirst, lane);
-      asm volatile("bar.sync 1, %0;" ::"n"(32 * kEpiWarps) : "memory");   // staged columns visible to all epilogue warps
+      if (cfirst < args.N) epi_prefetch_res<EPI, 32>(args, tr, rcur, cfirst, lane);
+      // staged columns visible to all consumer warps; every warp is also done with the previous tile's staging buffer
+      asm volatile("bar.sync 1, %0;" ::"n"(32 * kEpiWarps) : "memory");
 
-      mbar_wait(&tmem_full[as], aphase);
-      tc_fence_after_sync();
-      if (trace && it == 0 && threadIdx.x == 64) trace[4] = globaltimer_ns();
-      const uint32_t tbase = tmem_base + ((uint32_t)(quad * 32) << 16) + as * BN;
+      float acc[BN / 2];
+#pragma unroll
+      for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
+      int prev = -1;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        if (trace && kb == 0 && it == 0 && threadIdx.x == 128) trace[3] = globaltimer_ns();
+        const uint32_t sa = smem_u + stage * Cfg::STAGE;
+        const uint64_t da_hi = wgmma_desc_sw128_kmajor(sa + wg * (64 * BK * 2));
+        const uint64_t da_lo = wgmma_desc_sw128_kmajor(sa + Cfg::A_TILE + wg * (64 * BK * 2));
+        const uint64_t db_hi = wgmma_desc_sw128_kmajor(sa + 2 * Cfg::A_TILE);
+        const uint64_t db_lo = wgmma_desc_sw128_kmajor(sa + 2 * Cfg::A_TILE + Cfg::B_TILE);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < BK / 16; ++kk) {
+          const uint64_t ko = (uint64_t)(kk * 32 >> 4);  // 16 bf16 = 32 bytes along K inside the swizzle span
+          wgmma_bf16<BN>(acc, da_hi + ko, db_lo + ko, 1);
+          wgmma_bf16<BN>(acc, da_lo + ko, db_hi + ko, 1);
+          wgmma_bf16<BN>(acc, da_hi + ko, db_hi + ko, 1);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();   // the previous k-block's MMAs have retired: its stage goes back to the producer
+        if (prev >= 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty_bar[prev]);
+        }
+        prev = stage;
+        if (++stage == Cfg::STAGES) {
+          stage = 0;
+          phase ^= 1;
+        }
+      }
+      wgmma_wait<0>();
+      if (prev >= 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      }
+      if (trace && it == 0 && threadIdx.x == 128) trace[4] = globaltimer_ns();
 
       float ht_acc[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll 1
+#pragma unroll
       for (int cc = 0; cc < CH; ++cc) {
+        if (cc > 0) asm volatile("bar.sync 1, %0;" ::"n"(32 * kEpiWarps) : "memory");   // previous chunk consumed
+        // accumulator fragment -> staging rows: chunk cc of each column half
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float* dst = sacc + h * (BM * kAccLD);
+#pragma unroll
+          for (int ii = 0; ii < 4; ++ii) {
+            const int i = (h * CH + cc) * 4 + ii;                 // 8-column block of the accumulator
+            const int r = wg * 64 + wq * 16 + (lane >> 2);
+            const int c = ii * 8 + 2 * (lane & 3);
+            *reinterpret_cast<float2*>(dst + r * kAccLD + c) = make_float2(acc[4 * i], acc[4 * i + 1]);
+            *reinterpret_cast<float2*>(dst + (r + 8) * kAccLD + c) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
+          }
+        }
+        asm volatile("bar.sync 1, %0;" ::"n"(32 * kEpiWarps) : "memory");
+        float* myrows = sacc + half * (BM * kAccLD) + quad * 32 * kAccLD;   // also this warp's staging tile below
+        float v[32];
+        {
+          const float4* src = reinterpret_cast<const float4*>(myrows + lane * kAccLD);
+#pragma unroll
+          for (int q = 0; q < 8; ++q) {
+            const float4 t = src[q];
+            v[4 * q] = t.x; v[4 * q + 1] = t.y; v[4 * q + 2] = t.z; v[4 * q + 3] = t.w;
+          }
+        }
+        __syncwarp();
         const int c = half * CH + cc;
         const int col0 = nt * BN + c * 32;
-        if (col0 >= args.N) break;  // warp-uniform
-        uint32_t raw[32];
-        tmem_ld_32x32(tbase + c * 32, raw);
-        if (cc + 1 < CH && col0 + 32 < args.N) epi_prefetch_res<EPI, SW>(args, tr, rnxt, col0 + 32, lane);
-        tmem_ld_wait();
-        if (trace && it == 0 && cc == 0 && threadIdx.x == 64) trace[8] = globaltimer_ns();
-        float v[32];
+        if (col0 < args.N) {   // warp-uniform
+          if (cc + 1 < CH && col0 + 32 < args.N) epi_prefetch_res<EPI, 32>(args, tr, rnxt, col0 + 32, lane);
+          epi_chunk<EPI, 32>(args, v, sb + c * 32, scs + c * 32, myrows, tg, er, tr, rcur, col0, lane, ht_acc);
 #pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(raw[j]);
-
-        epi_chunk<EPI, SW>(args, v, sb + c * 32, scs + c * 32, stg, tg, er, tr, rcur, col0, lane, ht_acc);
-        if (trace && it == 0 && cc == 0 && threadIdx.x == 64) trace[9] = globaltimer_ns();
-#pragma unroll
-        for (int q = 0; q < 8; ++q) rcur[q] = rnxt[q];
+          for (int q = 0; q < 8; ++q) rcur[q] = rnxt[q];
+        }
       }
-      if (trace && it == 0 && threadIdx.x == 64) trace[10] = globaltimer_ns();
-      // accumulator fully read -> hand the TMEM stage back to the MMA warp
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[as]);
 
       if constexpr (EPI == EPI_HEADTAIL) {
         // the row's 4 dot products are split over the two column halves: half 1 hands its partial sums to half 0
-        // through its staging tile (two alternating slots), 64-thread named barrier per lane quadrant
-        uint8_t* stg_base = reinterpret_cast<uint8_t*>(colv) + Cfg::COLV;
-        float4* slot = reinterpret_cast<float4*>(stg_base + (4 + quad) * Stg<SW>::WARP_BYTES) + (it & 1) * 32;
+        // (two alternating slots), 64-thread named barrier per lane quadrant
+        float4* slot = hts + (quad * 2 + (it & 1)) * 32;
         if (half == 1) slot[lane] = make_float4(ht_acc[0], ht_acc[1], ht_acc[2], ht_acc[3]);
         asm volatile("bar.sync %0, 64;" ::"r"(2 + quad) : "memory");
         if (half == 0) {
@@ -306,16 +303,9 @@ __global__ void __launch_bounds__(kNumThreads, 1) gemm_bf16x3_kernel(const __gri
         }
       }
     }
+    if (trace && threadIdx.x == 128) trace[5] = globaltimer_ns();   // epilogue of this CTA's last tile done
   }
-
-  if (trace && threadIdx.x == 64) trace[5] = globaltimer_ns();   // epilogue of this CTA's last tile done
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after_sync();
-    tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
-  }
-  if (trace && threadIdx.x == 0) trace[6] = globaltimer_ns();
+  if (trace && threadIdx.x == 128) trace[6] = globaltimer_ns();     // exit (the producer warpgroup has no work left)
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -383,11 +373,7 @@ static int next_pow2(int x) {
 Options& options() {
   static Options o = [] {
     Options x;
-    if (const char* e = getenv("S3R_GEMM2")) x.gemm2 = atoi(e);
-    if (const char* e = getenv("S3R_GEMM2_64")) x.gemm2_64 = atoi(e);
     if (const char* e = getenv("S3R_PREFETCH_B")) x.prefetch_b = atoi(e);
-    if (const char* e = getenv("S3R_ATTN_PAIR")) x.attn_pair = atoi(e);
-    if (const char* e = getenv("S3R_CHAIN")) x.chain = atoi(e);
     return x;
   }();
   return o;
@@ -400,7 +386,7 @@ int num_sms() {
   int& n = g_num_sms[dev & 63];
   if (!n) {
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }
@@ -426,50 +412,26 @@ int gemm_plan_init(GemmPlan* plan, const __nv_bfloat16* a_hi, const __nv_bfloat1
   a.tiles_w = (W + a.bw - 1) / a.bw;
   a.tiles_h = (H + a.bh - 1) / a.bh;
   a.out_group_rows = (long long)NB * H * W;
-  // Tile shape: the cheapest of {128 x 64, 128 x 128 (1 CTA), 256 x 128 (CTA pair)} under a two-constant model fitted to
-  // tools/gemm_sweep.py / conv_sweep.py on B200 (profiles/r1_tile_sweep.md): makespan = waves x k-blocks x period, with
-  // waves = ceil(tiles / CTAs (148) or CTA pairs (74)) for the persistent static schedule and the measured k-block
-  // periods 0.45 us (128 x 64), 0.62 us (128 x 128), 0.58 us (256 x 128 per pair: each SM stages only half of B).
-  // 256-wide tiles never win any more (two-stage ring), so they are only reachable through force_bn.
+  // Tile shape: 128 x 64 or 128 x 128, the cheaper under makespan = waves x (bytes staged per k-block), with waves =
+  // ceil(tiles / SMs) for the persistent static schedule and 48 KB (128 x 64) / 64 KB (128 x 128) staged per k-block.
+  // A 64-row warpgroup holds a 64 x BN fp32 accumulator in registers next to the epilogue's working set, so 128 is the
+  // widest tile; wider requests (force_bn 256, and 2064 / 2128 / 2256, the tile widths of CTA-pair kernels on other
+  // architectures) run at the nearest width the kernel has.
   const long long m_tiles = (long long)a.tiles_w * a.tiles_h * NB * groups;
-  const long long m_tiles_group = (long long)a.tiles_w * a.tiles_h * NB;
   const int sms = num_sms();
   auto waves = [](long long tiles, long long slots) { return (double)((tiles + slots - 1) / slots); };
   const long long nt64 = (N + 63) / 64, nt128 = (N + 127) / 128;
-  const double c64 = waves(m_tiles * nt64, sms) * 0.45;
-  const double c128 = (N > 64) ? waves(m_tiles * nt128, sms) * 0.62 : 1e30;
-  const bool legal2 = (m_tiles_group % 2 == 0) && N >= 128;
-  const int g2_mode = options().gemm2;   // 0 off, 1 auto, 128/256 fixed
-  const double c2128 = (legal2 && g2_mode != 0) ? waves(m_tiles / 2 * nt128, sms / 2) * 0.58 : 1e30;
-  int bn = 64, two = 0;
-  if (c128 < c64) bn = 128;
-  if (c2128 <= (bn == 64 ? c64 : c128)) { bn = 128; two = 1; }
-  if (N <= 64) { bn = 64; two = 0; }
-  // many-wave GEMMs whose width is a multiple of 256 (the batched encoder): 256 x 256 pair tiles halve the number of
-  // per-tile epilogue preambles (LayerNorm statistics, staged columns) -- measured in situ, not visible in the sweep
-  const long long tiles128 = m_tiles * nt128;
-  if (two && taps == 1 && N % 256 == 0 && tiles128 >= 400) bn = 256;
-  // (Tried in round 2 and removed: 256 x 256 pair tiles for few-wave GEMMs whose last 256 x 128 wave is badly filled -- the
-  // decoder's / value encoder's fc1 at B = 1 -- one wave at 4/3 of the bytes per SM instead of two: +1.8 % per sequence in the
-  // in-process A/B, profiles/r2g_ab_256.jsonl.  Three ring slots of 64 KB do not cover the TMA latency of a one-wave launch.)
-  if (force_bn == 0 && legal2 && (g2_mode == 128 || g2_mode == 256)) {
-    two = 1;
-    bn = (g2_mode == 256 && N % 256 == 0) ? 256 : 128;
+  const double c64 = waves(m_tiles * nt64, sms) * 48.0;
+  const double c128 = (N > 64) ? waves(m_tiles * nt128, sms) * 64.0 : 1e30;
+  int bn = (c128 <= c64) ? 128 : 64;
+  int fb = force_bn >= 2000 ? force_bn - 2000 : force_bn == 1128 ? 128 : force_bn;
+  if (fb > 0) {
+    if (fb != 64 && fb != 128 && fb != 256) {
+      set_error("gemm_plan_init: force_bn %d (64, 128, 256, 1128, 2064, 2128, 2256 or 0)", force_bn);
+      return -1;
+    }
+    bn = fb > 128 ? 128 : fb;
   }
-  // EXPERIMENT (off by default, not yet measured): where the planner settles on 1-CTA 128 x 64 tiles -- the N = 768 / 1024
-  // GEMMs of the decoder and value encoder at B = 1, one wave of 144 CTAs, bound by the per-SM operand ingest (DESIGN.md
-  // section 4b) -- a 256 x 64 CTA-pair tile keeps the CTA count and the MMA work per SM but stages only half of B per SM:
-  // 40 KB instead of 48 KB per k-block.  S3R_GEMM2_64=1 switches those launches over for an in-situ A/B.
-  const bool pair64 = options().gemm2_64 != 0;
-  if (pair64 && force_bn == 0 && !two && bn == 64 && m_tiles_group % 2 == 0 && N >= 64) two = 1;
-  if (force_bn == 1128) { two = legal2 ? 1 : 0; bn = 128; }   // width 128 (EPI_HEADTAIL), CTA pairs where legal
-  else if (force_bn >= 2000) { two = 1; bn = force_bn - 2000; }
-  else if (force_bn > 0) { two = 0; bn = force_bn; }
-  if (two && (m_tiles_group % 2 != 0 || (bn != 64 && bn != 128 && bn != 256))) {
-    set_error("gemm_plan_init: 2-CTA tiles need an even m-tile count per group and bn in {64,128,256}");
-    return -1;
-  }
-  plan->two_cta = two;
   plan->bn = bn;
 
   const uint64_t esz = 2;
@@ -485,7 +447,7 @@ int gemm_plan_init(GemmPlan* plan, const __nv_bfloat16* a_hi, const __nv_bfloat1
     uint64_t dims[3] = {(uint64_t)Kc, (uint64_t)taps, (uint64_t)(b_group_rows * (groups - 1) + N)};
     // with a single tap the tap stride is never used, but must still be a multiple of 16 bytes
     uint64_t str[2] = {(uint64_t)(taps == 1 ? ldb : Kc) * esz, (uint64_t)ldb * esz};
-    uint32_t box[3] = {(uint32_t)BK, 1, (uint32_t)(two ? bn / 2 : bn)};
+    uint32_t box[3] = {(uint32_t)BK, 1, (uint32_t)bn};
     int r;
     if ((r = encode_tmap(&a.tmB_hi, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, b_hi, dims, str, box))) return r;
     if ((r = encode_tmap(&a.tmB_lo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, b_lo, dims, str, box))) return r;
@@ -493,13 +455,7 @@ int gemm_plan_init(GemmPlan* plan, const __nv_bfloat16* a_hi, const __nv_bfloat1
   const long long n_tiles = (N + bn - 1) / bn;
   const long long total = m_tiles * n_tiles;
   a.groups = groups;
-  if (two) {
-    const long long pairs = total / 2;
-    const long long clusters = pairs < num_sms() / 2 ? pairs : num_sms() / 2;
-    plan->grid = dim3((unsigned)(2 * clusters), 1, 1);
-  } else {
-    plan->grid = dim3((unsigned)((total < num_sms()) ? total : num_sms()), 1, 1);  // persistent: <= 1 CTA per SM
-  }
+  plan->grid = dim3((unsigned)((total < num_sms()) ? total : num_sms()), 1, 1);  // persistent: <= 1 CTA per SM
   plan->flops = 2.0 * (double)NB * H * W * groups * (double)N * (double)Kc * taps;
   return 0;
 }
@@ -539,11 +495,9 @@ static int launch_epi(const GemmPlan& plan, cudaStream_t stream) {
 }
 
 int gemm_launch(const GemmPlan& plan, cudaStream_t stream) {
-  if (plan.two_cta) return gemm2_launch(plan, stream);
   switch (plan.bn) {
     case 64: return launch_epi<64>(plan, stream);
     case 128: return launch_epi<128>(plan, stream);
-    case 256: return launch_epi<256>(plan, stream);
   }
   set_error("gemm_launch: bad bn %d", plan.bn);
   return -1;

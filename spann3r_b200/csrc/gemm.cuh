@@ -1,4 +1,4 @@
-// Host-visible description of one launch of the split-bf16 tcgen05 GEMM / implicit-GEMM conv engine.
+// Host-visible description of one launch of the split-bf16 wgmma GEMM / implicit-GEMM conv engine.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -50,7 +50,8 @@ struct GemmArgs {
   int swap_col0;                      // ... for output columns >= swap_col0 only (0 = all); must be a multiple of the tile width
   // Producer side (EPI_PLAIN): write (sum, sum of squares) of every output row chunk, [rows, N/32]
   float2* stats_out;
-  // optional timeline of CTA 0 (tools/trace_gemm.py): 8 x %globaltimer stamps, null = off
+  // optional timeline of CTA 0 (tools/trace_gemm.py): %globaltimer stamps [0..6] = entry, prologue done, dependency wait
+  // done, first operands landed, first accumulator ready, last epilogue done, exit; null = off
   unsigned long long* trace;
   // EPI_PIXSHUF
   int ps_s, ps_cout;
@@ -71,8 +72,7 @@ struct GemmArgs {
 struct GemmPlan {
   GemmArgs args;
   dim3 grid;
-  int bn;          // 64 / 128 / 256
-  int two_cta;     // 1: 256 x bn tiles on CTA pairs (gemm2.cu)
+  int bn;          // 64 / 128
   int b_static;    // engine: B is a packed weight and the prefetch option was on when the plan was built
   double flops;    // algorithmic 2*M*N*K (all groups), for roofline accounting
 };
@@ -80,55 +80,22 @@ struct GemmPlan {
 // Encodes the four tensor maps and picks the tile shape.  Returns 0 or a negative error.
 // lda / ldb: row strides (elements) of A pixels / B rows (0 = dense: Kc resp. taps*Kc);
 // b_group_rows: rows between consecutive groups of B (0 = N).
-// force_bn: 0 = planner's choice; 64/128/256 = 1-CTA kernel with that tile width; 2128/2256 = 2-CTA kernel (256 x 128/256);
-// 1128 = width 128 on CTA pairs where legal, else 1 CTA.
+// force_bn: 0 = planner's choice; 64 / 128 = that tile width; 256, 1128, 2064, 2128, 2256 = the nearest width the kernel has
+// (128, 128, 64, 128, 128).
 int gemm_plan_init(GemmPlan* plan,
                    const __nv_bfloat16* a_hi, const __nv_bfloat16* a_lo,   // [G*NB, H, W, Kc]
                    const __nv_bfloat16* b_hi, const __nv_bfloat16* b_lo,   // [G*N, taps, Kc]
                    int groups, int NB, int H, int W, int Kc, int taps, int N, int force_bn = 0,
                    long long lda = 0, long long ldb = 0, long long b_group_rows = 0);
 int gemm_launch(const GemmPlan& plan, cudaStream_t stream);
-int gemm2_launch(const GemmPlan& plan, cudaStream_t stream);   // 2-CTA kernel (gemm2.cu)
 
 // Tuning knobs of the tile planner / producers (s3r_set_option): read when a plan is BUILT, so two engines of one
 // process can be planned under different settings and timed alternately (tools/ab_inproc.py).
 struct Options {
-  int gemm2 = 1;        // CTA-pair GEMM tiles: 0 off, 1 planner's choice, 128 / 256 forced width
-  int gemm2_64 = 1;     // 256 x 64 pair tiles where the planner picks 1-CTA 128 x 64 (N = 768 / 1024 GEMMs at B = 1): each SM
-                        // stages half of B.  In-process A/B on a B200: -1.8 % per sequence (profiles/r2b_ab_inproc.jsonl)
   int prefetch_b = 1;   // stage the first weight tiles before griddepcontrol.wait
-  int attn_pair = 1;    // two query tiles per CTA for many-wave attention launches
-  int chain = 0;        // dependent GEMM runs of a block (proj -> fc1 -> fc2 -> next qkv, ...) as ONE persistent launch
-                        // (gemm_chain.cu).  Verified bit-identical to separate launches, but measured SLOWER on a B200 in three
-                        // builds (in-process A/B: +9 .. +15 % per sequence, profiles/r2_chain.md): off by default
 };
 Options& options();
 int num_sms();
-
-// ---- persistent chain of dependent GEMMs in one launch (gemm_chain.cu) ----
-constexpr int kChainMaxPhases = 4;
-struct ChainPhase {      // one entry of the device-resident phase table
-  GemmArgs args;         // as the standalone launch would get them (tensor maps + fused epilogue)
-  int bn;                // tile width of this phase: 64 / 128 / 256 (always CTA pairs, 256 rows)
-  int dep;               // phase whose 128-row blocks feed this phase's A rows / statistics / residual (-1: inputs of the launch)
-  int dep_need;          // completions per row block of that phase = its n-tile count
-  int ctr_base;          // first counter of this phase: counters[ctr_base + group * m_tiles + m_tile]
-};
-struct ChainParams {     // the kernel's single __grid_constant__ parameter (3.9 KB of the 4 KB parameter space)
-  ChainPhase ph[kChainMaxPhases];
-  uint32_t* ctr;         // device; [0] = ticket of finished CTAs, then the per-(phase, group, row block) counters
-  int nph, n_ctr, bn_max, pad;
-};
-struct ChainPlan {
-  ChainParams params;
-  dim3 grid;
-  double flops;
-  int first, count;      // count > 0: NOT chainable (e.g. an odd number of row tiles): launch gemms[first .. first+count) one by one
-};
-// plans[p]: two-CTA linear-layer plans with EPI_PLAIN / EPI_QKV epilogues and identical row tiling, phase p+1 consuming the
-// rows phase p writes.  dev_counters: counters_cap uint32 (zeroed here).
-int chain_plan_init(ChainPlan* cp, const GemmPlan* const* plans, int nph, uint32_t* dev_counters, int counters_cap);
-int chain_launch(const ChainPlan& cp, cudaStream_t stream);
 
 int encode_tmap(CUtensorMap* out, CUtensorMapDataType dt, int rank, const void* base, const uint64_t* dims,
                 const uint64_t* strides_bytes, const uint32_t* box);

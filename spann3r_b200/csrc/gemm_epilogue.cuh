@@ -1,12 +1,11 @@
-// Fused epilogue of the split-bf16 GEMM engine, shared by the 1-CTA and the 2-CTA (cta_group::2) kernels.
+// Fused epilogue of the split-bf16 GEMM engine (gemm.cu).
 //
-// Two domains.  tcgen05.ld hands every thread one accumulator ROW (32 consecutive columns per chunk): everything that
+// Two domains.  Every thread holds one accumulator ROW (32 consecutive columns per chunk): everything that
 // is per column or per row -- folded LayerNorm, bias, activation, RoPE -- is done there.  Global memory is then touched
 // in a TRANSPOSED domain: the warp stages its 32 x 32 chunk in shared memory and re-reads it so that 8 consecutive
 // lanes cover one row's 128 bytes; residual loads, fp32 / split-bf16 stores, LayerNorm statistics and the q / k
 // head-split stores are issued from there.  With thread = row every 16-byte access of a warp hits 32 different cache
-// lines (32 L1 wavefronts per instruction, ~1 us per chunk measured with tools/trace_gemm.py); transposed, an
-// instruction covers 4 whole rows (4 wavefronts).
+// lines (32 L1 wavefronts per instruction); transposed, an instruction covers 4 whole rows (4 wavefronts).
 #pragma once
 #include "common.cuh"
 #include "gemm.cuh"
@@ -26,13 +25,7 @@ struct Stg {
   static constexpr int NPASS = 32 / SW;       // passes per 32-column chunk
 };
 
-// Global loads of data another CTA of the SAME launch may have written (chain kernel, gemm_chain.cu: LayerNorm statistics and
-// residual rows produced by an earlier phase): CG = true reads through L2 (ld.global.cg), never a stale L1 line.
-template <bool CG>
-__device__ __forceinline__ float4 ld_f4(const float* p) {
-  if constexpr (CG) return __ldcg(reinterpret_cast<const float4*>(p));
-  else return *reinterpret_cast<const float4*>(p);
-}
+__device__ __forceinline__ float4 ld_f4(const float* p) { return *reinterpret_cast<const float4*>(p); }
 
 __device__ __forceinline__ void apply_act(float (&v)[32], int act) {
   if (act == ACT_GELU) {
@@ -63,22 +56,6 @@ __device__ __forceinline__ void epi_stage_cols(const GemmArgs& args, float* sb, 
       if (args.bias != nullptr)
         b = __ldg(args.bias + ((EPI == EPI_PIXSHUF) ? (long long)g * args.ps_cout + (col % args.ps_cout)
                                                     : (long long)g * args.N + col));
-      if (args.ln_cs != nullptr) c = __ldg(args.ln_cs + (long long)g * args.N + col);
-    }
-    sb[j] = b;
-    scs[j] = c;
-  }
-}
-
-// Same with the tile width as a runtime value (chain kernel: the width changes from phase to phase).
-template <int EPI>
-__device__ __forceinline__ void epi_stage_cols_rt(const GemmArgs& args, float* sb, float* scs, int g, int nt, int bn,
-                                                  int tid_e, int nthr_e) {
-  for (int j = tid_e; j < bn; j += nthr_e) {
-    const int col = nt * bn + j;
-    float b = 0.f, c = 0.f;
-    if (col < args.N) {
-      if (args.bias != nullptr) b = __ldg(args.bias + (long long)g * args.N + col);
       if (args.ln_cs != nullptr) c = __ldg(args.ln_cs + (long long)g * args.N + col);
     }
     sb[j] = b;
@@ -122,7 +99,7 @@ struct EpiTRows {
 // the main loop.  LayerNorm statistics: (sum, sum of squares) per 32-column chunk of the A row, ln_np <= 32 chunks,
 // read cooperatively -- 16 lanes take one row's chunk pairs as float4 (one coalesced 256-byte read per row instead
 // of 16 strided 16-byte reads per thread), two rows per iteration, fixed reduction order.
-template <int EPI, int SW, bool CG = false>
+template <int EPI, int SW>
 __device__ __forceinline__ void epi_tile_pre(const GemmArgs& args, const TileGeom& tg, int quad, int lane, EpiRow& er,
                                              EpiTRows& tr) {
   using S = Stg<SW>;
@@ -143,7 +120,7 @@ __device__ __forceinline__ void epi_tile_pre(const GemmArgs& args, const TileGeo
       const bool v2 = row_pixel(args, tg, rr, h2, w2, pix2);
       t[i] = make_float4(0.f, 0.f, 0.f, 0.f);
       if (v2 && sub < np2)
-        t[i] = ld_f4<CG>(reinterpret_cast<const float*>(args.ln_stats + ((long long)ga * args.out_group_rows + pix2) * args.ln_np) + 4 * sub);
+        t[i] = ld_f4(reinterpret_cast<const float*>(args.ln_stats + ((long long)ga * args.out_group_rows + pix2) * args.ln_np) + 4 * sub);
     }
 #pragma unroll
     for (int i = 0; i < 16; ++i) {
@@ -196,7 +173,7 @@ __device__ __forceinline__ void epi_tile_pre(const GemmArgs& args, const TileGeo
 }
 
 // Residual values of one 32-column chunk in the transposed layout (EPI_PLAIN; requested one chunk ahead).
-template <int EPI, int SW, bool CG = false>
+template <int EPI, int SW>
 __device__ __forceinline__ void epi_prefetch_res(const GemmArgs& args, const EpiTRows& tr, float4 (&rp)[8], int col0,
                                                  int lane) {
   using S = Stg<SW>;
@@ -208,14 +185,14 @@ __device__ __forceinline__ void epi_prefetch_res(const GemmArgs& args, const Epi
 #pragma unroll
         for (int it = 0; it < S::NIT; ++it)
           if (tr.key[it] >= 0)
-            rp[p * S::NIT + it] = ld_f4<CG>(args.res1 + tr.key[it] * args.ldr1 + col0 + p * SW + cq);
+            rp[p * S::NIT + it] = ld_f4(args.res1 + tr.key[it] * args.ldr1 + col0 + p * SW + cq);
     }
   }
 }
 
 // One 32-column chunk.  v: this thread's accumulator row; sb / scs: the chunk's staged bias / colsum values; stg: the
 // warp's staging tile; rp: prefetched residual (transposed layout); ht_acc: running dot products of EPI_HEADTAIL.
-template <int EPI, int SW, bool CG = false>
+template <int EPI, int SW>
 __device__ __forceinline__ void epi_chunk(const GemmArgs& args, float (&v)[32], const float* sb, const float* scs,
                                           float* stg, const TileGeom& tg, const EpiRow& er, const EpiTRows& tr,
                                           const float4 (&rp)[8], int col0, int lane, float (&ht_acc)[4]) {
@@ -356,11 +333,11 @@ __device__ __forceinline__ void epi_chunk(const GemmArgs& args, float (&v)[32], 
           if (args.res1 != nullptr) {
             float4 t;
             if constexpr (EPI == EPI_PLAIN) t = rp[p * S::NIT + it];
-            else t = ld_f4<CG>(args.res1 + orow * args.ldr1 + ocol);
+            else t = ld_f4(args.res1 + orow * args.ldr1 + ocol);
             x.x += t.x; x.y += t.y; x.z += t.z; x.w += t.w;
           }
           if (args.res2 != nullptr) {
-            const float4 t = ld_f4<CG>(args.res2 + orow * args.ldr2 + ocol);
+            const float4 t = ld_f4(args.res2 + orow * args.ldr2 + ocol);
             x.x += t.x; x.y += t.y; x.z += t.z; x.w += t.w;
           }
         }

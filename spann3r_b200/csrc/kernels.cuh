@@ -37,7 +37,6 @@ struct AttnArgs {
 struct AttnPlan {
   AttnArgs args;
   dim3 grid;
-  int pair;        // 1: two query tiles per CTA (attention.cu, PAIR)
   double flops;
 };
 int attn_plan_init(AttnPlan* plan, const float* q, const float* k, const float* vt, int BH, int heads, int nq, int nk,
@@ -81,7 +80,7 @@ int launch_focal_median(const float* pts3d, int B, int H, int W, float ppx, floa
 
 int launch_conf_score(const float* conf, long long n, float* scratch256, float* out, cudaStream_t st);
 
-// fused attention (attention.cu): O = softmax(Q K^T) V per (batch*head), tf32 tcgen05, split-bf16 output
+// fused attention (attention.cu): O = softmax(Q K^T) V per (batch*head), tf32 wgmma, split-bf16 output
 int launch_attention(const float* q, const float* k, const float* vt, int BH, int heads, int nq, int nk, int nk_pad,
                      __nv_bfloat16* o_hi, __nv_bfloat16* o_lo, float* o_f32, long long ldo, cudaStream_t st);
 

@@ -6,7 +6,7 @@ same class names, constructor signature, `state_dict` keys (1101, strict-loadabl
 same dict keys / shapes -- so `demo.py` / `eval.py` run by changing one import (INTEGRATION.md).
 
 The modules below hold parameters only.  All arithmetic runs in libspann3r_b200.so through
-`engine.Engine`; there is no eager-PyTorch, CPU or Triton path -- on a machine without an sm_100
+`engine.Engine`; there is no eager-PyTorch, CPU or Triton path -- on a machine without an sm_90
 GPU `forward` raises.  Training mode (`train.py`): the same CUDA forward with the reference's
 training branches (attn_thresh=0, memory dropout, ungated add_mem) and a PyTorch-recompute backward (SURVEY.md §8f rank 1, staged).
 `offline_reconstruction` (SURVEY.md §8f rank 2) is built on the same engine stages.  Portrait frames follow the
@@ -338,7 +338,7 @@ class Spann3R(ParamModule):
         if self._packed is None or self._packed_dirty:
             dev = next(self.parameters()).device
             if dev.type != "cuda":
-                raise RuntimeError("spann3r_b200.Spann3R runs on a B200 only: call .to('cuda') first (no CPU path)")
+                raise RuntimeError("spann3r_b200.Spann3R runs on an H100 only: call .to('cuda') first (no CPU path)")
             self._engines.clear()
             self._packed = None
             self._packed = PackedWeights(self.state_dict(), device=dev)
@@ -350,7 +350,7 @@ class Spann3R(ParamModule):
         and IN PLACE (`PackedWeights.refresh`), which keeps the engines and their cached tile plans valid."""
         dev = next(self.parameters()).device
         if dev.type != "cuda":
-            raise RuntimeError("spann3r_b200.Spann3R runs on a B200 only: call .to('cuda') first (no CPU path)")
+            raise RuntimeError("spann3r_b200.Spann3R runs on an H100 only: call .to('cuda') first (no CPU path)")
         sd = self.state_dict()
         if self._packed is None or self._packed.host_math or self._packed.device != dev or self._packed_moved:
             self._engines.clear()

@@ -10,7 +10,7 @@ the rest is index bookkeeping and one fp32 affine map.
 
 Host side = the small, shape-only parts: the crop / scale geometry of `_crop_resize_if_necessary` and Pillow's
 coefficient tables (`precompute_coeffs` + `normalize_coeffs_8bpc` of src/libImaging/Resample.c), computed once per
-(image size, resolution) and cached on the device.  No CPU fallback: without the library / a B200 this raises.
+(image size, resolution) and cached on the device.  No CPU fallback: without the library / an H100 this raises.
 """
 from __future__ import annotations
 

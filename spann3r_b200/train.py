@@ -3,7 +3,7 @@ staged.
 
 What is native and what is not (said once, here):
 
-* FORWARD: every stage runs the sm_100a kernels of libspann3r_b200.so, exactly as in eval mode, with the reference's
+* FORWARD: every stage runs the sm_90a kernels of libspann3r_b200.so, exactly as in eval mode, with the reference's
   training-mode branches -- `attn_thresh=0` (no cut / renormalisation in the memory read, :474), `mem_dropout` on the
   attention weights (:167-168; Philox mask, reproducible: `s3r_engine_memory_read_train`), ungated `add_mem` (:518-519).
   The packed weights are refreshed in place from the (optimizer-updated) parameters at the start of every forward.
@@ -75,7 +75,7 @@ class _Stage(torch.autograd.Function):
 
 
 def set_native_linear(on: bool = True):
-    """Run the Linear layers of the backward (recompute forward, dgrad, wgrad) on the tcgen05 GEMM engine (`_native_linear.py`)
+    """Run the Linear layers of the backward (recompute forward, dgrad, wgrad) on the wgmma GEMM engine (`_native_linear.py`)
     instead of `F.linear` + PyTorch autograd."""
     from . import _native_linear
     _native_linear.ENABLED = bool(on)

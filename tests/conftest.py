@@ -10,8 +10,8 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
-    config.addinivalue_line("markers", "gpu_unverified: GPU test of a kernel that has not run on a B200 yet (skipped without a "
+    config.addinivalue_line("markers", "gpu: needs a real H100 (run with -m gpu)")
+    config.addinivalue_line("markers", "gpu_unverified: GPU test of a kernel that has not run on an H100 yet (skipped without a "
                                        "GPU; NOT selected by -m gpu; run with -m gpu_unverified, then re-mark as gpu)")
 
 

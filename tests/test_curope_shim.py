@@ -67,8 +67,8 @@ def test_inplace_and_autograd_wiring_with_the_oracle_rotation(monkeypatch):
     assert rel_l2(x.grad, ref_x.grad) < 1e-6
 
 
-@pytest.mark.gpu          # verified on a B200 in round 2 (profiles/r2a_unverified.log)
-@pytest.mark.skipif(not torch.cuda.is_available(), reason="needs a B200")
+@pytest.mark.gpu
+@pytest.mark.skipif(not torch.cuda.is_available(), reason="needs an H100")
 def test_cuda_rope_matches_the_oracle_forward_and_backward():
     from oracle.spann3r_oracle import rope2d
     from spann3r_b200 import curope

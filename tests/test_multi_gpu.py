@@ -1,4 +1,5 @@
-"""GPU tests that need TWO devices (skipped on a 1-GPU box; run with `gpurun --gpus 2 -- python -m pytest tests/test_multi_gpu.py -m gpu`).
+"""GPU tests that need TWO devices (skipped on a machine with one GPU; run with `python -m pytest tests/test_multi_gpu.py -m gpu`
+on two).
 
 * a model living on cuda:1 while cuda:0 is the current device (ADVICE r1: nothing selected the device) gives the
   same result as on cuda:0 -- the reference's `.to(device)` works on any device;

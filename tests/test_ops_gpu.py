@@ -43,7 +43,7 @@ def test_split_roundtrip(L):
     (300, 96, 1536, 1, 0), (768, 768, 768, 2, 0), (768, 1792, 1792, 2, 0),
     (1000, 512, 512, 1, 64), (1000, 512, 512, 1, 128), (1000, 512, 512, 1, 256), (7680, 1024, 1024, 1, 0),
     (130, 64, 32, 1, 0),
-    # 2-CTA (cta_group::2) kernel, 256 x 128 / 256 x 256 pair tiles
+    # force_bn 2128 / 2256: CTA-pair tile widths of other architectures, the nearest width on sm_90a
     (768, 1024, 3072, 1, 2128), (768, 1024, 3072, 1, 2256), (768, 768, 768, 2, 2128), (7680, 1024, 1024, 1, 2256),
     (1536, 768, 96, 1, 2128), (768, 4096, 1024, 1, 2256),
     # K-heavy shapes with few tiles (value-encoder fc2, decoder fc2, tiny-M long-K)
@@ -68,7 +68,7 @@ def test_linear_bias_gelu_residual(L, rows, K, N, groups, bn):
 @pytest.mark.parametrize("NB,H,W,Cin,Cout,groups,bn", [
     (1, 12, 16, 256, 256, 2, 0), (1, 24, 32, 96, 256, 1, 0), (2, 7, 7, 256, 256, 1, 0), (1, 96, 128, 256, 128, 2, 0),
     (1, 14, 14, 384, 256, 1, 0), (1, 48, 64, 192, 256, 1, 0), (1, 12, 16, 768, 256, 2, 0),
-    # 2-CTA pair tiles on a 3x3 conv (two pixel tiles share the weight tile)
+    # force_bn 2128 / 2256 on a 3x3 conv
     (1, 96, 128, 256, 256, 2, 2256), (1, 96, 128, 256, 128, 1, 2128), (2, 24, 32, 96, 256, 1, 2256),
 ])
 def test_conv3x3(L, NB, H, W, Cin, Cout, groups, bn):
@@ -133,7 +133,7 @@ def _cs_table(maxpos=64):
 
 @pytest.mark.parametrize("B,gh,gw,heads,groups", [(1, 24, 32, 16, 1), (2, 14, 14, 12, 1), (1, 24, 32, 12, 2), (1, 5, 9, 2, 1)])
 def test_qkv_rope_attention(L, B, gh, gw, heads, groups):
-    """QKV projection with the fused RoPE/head-split epilogue, then the tcgen05 attention core,
+    """QKV projection with the fused RoPE/head-split epilogue, then the wgmma attention core,
     against croco/models/blocks.py:94-112 evaluated in fp64 (through the pinned oracle's rope2d)."""
     from oracle.spann3r_oracle import rope2d
     C = heads * 64

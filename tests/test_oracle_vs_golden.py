@@ -1,7 +1,8 @@
 """Pins the oracle (oracle/spann3r_oracle.py) to outputs of the REAL reference.
 
-The golden npz files were produced by tools/make_golden.py, which imports /root/reference and runs
-`Spann3R.forward` on CPU in strict fp32 with the same synthetic checkpoint / frames.  Tolerance:
+The golden npz files were produced by tools/make_golden.py, which imports the reference and runs
+`Spann3R.forward` on CPU in strict fp32 with the same synthetic checkpoint / frames.  They store every px_stride-th
+pixel of the prediction maps and every 7 mem_stride-th token (every 8th channel) of the memory bank.  Tolerance:
 2e-5 relative L2 = fp32 reassociation noise between two eager PyTorch programs (SURVEY.md §6 measured
 1-3e-6 run-to-run on the reference itself).
 """
@@ -171,6 +172,7 @@ def test_offline_reconstruction_matches_reference():
         assert rel_l2(graph["pred2"]["conf"][j][::4, ::4], g["graph/pred2_conf"][i]) < TOL
     preds, preds_all, idx_used = orc.offline_reconstruction(sd, frames, graph)
     assert list(idx_used) == list(g["idx_used"])
+    s = int(g["meta/px_stride"])
     for i, p in enumerate(preds):
         for k, v in p.items():
-            assert rel_l2(v, g[f"preds/{i}/{k}"]) < TOL, (i, k)
+            assert rel_l2(v[:, ::s, ::s], g[f"preds/{i}/{k}"]) < TOL, (i, k)

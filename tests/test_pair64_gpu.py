@@ -1,6 +1,5 @@
-"""256 x 64 CTA-pair GEMM tiles (`gemm2_bf16x3_kernel<64, *>`, force_bn 2064 / s3r_set_option("gemm2_64", 1)): the same
-op-level parity bodies as tests/test_ops_gpu.py.  Written without a GPU at the end of round 1, verified on a B200 in the
-first call of round 2 (profiles/r2a_unverified.log)."""
+"""GEMMs requested with force_bn 2064 (the 256 x 64 CTA-pair tile width of other architectures; on sm_90a the 128 x 64
+kernel): the same op-level parity bodies as tests/test_ops_gpu.py."""
 import pytest
 import torch
 

@@ -63,10 +63,9 @@ def test_median_mode_oracle_and_device_math_are_bit_exact(tmp_path):
 
 
 @pytest.mark.gpu
-@pytest.mark.skipif(not torch.cuda.is_available(), reason="needs a B200")
+@pytest.mark.skipif(not torch.cuda.is_available(), reason="needs an H100")
 def test_cuda_focal_median_is_bit_exact():
-    """The CUDA radix select (s3r_focal_median) against the real reference's values, bit for bit.  (Written without a GPU at
-    the end of round 1; verified on a B200 in the first call of round 2, profiles/r2a_unverified.log.)"""
+    """The CUDA radix select (s3r_focal_median) against the real reference's values, bit for bit."""
     from spann3r_b200.postprocess import estimate_focal_knowing_depth
     pm = _pointmap()
     for c in _cases():

@@ -170,7 +170,17 @@ class _TorchEngine:
         return R.memory_read(self.P, feat, torch.cat(self.bank_k, 1), torch.cat(self.bank_v, 1))
 
 
-def test_training_forward_and_recompute_backward_end_to_end_on_cpu(monkeypatch, sd):
+@pytest.fixture
+def one_cpu_thread():
+    """The parameter gradients below are sums of cancelling contributions: another CPU reduction order (thread count) alone
+    moves them by up to ~4e-4, so the test computes both sides on one thread, in the same order on every host."""
+    n = torch.get_num_threads()
+    torch.set_num_threads(1)
+    yield
+    torch.set_num_threads(n)
+
+
+def test_training_forward_and_recompute_backward_end_to_end_on_cpu(monkeypatch, sd, one_cpu_thread):
     """`train.forward_train` (the real frame loop, stage Functions and parameter routing) over a torch stand-in engine:
     outputs equal the oracle's training-branch forward and the gradients equal autograd through the oracle to fp32 rounding.
     (On the GPU the same backward is fed by the CUDA forward, whose activations differ by <= 3e-4: tests/test_train_gpu.py.)"""

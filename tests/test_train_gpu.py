@@ -78,8 +78,8 @@ def test_backward_gradients_vs_oracle_autograd(model):
     gradients of the same loss through the oracle differentiated by autograd (strict fp32), on a sample of parameters from
     every stage.  The backward itself is exact (tests/test_train_cpu.py: <= 2e-4 when it is fed fp32-exact activations);
     here it is fed the CUDA forward's activations (<= 3e-4 from fp32: bf16x3 / tf32), and the random-sign loss below makes
-    the parameter gradients sums of cancelling contributions, which amplifies that: measured 1.1e-4 (last head layer) to
-    2.2e-3 on a B200.  Bar: 3e-3 relative and cosine similarity >= 0.99999."""
+    the parameter gradients sums of cancelling contributions, which amplifies that.  Bar: 3e-3 relative and cosine
+    similarity >= 0.99999."""
     from oracle import spann3r_oracle as orc
     from spann3r_b200 import synth
     torch.backends.cuda.matmul.allow_tf32 = False
@@ -123,7 +123,7 @@ def test_backward_gradients_vs_oracle_autograd(model):
 
 
 def test_native_linear_forward_dgrad_wgrad_vs_torch():
-    """`_native_linear`: y = x W^T + b, dx = dy W, dW = dy^T x, db on the tcgen05 GEMM engine (bf16x3) against torch fp64,
+    """`_native_linear`: y = x W^T + b, dx = dy W, dW = dy^T x, db on the wgmma GEMM engine (bf16x3) against torch fp64,
     incl. a row count that is not a multiple of 8 (the wgrad contraction is zero-padded) and the 1792-wide key head."""
     from spann3r_b200 import _native_linear as NL
     g = torch.Generator().manual_seed(3)
@@ -144,8 +144,8 @@ def test_native_linear_forward_dgrad_wgrad_vs_torch():
 
 def test_backward_with_native_linear_matches_the_torch_backward(model):
     """The same training step differentiated with the Linear layers of the backward on the GEMM engine (`set_native_linear`)
-    and with PyTorch's: the gradients agree to bf16x3 accuracy (measured on a B200: 5e-5 .. 2.5e-4 -- each GEMM differs from
-    cuBLAS fp32 by ~1e-5, the parameter gradients are sums of cancelling terms; the op itself is held to 3e-5 against fp64 above)."""
+    and with PyTorch's: the gradients agree to bf16x3 accuracy (each GEMM differs from cuBLAS fp32 by ~1e-5, the parameter
+    gradients are sums of cancelling terms; the op itself is held to 3e-5 against fp64 above)."""
     from spann3r_b200 import synth, train
     torch.backends.cuda.matmul.allow_tf32 = False
     torch.backends.cudnn.allow_tf32 = False

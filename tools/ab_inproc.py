@@ -1,9 +1,9 @@
 #!/usr/bin/env python
 """In-process A/B of one planner option (s3r_set_option): two models in ONE process, planned under option=off / option=on,
 timed ALTERNATELY on the same sequences -- robust against the box-to-box and minute-to-minute clock / power drift that
-makes separate bench.py runs differ by +-1.5 % (profiles/r2a_ab.txt).  Prints one JSON line per option.
+makes separate bench.py runs differ by +-1.5 %.  Prints one JSON line per option.
 
-    python tools/ab_inproc.py gemm2_64=0,1 prefetch_b=1,0 [--rounds 12]
+    python tools/ab_inproc.py prefetch_b=1,0 [--rounds 12]
 """
 import json
 import os

@@ -42,7 +42,7 @@ try:
     H, W = case[0], case[1]
     u, v = np.meshgrid(np.arange(W), np.arange(H))
     p2 = np.stack((u, v), -1).reshape(-1, 2).astype(np.float32)
-    t0 = time.time()     # ONE frame: on a contended many-core host cv2 took 7.6 s per frame (profiles/r1_bench_demo_path.json)
+    t0 = time.time()     # ONE frame: on a contended many-core host cv2 took 7.6 s per frame
     cv2.solvePnPRansac(maps[0][0].reshape(-1, 3), p2, K.astype(np.float32), np.zeros(4, np.float32))
     res["cv2_ms_per_frame"] = (time.time() - t0) * 1e3
     res["cv2"] = cv2.__version__

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Time the tcgen05 GEMM engine over the path's shapes and tile widths (CUDA events, back-to-back launches)."""
+"""Time the wgmma GEMM engine over the path's shapes and tile widths (CUDA events, back-to-back launches)."""
 import os
 import sys
 

@@ -1,26 +1,25 @@
 #!/usr/bin/env python
 """Generate the committed golden vectors by running the REAL reference (CPU, strict fp32).
 
-Runs only in the authoring container (needs /root/reference, which does not exist on the
-GPU box).  Nothing under tests/, bench.py or smoke() imports this file; they read the small
-fixtures it writes into tests/golden/.
+Needs a reference checkout: $SPANN3R_REFERENCE, else a `reference` directory next to this repository.
+Nothing under tests/, bench.py or smoke() imports this file; they read the small fixtures (each under 1 MB) it
+writes into tests/golden/.
 
     python tools/make_golden.py            # everything (~10 min on 8 cores)
     python tools/make_golden.py --only spec
 
 Outputs
   spann3r_b200/state_dict_spec.json   key -> shape of the reference Spann3R state dict
-  tests/golden/cfg1_224_2f_raw.npz    BASELINE config 1 (2 x 224x224), raw random-init weights
-  tests/golden/seq_224_4f_sharp.npz   4 x 224x224, sharpened weights (two memory reads)
-  tests/golden/seq_384x512_3f_sharp.npz  3 x 384x512, sharpened, outputs sub-sampled (::4, ::4)
-  tests/golden/offline_224_4f_sharp.npz  offline mode: 4 x 224x224, complete pair graph -> offline_reconstruction
-  tests/golden/seq_288x224_4f_sharp.npz  PORTRAIT 4 x (H=288, W=224): transpose_to_landscape (dust3r/utils/misc.py:66-94), outputs (::2, ::2)
-  tests/golden/seq_512x384_3f_sharp.npz  PORTRAIT 3 x (H=512, W=384), outputs sub-sampled (::4, ::4)
+  tests/golden/cfg1_224_2f_raw.npz    BASELINE config 1 (2 x 224x224), raw random-init weights, outputs (::2, ::2)
+  tests/golden/seq_224_4f_sharp.npz   4 x 224x224, sharpened weights (two memory reads), outputs (::4, ::4)
+  tests/golden/seq_384x512_3f_sharp.npz  3 x 384x512, sharpened, outputs sub-sampled (::8, ::8)
+  tests/golden/offline_224_4f_sharp.npz  offline mode: 4 x 224x224, complete pair graph -> offline_reconstruction, outputs (::4, ::4)
+  tests/golden/seq_288x224_4f_sharp.npz  PORTRAIT 4 x (H=288, W=224): transpose_to_landscape (dust3r/utils/misc.py:66-94), outputs (::4, ::4)
+  tests/golden/seq_512x384_3f_sharp.npz  PORTRAIT 3 x (H=512, W=384), outputs sub-sampled (::8, ::8)
   tests/golden/seq_224_3f_sharp_mempos.npz  3 x 224x224 with Spann3R(mem_pos_enc=True) (RoPE inside the value encoder)
-  tests/golden/cfg2_384x512_10f_sharp.npz  BASELINE config 2 exactly (10 x 384x512, sharpened ckpt), outputs (::8, ::8)   [--only cfg2]
+  tests/golden/cfg2_384x512_10f_sharp.npz  BASELINE config 2 exactly (10 x 384x512, sharpened ckpt), outputs (::16, ::16), bank rows ::4   [--only cfg2]
   tests/golden/cfg2_384x512_10f_raw.npz    the same on the RAW random-init checkpoint (SURVEY 8d: report both)            [--only cfg2]
-Each npz also holds sub-sampled per-stage activations captured with forward hooks so that a
-parity failure can be localised to a stage.
+The hooked runs also store the sub-sampled per-stage activations the tests compare (GOLDEN_ACTS).
 """
 import argparse
 import json
@@ -32,7 +31,7 @@ import numpy as np
 import torch
 
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference"
+REF = os.environ.get("SPANN3R_REFERENCE") or os.path.join(os.path.dirname(REPO), "reference")
 sys.path.insert(0, REPO)
 GOLD = os.path.join(REPO, "tests", "golden")
 
@@ -77,7 +76,14 @@ def sub(t, tok_stride=7, ch_stride=8):
     return t.numpy()
 
 
-def run(model, frames, out_path, px_stride=1, hooks=True):
+# the hooked activations the tests compare (tests/test_oracle_vs_golden.py); the others are not stored
+GOLDEN_ACTS = ("act/attn_head_1#0", "act/attn_head_2#0", "act/dust3r.dec_blocks.0#0", "act/dust3r.dec_blocks2.0#0",
+               "act/value_out#0")
+
+
+def run(model, frames, out_path, px_stride=1, hooks=True, mem_stride=1):
+    """px_stride: every px_stride-th pixel of each prediction map; mem_stride: every mem_stride-th of the stored bank
+    tokens (which are every 7th token, every 8th channel).  Chosen per config so that each file stays under 1 MB."""
     acts = {}
     handles = []
     if hooks:
@@ -125,15 +131,17 @@ def run(model, frames, out_path, px_stride=1, hooks=True):
     for i, (r1, r2) in enumerate(preds_all):
         for k, v in r2.items():
             out[f"preds_all/{i}/res2/{k}"] = v[:, ::s, ::s].contiguous().numpy()
-    out["mem/mem_k_sub"] = sub(mem.mem_k)
-    out["mem/mem_v_sub"] = sub(mem.mem_v)
+    out["mem/mem_k_sub"] = np.ascontiguousarray(sub(mem.mem_k)[:, ::mem_stride])
+    out["mem/mem_v_sub"] = np.ascontiguousarray(sub(mem.mem_v)[:, ::mem_stride])
     out["mem/mem_attn"] = mem.mem_attn.numpy()
     out["mem/mem_count"] = mem.mem_count.numpy()
     out["meta/px_stride"] = np.array(s)
+    if mem_stride != 1:
+        out["meta/mem_stride"] = np.array(mem_stride)
     out["meta/ref_seconds"] = np.array(dt)
     out["meta/threads"] = np.array(torch.get_num_threads())
     finite = all(np.isfinite(v).all() for k, v in out.items() if k.startswith("preds"))
-    out.update(acts)
+    out.update({k: v for k, v in acts.items() if k in GOLDEN_ACTS})
     np.savez_compressed(out_path, **out)
     print(f"wrote {out_path}: {dt:.1f}s ref forward, finite={finite}, "
           f"|pts3d| max {max(np.abs(v).max() for k, v in out.items() if 'pts3d' in k):.3g}, "
@@ -155,11 +163,10 @@ def run_offline(model, frames, out_path):
            "graph/view2_idx": np.array(output["view2"]["idx"]),
            "graph/pred1_conf": output["pred1"]["conf"][:, ::4, ::4].contiguous().numpy(),
            "graph/pred2_conf": output["pred2"]["conf"][:, ::4, ::4].contiguous().numpy(),
-           "graph/pred1_pts3d": output["pred1"]["pts3d"][:, ::4, ::4].contiguous().numpy(),
-           "meta/ref_seconds": np.array(time.time() - t0)}
+           "meta/ref_seconds": np.array(time.time() - t0), "meta/px_stride": np.array(4)}
     for i, p in enumerate(preds):
         for k, v in p.items():
-            out[f"preds/{i}/{k}"] = v.contiguous().numpy()
+            out[f"preds/{i}/{k}"] = v[:, ::4, ::4].contiguous().numpy()
     np.savez_compressed(out_path, **out)
     print(f"wrote {out_path}: idx_used={idx_used}, {time.time() - t0:.1f}s, {os.path.getsize(out_path)/1e6:.2f} MB")
 
@@ -174,7 +181,7 @@ def main():
     if args.only in ("all", "spec", "cfg1"):
         m = build_reference(sharpen=False)
         if args.only != "spec":
-            run(m, synth.make_frames(2, 224, 224), os.path.join(GOLD, "cfg1_224_2f_raw.npz"))
+            run(m, synth.make_frames(2, 224, 224), os.path.join(GOLD, "cfg1_224_2f_raw.npz"), px_stride=2)
         del m
     if args.only in ("all", "mempos"):
         m = build_reference(sharpen=True, mem_pos_enc=True)
@@ -183,19 +190,20 @@ def main():
     if args.only in ("all", "cfg2"):   # the headline config itself, both checkpoints (~10 CPU-minutes each on 8 cores)
         for sharpen, tag in ((True, "sharp"), (False, "raw")):
             m = build_reference(sharpen=sharpen)
-            run(m, synth.make_frames(10, 384, 512), os.path.join(GOLD, f"cfg2_384x512_10f_{tag}.npz"), px_stride=8, hooks=False)
+            run(m, synth.make_frames(10, 384, 512), os.path.join(GOLD, f"cfg2_384x512_10f_{tag}.npz"), px_stride=16, hooks=False,
+                mem_stride=4)
             del m
     if args.only in ("all", "seq224", "seq512", "offline", "portrait"):
         m = build_reference(sharpen=True)
         if args.only in ("all", "portrait"):
-            run(m, synth.make_frames(4, 288, 224), os.path.join(GOLD, "seq_288x224_4f_sharp.npz"), px_stride=2, hooks=False)
-            run(m, synth.make_frames(3, 512, 384), os.path.join(GOLD, "seq_512x384_3f_sharp.npz"), px_stride=4, hooks=False)
+            run(m, synth.make_frames(4, 288, 224), os.path.join(GOLD, "seq_288x224_4f_sharp.npz"), px_stride=4, hooks=False)
+            run(m, synth.make_frames(3, 512, 384), os.path.join(GOLD, "seq_512x384_3f_sharp.npz"), px_stride=8, hooks=False)
         if args.only in ("all", "offline"):
             run_offline(m, synth.make_frames(4, 224, 224), os.path.join(GOLD, "offline_224_4f_sharp.npz"))
         if args.only in ("all", "seq224"):
-            run(m, synth.make_frames(4, 224, 224), os.path.join(GOLD, "seq_224_4f_sharp.npz"))
+            run(m, synth.make_frames(4, 224, 224), os.path.join(GOLD, "seq_224_4f_sharp.npz"), px_stride=4)
         if args.only in ("all", "seq512"):
-            run(m, synth.make_frames(3, 384, 512), os.path.join(GOLD, "seq_384x512_3f_sharp.npz"), px_stride=4)
+            run(m, synth.make_frames(3, 384, 512), os.path.join(GOLD, "seq_384x512_3f_sharp.npz"), px_stride=8)
 
 
 if __name__ == "__main__":

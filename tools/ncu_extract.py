@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """`ncu -i X.ncu-rep --page raw --csv` -> a compact markdown table (one row per captured launch) of the metrics the roofline
-discussion uses.  Usage: python tools/ncu_extract.py raw.csv [--title T] > profiles/rN_ncu_full.md"""
+discussion uses.  Usage: python tools/ncu_extract.py raw.csv [--title T] > ncu_full.md"""
 import csv
 import sys
 

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Summarise an `ncu --csv` launch list (metrics gpu__time_duration.sum [+ dram__bytes_read/write.sum]) into a
 per-kernel markdown table, and (with --traffic OUT.json) the DRAM bytes per GEMM launch that bench.py reports as
-roofline.traffic.  Usage: python tools/summarize_ncu.py launches.csv [--traffic profiles/gemm_traffic.json] [--title T]"""
+roofline.traffic.  Usage: python tools/summarize_ncu.py launches.csv [--traffic gemm_traffic.json] [--title T]"""
 import csv
 import json
 import re
@@ -53,7 +53,7 @@ if "--traffic" in sys.argv:
     g = [d for d in per_launch.values() if "gemm" in d["name"] and "bf16x3" in d["name"]]
     rd = sum(d.get("dram__bytes_read.sum", 0.0) for d in g)
     wr = sum(d.get("dram__bytes_write.sum", 0.0) for d in g)
-    json.dump({"kernel": "gemm_bf16x3_kernel<*> + gemm2_bf16x3_kernel<*> (all launches of one 10-frame 512x384 sequence)",
+    json.dump({"kernel": "gemm_bf16x3_kernel<*> (all launches of one 10-frame 512x384 sequence)",
                "launches": len(g), "dram_bytes_per_launch": (rd + wr) / max(len(g), 1), "dram_read_bytes_total": rd,
                "dram_write_bytes_total": wr,
                "algorithmic_bytes_note": "compulsory HBM bytes of one sequence with the batched encoder: weights 1.21 GB (encoder, read once per sequence: all 10 frames in one M = 7680 call) + 9 x 1.42 GB (decoder, heads, value encoder per step) = 14.0 GB, plus ~1.3 GB per step of unfused DPT activations (SURVEY 8d) = 25.7 GB; the measured total is ~1.55x that and runs at ~12 % of the measured HBM peak: not the limiter",

@@ -37,7 +37,7 @@ for K in (64, 768):
             L.gemm(d)
     torch.cuda.synchronize()
     t = trace.cpu().double()
-    names = ["entry", "prologue", "pdl_wait", "operands", "accum", "epilogue", "exit", "mma_issued", "ld0", "chunk0", "loop_end"]
+    names = ["entry", "prologue", "pdl_wait", "operands", "accum", "epilogue", "exit"]   # the stamps gemm.cu writes
     print(f"K={K}: per-launch timeline of CTA 0, ns relative to the previous launch's exit stamp (launches 8..15)")
     for i in range(8, 16):
         base = t[i - 1, 6]

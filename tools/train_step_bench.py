@@ -6,10 +6,10 @@
 
 One step = `spann3r/training.py:216-228`: forward of a batch of `--batch` sequences per rank -> `ConfLoss_t(Regr3D_t(L21,
 norm_mode='avg_dis', fix_first=False), alpha=0.4).compute_frame_loss` (the REFERENCE's criterion, imported from the staged
-copy under baseline/_ref: losses are callers of the path, SURVEY.md §2) -> backward -> DDP gradient all-reduce (NCCL, 2.63 GB
+copy under oracle/_ref: losses are callers of the path, SURVEY.md §2) -> backward -> DDP gradient all-reduce (NCCL, 2.63 GB
 fp32 per rank, `DistributedDataParallel(find_unused_parameters=True, static_graph=True)` as `training.py:322-325`) -> AdamW.
 
---impl ours: `spann3r_b200.Spann3R` in training mode = the sm_100a kernels forward (attn_thresh=0, Philox memory dropout,
+--impl ours: `spann3r_b200.Spann3R` in training mode = the sm_90a kernels forward (attn_thresh=0, Philox memory dropout,
 ungated add_mem) + the PyTorch-RECOMPUTE backward of `spann3r_b200/train.py` (native dgrad / wgrad not written yet: backward
 time is eager PyTorch and is reported as such).  --impl reference: the unmodified reference module, eager PyTorch both ways.
 
@@ -134,7 +134,7 @@ def main():
             "ms_per_step_no_sync": ms_ns, "exposed_allreduce_ms": max(0.0, ms - ms_ns) if world > 1 else None,
             "gradient_bytes_per_rank": 4 * nparam, "loss_first": l0, "loss_last": l1,
             "backward": "PyTorch recompute (spann3r_b200/train.py)" if a.impl == "ours" else "PyTorch autograd (reference)",
-            "forward": "sm_100a kernels (libspann3r_b200.so)" if a.impl == "ours" else "PyTorch eager (reference)",
+            "forward": "sm_90a kernels (libspann3r_b200.so)" if a.impl == "ours" else "PyTorch eager (reference)",
             "wall_s": time.time() - t0}), flush=True)
     if world > 1:
         dist.barrier()
