@@ -174,6 +174,43 @@ int s3r_pnp_ransac(const float* pts3d, const float* img_pts, int b, int64_t n, i
                    double cy, float reproj_err, int n_samples, int refine_iters, uint64_t seed, void* workspace,
                    double* out, uint8_t* inlier_mask, void* stream);
 
+/* ---- reconstruction metrics: eval.py:189-218 on the device ------------------------------------------------------------
+ * Open3D point-to-point ICP, 30-NN normals and spann3r/tools/eval_recon.py accuracy / completion (scipy cKDTree queries).
+ * Points are [n, 3] fp32 (is_f64 = 0) or fp64 (is_f64 = 1); all arithmetic is fp64.  1 <= n < 2^31 everywhere.
+ * transform: optional 3x4 row-major fp64 [R | t] on the device, applied to every input point (NULL = identity).
+ *
+ * Spatial index over one cloud: s3r_pcl_index_bytes(n) bytes of caller-owned device memory, 16-byte aligned (0 = n out of
+ * range).  Every call that takes an index takes the n it was built with.  The index holds the (transformed) points. */
+size_t s3r_pcl_index_bytes(int64_t n);
+int s3r_pcl_index_build(const void* pts, int is_f64, int64_t n, const double* transform, void* index, void* stream);
+/* Exact 1-NN of nq queries (optionally transformed): dist [nq] fp64 (sqrt of ((dx dx + dy dy) + dz dz), each step
+ * rounded), idx [nq] int64 original index; ties -> the smallest index; nothing within max_dist (inclusive; +inf = no
+ * bound) -> idx -1, dist +inf. */
+int s3r_pcl_nearest(const void* index, int64_t n, const void* queries, int is_f64, int64_t nq, const double* transform,
+                    double max_dist, double* dist, int64_t* idx, void* stream);
+/* Normal of every indexed point: unit eigenvector of the smallest eigenvalue of the mean-centred covariance of its
+ * k nearest points (itself included; 1 <= k <= 32; ties -> smaller index), sign as the solver produces it, in original
+ * order -> normals [n, 3] fp64.  Fewer than 3 points or a zero covariance -> (0, 0, 1). */
+int s3r_pcl_normals(const void* index, int64_t n, int k, double* normals, void* stream);
+/* Point-to-point ICP of ns source points onto an indexed target, with the semantics of Open3D's registration_icp +
+ * TransformationEstimationPointToPoint: pass j pairs each source point (under the current T) with its nearest target point
+ * within max_correspondence_distance; stop after pass j if j >= 1 and |d fitness| < relative_fitness and |d rmse| <
+ * relative_rmse, or j == max_iteration; else T <- Umeyama(correspondences) T.  No host synchronisation: 2 *
+ * (max_iteration + 1) launches, later ones return at once after convergence.  init: 3x4 fp64 (device) or NULL.
+ * workspace: s3r_pcl_icp_workspace_bytes() bytes, 16-byte aligned.  out (fp64, 19 + 2 * (max_iteration + 1)):
+ * T of the last pass (4x4 row-major), its fitness, its inlier rmse, the number of passes, then per pass the
+ * correspondence count and the inlier rmse (max_iteration + 1 slots each; unused slots 0). */
+size_t s3r_pcl_icp_workspace_bytes(void);
+int s3r_pcl_icp(const void* source, int is_f64, int64_t ns, const void* target_index, int64_t nt,
+                double max_correspondence_distance, const double* init, int max_iteration, double relative_fitness,
+                double relative_rmse, void* workspace, double* out, void* stream);
+/* x [n] fp64, non-negative -> out[0] mean (fixed-order sum), out[1] exact median (np.median: the mean of the two middle
+ * order statistics for even n), out[2] count of x < threshold.  workspace: s3r_pcl_stats_workspace_bytes() bytes. */
+size_t s3r_pcl_stats_workspace_bytes(void);
+int s3r_pcl_stats(const double* x, int64_t n, double threshold, void* workspace, double* out, void* stream);
+/* out[i] = |a[i] . b[idx[i]]| for a [n, 3], b [*, 3] fp64, idx [n] int64 (eval_recon.py's normal consistency). */
+int s3r_pcl_abs_dot(const double* a, const double* b, const int64_t* idx, int64_t n, double* out, void* stream);
+
 /* ---- model level: the per-frame forward path -------------------------------------------------
  * Packed weights.  The host (spann3r_b200/weights.py) converts the reference state dict ONCE into
  * split-bf16 planes laid out [groups*N, taps*Kc] (K contiguous) plus fp32 biases / LayerNorm params,

@@ -63,6 +63,15 @@ _PROTOS = {
     "s3r_pnp_workspace_bytes": (C.c_size_t, [_i, _i]),
     "s3r_pnp_ransac": (_i, [_vp, _vp, _i, _i64, _i, C.c_double, C.c_double, C.c_double, C.c_double, _f, _i, _i, C.c_uint64,
                             _vp, _vp, _vp, _vp]),
+    "s3r_pcl_index_bytes": (C.c_size_t, [_i64]),
+    "s3r_pcl_index_build": (_i, [_vp, _i, _i64, _vp, _vp, _vp]),
+    "s3r_pcl_nearest": (_i, [_vp, _i64, _vp, _i, _i64, _vp, C.c_double, _vp, _vp, _vp]),
+    "s3r_pcl_normals": (_i, [_vp, _i64, _i, _vp, _vp]),
+    "s3r_pcl_icp_workspace_bytes": (C.c_size_t, []),
+    "s3r_pcl_icp": (_i, [_vp, _i, _i64, _vp, _i64, C.c_double, _vp, _i, C.c_double, C.c_double, _vp, _vp, _vp]),
+    "s3r_pcl_stats_workspace_bytes": (C.c_size_t, []),
+    "s3r_pcl_stats": (_i, [_vp, _i64, C.c_double, _vp, _vp, _vp]),
+    "s3r_pcl_abs_dot": (_i, [_vp, _vp, _vp, _i64, _vp, _vp]),
     "s3r_resample_h_u8": (_i, [_vp, _i64, _i, _i, _vp, _vp, _i, _i, _vp, _vp]),
     "s3r_resample_v_u8_norm": (_i, [_vp, _i, _i, _vp, _vp, _i, _vp, _vp]),
 }

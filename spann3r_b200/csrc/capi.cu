@@ -176,6 +176,33 @@ int s3r_pnp_ransac(const float* pts3d, const float* img_pts, int b, int64_t n, i
                            workspace, out, inlier_mask, S(stream));
 }
 
+size_t s3r_pcl_index_bytes(int64_t n) { return pcl_index_bytes(n); }
+int s3r_pcl_index_build(const void* pts, int is_f64, int64_t n, const double* transform, void* index, void* stream) {
+  return launch_pcl_index_build(pts, is_f64, n, transform, index, S(stream));
+}
+int s3r_pcl_nearest(const void* index, int64_t n, const void* queries, int is_f64, int64_t nq, const double* transform,
+                    double max_dist, double* dist, int64_t* idx, void* stream) {
+  return launch_pcl_nearest(index, n, queries, is_f64, nq, transform, max_dist, dist, reinterpret_cast<long long*>(idx),
+                            S(stream));
+}
+int s3r_pcl_normals(const void* index, int64_t n, int k, double* normals, void* stream) {
+  return launch_pcl_normals(index, n, k, normals, S(stream));
+}
+size_t s3r_pcl_icp_workspace_bytes(void) { return pcl_icp_workspace_bytes(); }
+int s3r_pcl_icp(const void* source, int is_f64, int64_t ns, const void* target_index, int64_t nt,
+                double max_correspondence_distance, const double* init, int max_iteration, double relative_fitness,
+                double relative_rmse, void* workspace, double* out, void* stream) {
+  return launch_pcl_icp(source, is_f64, ns, target_index, nt, max_correspondence_distance, init, max_iteration,
+                        relative_fitness, relative_rmse, workspace, out, S(stream));
+}
+size_t s3r_pcl_stats_workspace_bytes(void) { return pcl_stats_workspace_bytes(); }
+int s3r_pcl_stats(const double* x, int64_t n, double threshold, void* workspace, double* out, void* stream) {
+  return launch_pcl_stats(x, n, threshold, workspace, out, S(stream));
+}
+int s3r_pcl_abs_dot(const double* a, const double* b, const int64_t* idx, int64_t n, double* out, void* stream) {
+  return launch_pcl_abs_dot(a, b, reinterpret_cast<const long long*>(idx), n, out, S(stream));
+}
+
 int s3r_conf_score(const float* conf, int64_t n, float* scratch256, float* out, void* stream) {
   return launch_conf_score(conf, n, scratch256, out, S(stream));
 }

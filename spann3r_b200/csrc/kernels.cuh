@@ -80,6 +80,20 @@ int launch_focal_median(const float* pts3d, int B, int H, int W, float ppx, floa
 
 int launch_conf_score(const float* conf, long long n, float* scratch256, float* out, cudaStream_t st);
 
+// reconstruction metrics (pointcloud.cu): spatial index, 1-NN, k-NN normals, point-to-point ICP, vector statistics
+size_t pcl_index_bytes(long long n);
+int launch_pcl_index_build(const void* pts, int f64, long long n, const double* T, void* index, cudaStream_t st);
+int launch_pcl_nearest(const void* index, long long n, const void* q, int f64, long long nq, const double* T,
+                       double max_dist, double* dist, long long* idx, cudaStream_t st);
+int launch_pcl_normals(const void* index, long long n, int k, double* normals, cudaStream_t st);
+size_t pcl_icp_workspace_bytes();
+int launch_pcl_icp(const void* src, int f64, long long ns, const void* target_index, long long nt, double max_corr,
+                   const double* init, int max_iteration, double rel_fitness, double rel_rmse, void* workspace,
+                   double* out, cudaStream_t st);
+size_t pcl_stats_workspace_bytes();
+int launch_pcl_stats(const double* v, long long n, double threshold, void* workspace, double* out, cudaStream_t st);
+int launch_pcl_abs_dot(const double* a, const double* b, const long long* idx, long long n, double* out, cudaStream_t st);
+
 // fused attention (attention.cu): O = softmax(Q K^T) V per (batch*head), tf32 wgmma, split-bf16 output
 int launch_attention(const float* q, const float* k, const float* vt, int BH, int heads, int nq, int nk, int nk_pad,
                      __nv_bfloat16* o_hi, __nv_bfloat16* o_lo, float* o_f32, long long ldo, cudaStream_t st);

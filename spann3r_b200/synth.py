@@ -154,6 +154,105 @@ def make_pointmap_case(height: int, width: int, focal: float, rvec, tvec, noise:
     return xw.astype(np.float32).reshape(height, width, 3), K
 
 
+def _rotation(rvec):
+    import numpy as np
+    r = np.asarray(rvec, np.float64)
+    th = float(np.linalg.norm(r))
+    if th < 1e-12:
+        return np.eye(3)
+    kx, ky, kz = r / th
+    Kx = np.array([[0, -kz, ky], [kz, 0, -kx], [-ky, kx, 0]])
+    return np.eye(3) + np.sin(th) * Kx + (1 - np.cos(th)) * Kx @ Kx
+
+
+def _surface(kind: str, n: int, rng):
+    """n points on a unit-sized surface: 'plane' (z = 0), 'corner' (three faces of a box), 'curved' (a wavy sheet)."""
+    import numpy as np
+    u = rng.uniform(-1, 1, (n, 2))
+    if kind == "plane":
+        return np.stack((u[:, 0], u[:, 1], np.zeros(n)), -1)
+    if kind == "corner":
+        face = rng.integers(0, 3, n)
+        p = np.zeros((n, 3))
+        for f in range(3):
+            sel = face == f
+            axes = [a for a in range(3) if a != f]
+            p[sel, axes[0]] = (u[sel, 0] + 1) / 2
+            p[sel, axes[1]] = (u[sel, 1] + 1) / 2
+        return p
+    if kind == "curved":
+        return np.stack((u[:, 0], u[:, 1], 0.25 * np.sin(2.5 * u[:, 0]) * np.cos(2.0 * u[:, 1])), -1)
+    raise ValueError(kind)
+
+
+def make_recon_case(surface: str, n_gt: int, n_pred: int, scale: float, noise: float, outlier_frac: float,
+                    dup_frac: float, rvec, tvec, seed: int):
+    """A seeded (ground truth, prediction) pair of clouds for the reconstruction-metric tests (numpy, float32 like the
+    network's pointmaps).  Both sample the same surface independently; the prediction gets Gaussian noise (`noise`,
+    relative to the scene), `outlier_frac` far outliers (up to 50x the scene scale), `dup_frac` exact duplicates of its
+    own points, and is then moved off the ground truth by the rigid x -> R(rvec) x + tvec * scale.  With noise 0 and
+    n_pred == n_gt the prediction is exactly the moved ground truth.  Returns (gt [n_gt, 3], pred [n_pred, 3], T [4, 4]
+    fp64 with gt ~ T pred)."""
+    import numpy as np
+    rng = np.random.default_rng(seed)
+    gt = _surface(surface, n_gt, rng)
+    if noise == 0 and n_pred == n_gt:
+        pred = gt.copy()
+    else:
+        pred = _surface(surface, n_pred, rng) + rng.normal(0, noise, (n_pred, 3))
+    n_out = int(round(outlier_frac * n_pred))
+    if n_out:
+        i = rng.choice(n_pred, n_out, replace=False)
+        pred[i] = rng.uniform(-50, 50, (n_out, 3))
+    n_dup = int(round(dup_frac * n_pred))
+    if n_dup:
+        src = rng.choice(n_pred, n_dup, replace=False)
+        dst = rng.choice(n_pred, n_dup, replace=False)
+        pred[dst] = pred[src]
+    gt, pred = gt * scale, pred * scale
+    R = _rotation(rvec)
+    t = np.asarray(tvec, np.float64) * scale
+    pred = pred @ R.T + t                       # moved off the ground truth; gt ~ R^T (pred - t)
+    T = np.eye(4)
+    T[:3, :3] = R.T
+    T[:3, 3] = -R.T @ t
+    return gt.astype(np.float32), pred.astype(np.float32), T
+
+
+# (surface, n_gt, n_pred, scale, noise, outlier_frac, dup_frac, rvec, tvec, seed): tests/golden/recon_eval.json
+RECON_CASES = [
+    ("plane", 20000, 15000, 1.0, 0.003, 0.01, 0.0, (0.02, -0.01, 0.03), (0.01, 0.02, -0.01), 0),
+    ("curved", 50000, 40000, 0.1, 0.004, 0.03, 0.02, (0.01, 0.02, 0.0), (0.0, 0.01, 0.02), 1),
+    ("curved", 200000, 180000, 100.0, 0.002, 0.05, 0.01, (-0.03, 0.02, 0.01), (0.02, 0.0, 0.01), 2),
+    ("corner", 30000, 30000, 1.0, 0.002, 0.0, 0.05, (0.0, 0.0, 0.02), (0.01, -0.01, 0.0), 3),
+    ("curved", 20000, 20000, 1.0, 0.0, 0.0, 0.0, (0.03, -0.02, 0.01), (0.02, 0.01, -0.02), 4),   # clean: ICP recovers T
+    ("plane", 1, 7, 1.0, 0.01, 0.0, 0.0, (0.0, 0.0, 0.0), (0.0, 0.0, 0.0), 5),
+    ("plane", 5, 2, 100.0, 0.01, 0.0, 0.5, (0.0, 0.0, 0.0), (0.0, 0.0, 0.0), 6),
+]
+
+
+def make_eval_scene(n_frames: int = 50, height: int = 224, width: int = 224, seed: int = 0):
+    """An eval.py-sized scene (generated, never stored): ground-truth pointmaps [F, H, W, 3] of a wavy surface seen by
+    a sweeping camera, the prediction = ground truth + noise + 1 % far outliers, moved by a small rigid transform, and a
+    validity mask [F, H, W] (~95 % true).  float32, like eval.py's pts_all / pts_gt_all / masks_all."""
+    import numpy as np
+    rng = np.random.default_rng(seed)
+    v, u = np.meshgrid(np.linspace(-1, 1, height), np.linspace(-1, 1, width), indexing="ij")
+    gt = np.empty((n_frames, height, width, 3))
+    for f in range(n_frames):
+        x = u * 0.6 + 0.04 * f
+        y = v * 0.6
+        gt[f] = np.stack((x, y, 0.2 * np.sin(3 * x) * np.cos(2 * y) + 1.0), -1)
+    pred = gt + rng.normal(0, 0.003, gt.shape)
+    flat = pred.reshape(-1, 3)
+    n_out = int(0.01 * len(flat))
+    flat[rng.choice(len(flat), n_out, replace=False)] = rng.uniform(-50, 50, (n_out, 3))
+    R = _rotation((0.01, -0.015, 0.02))
+    pred = pred @ R.T + np.array([0.01, -0.02, 0.015])
+    masks = rng.random((n_frames, height, width)) < 0.95
+    return pred.astype(np.float32), gt.astype(np.float32), masks
+
+
 # (height, width, focal, rvec, tvec, noise, outlier_frac, seed): the cases of tests/golden/pnp.json
 PNP_CASES = [
     (384, 512, 400.0, (0.1, -0.2, 0.05), (0.3, -0.1, 0.2), 0.002, 0.0, 1),
