@@ -72,6 +72,25 @@ int s3r_im2col_3x3s2(const void* ihi, const void* ilo, int nb, int h, int w, int
  * croco/models/dpt_block.py:214-215, 246-253. */
 int s3r_upsample2x(const float* x, int nb, int h, int w, int c, float* out, void* hi, void* lo, void* stream);
 
+/* ---- convolution backward (training): the weight gradient of the DPT-head convolutions ---------------------------
+ * dW[n, tap, c] = sum over b, y, x of dY[b, y, x, n] * X[b, y + dy(tap), x + dx(tap), c]  (fp32, split-bf16 x3 products)
+ *   dy planes [nb, h, w, n] (row stride ldy elements), x planes [nb, h, w, kc] (row stride ldx), device pointers,
+ *   16-byte aligned; n, kc, ldy, ldx multiples of 8.  taps = 1 (no shift: 1x1 convs, and ConvTranspose / patch /
+ *   stride-2 wgrads over re-laid-out operands) or 9 (3x3 stride 1 pad 1, tap = 3 (dy + 1) + (dx + 1); reads outside the
+ *   image are zero).  dw fp32 [n, taps, kc] = the packed-weight layout, i.e. the gradient of a Conv2d weight [n, kc, 3, 3]
+ *   permuted (0, 2, 3, 1).  workspace: s3r_conv_wgrad_workspace_bytes(...) bytes (0 = unsupported shape) of caller-owned
+ *   device memory for the per-CTA partials, summed in a fixed order: two calls on the same inputs give bitwise-identical dw.
+ *   Backward of croco/models/dpt_block.py (every Conv2d / ConvTranspose2d), dust3r/patch_embed.py:19-29 and
+ *   spann3r/model.py:310 (pos_patch_embed). */
+size_t s3r_conv_wgrad_workspace_bytes(int nb, int h, int w, int n, int kc, int taps);
+int s3r_conv_wgrad(const void* dy_hi, const void* dy_lo, int64_t ldy, const void* x_hi, const void* x_lo, int64_t ldx,
+                   int nb, int h, int w, int n, int kc, int taps, void* workspace, size_t workspace_bytes, float* dw,
+                   void* stream);
+/* Adjoint of s3r_im2col_3x3s2 in fp32: cols [nb*ho*wo, 9*c] (k = tap*c + channel) -> out [nb, h, w, c], each input pixel
+ * the sum of the (at most 4) taps that read it, in tap order (deterministic).  c a multiple of 8, ho = (h+1)/2,
+ * wo = (w+1)/2.  The input gradient of the stride-2 conv of croco/models/dpt_block.py:396-408 (act_4_postprocess). */
+int s3r_col2im_3x3s2(const float* cols, int nb, int h, int w, int c, int ho, int wo, float* out, void* stream);
+
 /* The tensor-core workhorse: D = A * B^T with fused epilogue (see EPI modes).
  *   A planes [groups*nb, h, w, kc] (a linear layer is h = 1, w = rows), B planes [groups*n, taps, kc],
  *   taps = 1 (linear / 1x1 conv / ConvTranspose with kernel == stride) or 9 (3x3, stride 1, pad 1).

@@ -52,6 +52,9 @@ _PROTOS = {
     "s3r_im2col_patch16": (_i, [_vp, _i64, _i64, _i64, _i64, _i, _i, _i, _vp, _vp, _vp]),
     "s3r_im2col_3x3s2": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
     "s3r_upsample2x": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
+    "s3r_conv_wgrad_workspace_bytes": (C.c_size_t, [_i, _i, _i, _i, _i, _i]),
+    "s3r_conv_wgrad": (_i, [_vp, _vp, _i64, _vp, _vp, _i64, _i, _i, _i, _i, _i, _i, _vp, C.c_size_t, _vp, _vp]),
+    "s3r_col2im_3x3s2": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp]),
     "s3r_gemm": (_i, [C.POINTER(GemmDesc), _vp]),
     "s3r_gemm_tile_n": (_i, [C.POINTER(GemmDesc)]),
     "s3r_attention": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i64, _vp]),
@@ -213,6 +216,37 @@ def linear(x_planes, w_planes, bias=None, act=ACT_NONE, res=None, want_f32=True,
         d.out_hi, d.out_lo, d.ldp = oh.data_ptr(), ol.data_ptr(), N
     gemm(d, dev)
     return out, oh, ol
+
+
+def conv_wgrad(dy_planes, x_planes, taps: int) -> torch.Tensor:
+    """Conv weight gradient over pixels: dy planes [nb, h, w, n], x planes [nb, h, w, kc] (NHWC, contiguous) ->
+    fp32 dW [n, taps, kc] (taps 9: the 3x3 stride-1 pad-1 shifts).  Bitwise reproducible."""
+    yh, yl = dy_planes
+    xh, xl = x_planes
+    nb, h, w, n = yh.shape
+    kc = xh.shape[-1]
+    assert tuple(xh.shape[:3]) == (nb, h, w) and yh.is_contiguous() and xh.is_contiguous(), (tuple(yh.shape), tuple(xh.shape))
+    L = lib()
+    ws_bytes = L.s3r_conv_wgrad_workspace_bytes(nb, h, w, n, kc, taps)
+    if ws_bytes == 0:
+        raise S3RError(f"s3r_conv_wgrad: unsupported shape nb={nb} h={h} w={w} n={n} kc={kc} taps={taps}")
+    dev = yh.device
+    ws = torch.empty(ws_bytes // 4, dtype=torch.float32, device=dev)
+    dw = torch.empty((n, taps, kc), dtype=torch.float32, device=dev)
+    with on_device(dev):
+        check(L.s3r_conv_wgrad(ptr(yh), ptr(yl), n, ptr(xh), ptr(xl), kc, nb, h, w, n, kc, taps, ptr(ws), ws_bytes, ptr(dw),
+                               stream_ptr(dev)), "s3r_conv_wgrad")
+    return dw
+
+
+def col2im_3x3s2(cols: torch.Tensor, nb: int, h: int, w: int, c: int) -> torch.Tensor:
+    """Adjoint of s3r_im2col_3x3s2: fp32 cols [nb*ho*wo, 9*c] -> fp32 [nb, h, w, c]."""
+    assert cols.dtype == torch.float32 and cols.is_cuda and cols.is_contiguous()
+    out = torch.empty((nb, h, w, c), dtype=torch.float32, device=cols.device)
+    with on_device(cols):
+        check(lib().s3r_col2im_3x3s2(ptr(cols), nb, h, w, c, (h + 1) // 2, (w + 1) // 2, ptr(out), stream_ptr(cols.device)),
+              "s3r_col2im_3x3s2")
+    return out
 
 
 def conf_score(conf: torch.Tensor) -> torch.Tensor:

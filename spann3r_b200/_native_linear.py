@@ -1,12 +1,14 @@
-"""`nn.Linear` forward AND backward on the wgmma GEMM engine -- the first native piece of the training backward
-(SURVEY.md §8f rank 1).
+"""`nn.Linear` forward AND backward on the wgmma GEMM engine -- part of the native training backward (SURVEY.md §8f rank 1;
+the convolutions are `_native_conv.py`).
 
 `_recompute.py` (the PyTorch recompute that `train.py` differentiates) routes every Linear through `linear()` below.  With the
 switch off (default) that is `F.linear` and PyTorch autograd.  With it on, the three GEMMs of a Linear -- y = x W^T + b in the
 recompute, dx = dy W (dgrad) and dW = dy^T x (wgrad) in the backward -- run as split-bf16 (`bf16x3`, ~fp32-accurate) launches of
 `s3r_gemm` through the C ABI: the same `gemm_bf16x3_kernel` the forward path uses, operands re-laid-out by
-plain data movement (transpose, zero-pad of the contraction to a multiple of 8, split into planes).  Linears carry ~85 % of the
-backward's FLOPs; attention, LayerNorm, GELU, the DPT convolutions and the elementwise glue remain PyTorch autograd.
+plain data movement (transpose, zero-pad of the contraction to a multiple of 8, split into planes).  Linears carry about
+70 % of the FLOPs (BASELINE.md §3 at 224 x 224: ~2.3 of ~3.26 TFLOP per 10-frame sequence forward), the DPT-head
+convolutions about 26 % (`_native_conv.py`, its own switch); attention, LayerNorm, GELU and the elementwise glue remain
+PyTorch autograd.
 
 Enable with `spann3r_b200.train.set_native_linear(True)` or `S3R_TRAIN_NATIVE_LINEAR=1`.  CUDA tensors only; on the CPU (tests of
 the recompute against the oracle) the call is `F.linear`.

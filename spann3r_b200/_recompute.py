@@ -1,10 +1,13 @@
 """PyTorch RECOMPUTE of the four engine stages -- used ONLY by the backward pass of training mode (`train.py`).
 
 This is NOT a forward path: `Spann3R.forward` always runs the sm_90a kernels (training mode included), and nothing here
-is reachable from eval-mode code.  The native dgrad / wgrad kernels of SURVEY.md §8f rank 1 are not written yet; until
-they are, `torch.autograd.Function.backward` of every stage re-evaluates that stage with these differentiable
-restatements (activation checkpointing at stage granularity) and lets PyTorch autograd produce the gradients -- labelled
-"PyTorch recompute backward" wherever a number from it is reported.  Each function cites the reference lines it restates
+is reachable from eval-mode code.  `torch.autograd.Function.backward` of every stage re-evaluates that stage with these
+differentiable restatements (activation checkpointing at stage granularity) and lets autograd produce the gradients --
+labelled "PyTorch recompute backward" wherever a number from it is reported.  Two switches put the GEMM-shaped ops of the
+recompute and of its backward on the library's kernels: every Linear goes through `_lin` (`_native_linear`,
+`train.set_native_linear`), every convolution through `_conv` / `_convT` (`_native_conv`, `train.set_native_conv`).  Both
+are off by default.  Attention, the memory read, LayerNorm, GELU, the upsample, ReLU and the elementwise glue stay PyTorch
+autograd, as do `head.4` (128 -> 4 channels) and anything on the CPU.  Each function cites the reference lines it restates
 (paths relative to the reference root); `tests/test_train_cpu.py` pins them to the oracle on the CPU.
 
 P: dict parameter name (the reference's state-dict keys) -> tensor.
@@ -14,7 +17,7 @@ from __future__ import annotations
 import torch
 import torch.nn.functional as F
 
-from . import _native_linear
+from . import _native_conv, _native_linear
 
 ENC_HEADS, DEC_HEADS, VAL_HEADS = 16, 12, 16
 
@@ -22,6 +25,15 @@ ENC_HEADS, DEC_HEADS, VAL_HEADS = 16, 12, 16
 def _lin(P, n, x):
     # F.linear + PyTorch autograd by default; with the switch on, forward / dgrad / wgrad on the wgmma GEMM engine
     return _native_linear.linear(x, P[n + ".weight"], P[n + ".bias"])
+
+
+def _conv(P, n, x, stride=1, padding=0, bias=True):
+    # F.conv2d + PyTorch autograd by default; with the switch on, forward / dgrad on the GEMM engine, wgrad on s3r_conv_wgrad
+    return _native_conv.conv2d(x, P[n + ".weight"], P[n + ".bias"] if bias else None, stride, padding)
+
+
+def _convT(P, n, x, stride):
+    return _native_conv.conv_transpose2d(x, P[n + ".weight"], P[n + ".bias"], stride)
 
 
 def _ln(P, n, x, eps):
@@ -100,7 +112,7 @@ def _dec_block(P, n, x, y, cs):
 # ------------------------------------------------------------------------------------------------ stages
 def encode(P, img):
     """dust3r/model.py:131-154 + dust3r/patch_embed.py:19-29: img [n, 3, H, W] -> [n, N, 1024]."""
-    x = F.conv2d(img, P["dust3r.patch_embed.proj.weight"], P["dust3r.patch_embed.proj.bias"], stride=16)
+    x = _conv(P, "dust3r.patch_embed.proj", img, stride=16)
     gh, gw = x.shape[-2:]
     cs = _rope_cs(gh, gw, img.device)
     x = x.flatten(2).transpose(1, 2)
@@ -122,8 +134,8 @@ def memory_read(P, feat, mem_k, mem_v, keep_scale=None):
 
 def _rcu(P, n, x):
     """ResidualConvUnit_custom, croco/models/dpt_block.py:121-142."""
-    o = F.conv2d(F.relu(x), P[n + ".conv1.weight"], P[n + ".conv1.bias"], padding=1)
-    o = F.conv2d(F.relu(o), P[n + ".conv2.weight"], P[n + ".conv2.bias"], padding=1)
+    o = _conv(P, n + ".conv1", F.relu(x), padding=1)
+    o = _conv(P, n + ".conv2", F.relu(o), padding=1)
     return o + x
 
 
@@ -132,29 +144,26 @@ def _fusion(P, n, path, skip=None):
     o = path if skip is None else path + _rcu(P, n + ".resConfUnit1", skip)
     o = _rcu(P, n + ".resConfUnit2", o)
     o = F.interpolate(o, scale_factor=2, mode="bilinear", align_corners=True)
-    return F.conv2d(o, P[n + ".out_conv.weight"], P[n + ".out_conv.bias"])
+    return _conv(P, n + ".out_conv", o)
 
 
 def _dpt(P, p, hooks, gh, gw):
     """DPTOutputAdapter_fix.forward, dust3r/heads/dpt_head.py:34-65 + postprocess.py:10-58 -> (pts3d [B,H,W,3], conf)."""
     L = [t.view(t.shape[0], gh, gw, t.shape[-1]).permute(0, 3, 1, 2) for t in hooks]
     ap = p + ".act_postprocess"
-    l0 = F.conv_transpose2d(F.conv2d(L[0], P[ap + ".0.0.weight"], P[ap + ".0.0.bias"]), P[ap + ".0.1.weight"],
-                            P[ap + ".0.1.bias"], stride=4)
-    l1 = F.conv_transpose2d(F.conv2d(L[1], P[ap + ".1.0.weight"], P[ap + ".1.0.bias"]), P[ap + ".1.1.weight"],
-                            P[ap + ".1.1.bias"], stride=2)
-    l2 = F.conv2d(L[2], P[ap + ".2.0.weight"], P[ap + ".2.0.bias"])
-    l3 = F.conv2d(F.conv2d(L[3], P[ap + ".3.0.weight"], P[ap + ".3.0.bias"]), P[ap + ".3.1.weight"], P[ap + ".3.1.bias"],
-                  stride=2, padding=1)
-    ls = [F.conv2d(t, P[p + f".scratch.layer_rn.{i}.weight"], None, padding=1) for i, t in enumerate((l0, l1, l2, l3))]
+    l0 = _convT(P, ap + ".0.1", _conv(P, ap + ".0.0", L[0]), stride=4)
+    l1 = _convT(P, ap + ".1.1", _conv(P, ap + ".1.0", L[1]), stride=2)
+    l2 = _conv(P, ap + ".2.0", L[2])
+    l3 = _conv(P, ap + ".3.1", _conv(P, ap + ".3.0", L[3]), stride=2, padding=1)
+    ls = [_conv(P, p + f".scratch.layer_rn.{i}", t, padding=1, bias=False) for i, t in enumerate((l0, l1, l2, l3))]
     path = _fusion(P, p + ".scratch.refinenet4", ls[3])[:, :, : ls[2].shape[2], : ls[2].shape[3]]
     path = _fusion(P, p + ".scratch.refinenet3", path, ls[2])
     path = _fusion(P, p + ".scratch.refinenet2", path, ls[1])
     path = _fusion(P, p + ".scratch.refinenet1", path, ls[0])
-    o = F.conv2d(path, P[p + ".head.0.weight"], P[p + ".head.0.bias"], padding=1)
+    o = _conv(P, p + ".head.0", path, padding=1)
     o = F.interpolate(o, scale_factor=2, mode="bilinear", align_corners=True)
-    o = F.relu(F.conv2d(o, P[p + ".head.2.weight"], P[p + ".head.2.bias"], padding=1))
-    o = F.conv2d(o, P[p + ".head.4.weight"], P[p + ".head.4.bias"]).permute(0, 2, 3, 1)
+    o = F.relu(_conv(P, p + ".head.2", o, padding=1))
+    o = _conv(P, p + ".head.4", o).permute(0, 2, 3, 1)
     xyz = o[..., :3]
     d = xyz.norm(dim=-1, keepdim=True)
     return xyz / d.clip(min=1e-8) * torch.expm1(d), 1 + o[..., 3].exp()
@@ -186,7 +195,7 @@ def step(P, feat_fuse, feat1, feat2, H, W):
 
 def value(P, pts3d, feat_k1, rope: bool):
     """spann3r/model.py:305-320 encode_cur_value (+ `cur_v + feat_k1`, :519-521): pts3d [B, H, W, 3] -> [B, N, 1024]."""
-    x = F.conv2d(pts3d.permute(0, 3, 1, 2), P["pos_patch_embed.proj.weight"], P["pos_patch_embed.proj.bias"], stride=16)
+    x = _conv(P, "pos_patch_embed.proj", pts3d.permute(0, 3, 1, 2), stride=16)
     gh, gw = x.shape[-2:]
     cs = _rope_cs(gh, gw, x.device) if rope else None
     x = x.flatten(2).transpose(1, 2)

@@ -70,6 +70,19 @@ int s3r_upsample2x(const float* x, int nb, int h, int w, int c, float* out, void
   return launch_upsample2x(x, nb, h, w, c, out, B(hi), B(lo), S(stream));
 }
 
+size_t s3r_conv_wgrad_workspace_bytes(int nb, int h, int w, int n, int kc, int taps) {
+  return conv_wgrad_workspace_bytes(nb, h, w, n, kc, taps);
+}
+int s3r_conv_wgrad(const void* dy_hi, const void* dy_lo, int64_t ldy, const void* x_hi, const void* x_lo, int64_t ldx,
+                   int nb, int h, int w, int n, int kc, int taps, void* workspace, size_t workspace_bytes, float* dw,
+                   void* stream) {
+  return launch_conv_wgrad(B(dy_hi), B(dy_lo), ldy, B(x_hi), B(x_lo), ldx, nb, h, w, n, kc, taps, workspace,
+                           workspace_bytes, dw, S(stream));
+}
+int s3r_col2im_3x3s2(const float* cols, int nb, int h, int w, int c, int ho, int wo, float* out, void* stream) {
+  return launch_col2im_3x3s2(cols, nb, h, w, c, ho, wo, out, S(stream));
+}
+
 static int fill_plan(const s3r_gemm_desc* d, GemmPlan* plan) {
   if (d->epi == S3R_EPI_HEADTAIL && d->n != 128) {
     set_error("s3r_gemm: EPI_HEADTAIL needs n == 128");

@@ -7,9 +7,12 @@ What is native and what is not (said once, here):
   training-mode branches -- `attn_thresh=0` (no cut / renormalisation in the memory read, :474), `mem_dropout` on the
   attention weights (:167-168; Philox mask, reproducible: `s3r_engine_memory_read_train`), ungated `add_mem` (:518-519).
   The packed weights are refreshed in place from the (optimizer-updated) parameters at the start of every forward.
-* BACKWARD: **PyTorch recompute** -- each stage is an `autograd.Function` that saves its inputs and, in `backward`,
-  re-evaluates the stage with the differentiable restatement in `_recompute.py` and calls `torch.autograd.grad`.  The
-  native dgrad / wgrad kernels are the next step of this row; until they exist, backward time is eager PyTorch.
+* BACKWARD: **recompute** -- each stage is an `autograd.Function` that saves its inputs and, in `backward`,
+  re-evaluates the stage with the differentiable restatement in `_recompute.py` and calls `torch.autograd.grad`.  By
+  default that is eager PyTorch throughout.  `set_native_linear(True)` runs every Linear's recompute, dgrad and wgrad on
+  the split-bf16 GEMM engine; `set_native_conv(True)` does the same for the convolutions of the DPT heads and the two patch
+  embeddings (wgrad on `s3r_conv_wgrad`).  The two switches are independent and combine.  Attention, the memory read,
+  LayerNorm, GELU, the upsample, ReLU and the elementwise glue stay PyTorch autograd either way.
   Gradients reach the `nn.Parameter`s through the Function's parameter inputs, so `DistributedDataParallel`
   (`spann3r/training.py:322-325`) all-reduces them over NCCL like the reference's.
 
@@ -79,6 +82,13 @@ def set_native_linear(on: bool = True):
     instead of `F.linear` + PyTorch autograd."""
     from . import _native_linear
     _native_linear.ENABLED = bool(on)
+
+
+def set_native_conv(on: bool = True):
+    """Run the convolutions of the backward (recompute forward, dgrad, wgrad) on the library's kernels (`_native_conv.py`)
+    instead of `F.conv2d` / `F.conv_transpose2d` + PyTorch autograd.  Independent of `set_native_linear`."""
+    from . import _native_conv
+    _native_conv.ENABLED = bool(on)
 
 
 def _apply(native, torch_fn, names, params, *acts):
