@@ -270,6 +270,18 @@ typedef struct s3r_model_w {
   s3r_ln norm_q, norm_k, norm_v;
   const float* rope_cs;            /* [rope_maxpos, 16, 2] (cos, sin), models/pos_embed.py:120-129 */
   int rope_maxpos;
+  /* Width of the value encoder (spann3r/model.py:225).  0 or 1024: the default encoder (pos_patch_embed on the pointmap,
+   * 16 heads of 64).  768: Spann3R(use_feat=True), fed with head 1's last decoder tokens, 16 heads of 48; pos_patch_embed
+   * is unused.  Its blocks are packed with every 48-wide head in a 64-wide slot, zeros in the padding: head h, half
+   * s (y / x), in-half index i < 24 -> column 64 h + 32 s + (i < 12 ? i : 16 + (i - 12)) of q, k and v, so
+   *   qkv  = planes [3 * 1024, 768] (zero rows, zero bias and cs there; norm1 folded as usual),
+   *   proj = planes [768, 1024] (zero columns); fc1, fc2, value_norm, value_out are ordinary 768-wide layers.
+   * A padding column of q / k / v is exactly 0, adds exactly 0 to Q K^T and to the output, so the result is the
+   * 48-wide attention's. */
+  int value_dim;
+  /* value_dim == 768: the (cos, sin) table of the value blocks' RoPE, [rope_maxpos, 16, 2]; entry j < 12 has angle
+   * pos * 100^(-j/12) (models/pos_embed.py:120-129 with D = 24), entries 12..15 are (1, 0) and rotate the zero pairs */
+  const float* rope_cs_v;
 } s3r_model_w;
 
 /* The spatial-memory bank of one batch of sequences (spann3r/model.py:11-95), caller-owned buffers.
@@ -303,9 +315,16 @@ int s3r_engine_heads(s3r_engine* e, float* pts, float* conf, void* stream);
  *   S3R_VALUE_PTS_TRANSPOSED  portrait frame (H > W): the reference's landscape wrapper (dust3r/utils/misc.py:66-94,
  *                             landscape_only=True at spann3r/model.py:222) gives the value encoder the map with
  *                             axes 1, 2 swapped; read it that way (patch grid W/16 x H/16), no copy
- *   S3R_VALUE_ROPE            Spann3R(mem_pos_enc=True): RoPE inside the value encoder's blocks (spann3r/model.py:231) */
+ *   S3R_VALUE_ROPE            Spann3R(mem_pos_enc=True): RoPE inside the value encoder's blocks (spann3r/model.py:231)
+ *   S3R_VALUE_DEC_TOKENS      Spann3R(use_feat=True), required by and only valid on a value_dim == 768 engine
+ *                             (spann3r/model.py:312-314): the first pointer is dec1[-1] = dec_norm of head 1's last
+ *                             decoder layer, [B, N, 768] fp32, or NULL for the engine's own copy from its last
+ *                             s3r_engine_decode.  Positions are the frame's own patch grid (no transposition: together
+ *                             with S3R_VALUE_PTS_TRANSPOSED it is an error).
+ * Flag / width errors are reported before any CUDA call. */
 #define S3R_VALUE_PTS_TRANSPOSED 1
 #define S3R_VALUE_ROPE 2
+#define S3R_VALUE_DEC_TOKENS 4
 int s3r_engine_value(s3r_engine* e, const float* pts3d, const float* feat_k1, int flags, float* out, void* stream);
 /* spann3r/model.py:145-183 memory_read (eval: thresh = 5e-4; 0 disables): out = attn.V + feat; bank.attn += colsum */
 int s3r_engine_memory_read(s3r_engine* e, const s3r_bank* bank, const float* feat, float thresh, float* out,

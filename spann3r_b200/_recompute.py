@@ -40,10 +40,11 @@ def _ln(P, n, x, eps):
     return F.layer_norm(x, x.shape[-1:], P[n + ".weight"], P[n + ".bias"], eps)
 
 
-def _rope_cs(gh: int, gw: int, device, base: float = 100.0):
-    """cos / sin of pos * base^(-j/16), j < 16 (croco/models/pos_embed.py:120-129, D = 32), for the row-major patch grid:
-    returns (cos_y, sin_y, cos_x, sin_x), each [gh*gw, 16]."""
-    inv = 1.0 / (base ** (torch.arange(0, 32, 2, device=device).float() / 32))
+def _rope_cs(gh: int, gw: int, device, base: float = 100.0, head_dim: int = 64):
+    """cos / sin of pos * base^(-j/P), j < P = head_dim / 4 (croco/models/pos_embed.py:120-129, D = head_dim / 2), for the
+    row-major patch grid: returns (cos_y, sin_y, cos_x, sin_x), each [gh*gw, P]."""
+    D = head_dim // 2
+    inv = 1.0 / (base ** (torch.arange(0, D, 2, device=device).float() / D))
     ys = torch.arange(gh, device=device).float().repeat_interleave(gw)
     xs = torch.arange(gw, device=device).float().repeat(gh)
     fy, fx = ys[:, None] * inv[None], xs[:, None] * inv[None]
@@ -51,13 +52,14 @@ def _rope_cs(gh: int, gw: int, device, base: float = 100.0):
 
 
 def _rope(t, cs):
-    """2-D RoPE on [B, heads, N, 64] (pos_embed.py:131-159): the head dim is [y half | x half], each half 16 (u, v) pairs
-    (j, j + 16) rotated by its position's angle."""
+    """2-D RoPE on [B, heads, N, dh] (pos_embed.py:131-159): the head dim is [y half | x half], each half dh / 4 (u, v)
+    pairs (j, j + dh / 4) rotated by its position's angle."""
     cy, sy, cx, sx = cs
-    y, x = t[..., :32], t[..., 32:]
+    half = t.shape[-1] // 2
+    y, x = t[..., :half], t[..., half:]
 
     def rot(h, c, s):
-        u, v = h[..., :16], h[..., 16:]
+        u, v = h[..., : half // 2], h[..., half // 2:]
         return torch.cat((u * c - v * s, v * c + u * s), dim=-1)
     return torch.cat((rot(y, cy, sy), rot(x, cx, sx)), dim=-1)
 
@@ -169,9 +171,10 @@ def _dpt(P, p, hooks, gh, gw):
     return xyz / d.clip(min=1e-8) * torch.expm1(d), 1 + o[..., 3].exp()
 
 
-def step(P, feat_fuse, feat1, feat2, H, W):
+def step(P, feat_fuse, feat1, feat2, H, W, dec_tokens: bool = False):
     """One frame step between the memory read and the memory write: the twin decoder (dust3r/model.py:186-205), the two
-    key heads (spann3r/model.py:299-303) and the two DPT heads.  Returns (feat_k1, feat_k2, pts [2,B,H,W,3], conf)."""
+    key heads (spann3r/model.py:299-303) and the two DPT heads.  Returns (feat_k1, feat_k2, pts [2,B,H,W,3], conf), and
+    with dec_tokens (use_feat) also dec1[-1] = dec_norm of stream 1's last layer, the value encoder's input."""
     gh, gw = H // 16, W // 16
     cs = _rope_cs(gh, gw, feat1.device)
     a, b = _lin(P, "dust3r.decoder_embed", feat_fuse), _lin(P, "dust3r.decoder_embed", feat2)
@@ -190,6 +193,8 @@ def step(P, feat_fuse, feat1, feat2, H, W):
     k1, k2 = key_head("attn_head_1", feat1, a), key_head("attn_head_2", feat2, b)
     p1, c1 = _dpt(P, "dust3r.downstream_head1.dpt", h1, gh, gw)
     p2, c2 = _dpt(P, "dust3r.downstream_head2.dpt", h2, gh, gw)
+    if dec_tokens:
+        return k1, k2, torch.stack((p1, p2)), torch.stack((c1, c2)), a
     return k1, k2, torch.stack((p1, p2)), torch.stack((c1, c2))
 
 
@@ -199,6 +204,16 @@ def value(P, pts3d, feat_k1, rope: bool):
     gh, gw = x.shape[-2:]
     cs = _rope_cs(gh, gw, x.device) if rope else None
     x = x.flatten(2).transpose(1, 2)
+    for i in range(6):
+        x = _block(P, f"value_encoder.{i}", x, VAL_HEADS, cs)
+    return _lin(P, "value_out", _ln(P, "value_norm", x, 1e-6)) + feat_k1
+
+
+def value_tokens(P, dec_last, feat_k1, rope: bool, H: int, W: int):
+    """spann3r/model.py:312-314 with use_feat=True (+ `cur_v + feat_k1`): the 768-wide value encoder (16 heads of 48) on
+    dec1[-1] [B, N, 768], positions = the frame's own (H/16, W/16) patch grid."""
+    x = dec_last
+    cs = _rope_cs(H // 16, W // 16, x.device, head_dim=x.shape[-1] // VAL_HEADS) if rope else None
     for i in range(6):
         x = _block(P, f"value_encoder.{i}", x, VAL_HEADS, cs)
     return _lin(P, "value_out", _ln(P, "value_norm", x, 1e-6)) + feat_k1

@@ -47,6 +47,55 @@ int launch_split(const float* x, long long ldx, __nv_bfloat16* hi, __nv_bfloat16
 }
 
 // ------------------------------------------------------------------------------------------------
+// fp32 [rows, C] -> split-bf16 planes [rows, C] + LayerNorm chunk statistics [rows, C/32] float2 (sum, sum of squares of
+// each 32-column chunk), optionally an fp32 copy [rows, C].  The same statistics the GEMM epilogue's producer side
+// (stats_out) writes, for a residual stream that enters a block from outside the GEMM chain -- the use_feat value
+// encoder's input, dec_norm tokens of the decoder.  One warp per row; 8 lanes hold one chunk (4 columns each) and reduce
+// it in the epilogue's order.  C % 128 == 0, so every lane of a warp walks the same number of iterations.
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) split_stats_kernel(const float* __restrict__ x, long long ldx, long long rows, int C,
+                                                          float* __restrict__ out, long long ldo, __nv_bfloat16* __restrict__ hi,
+                                                          __nv_bfloat16* __restrict__ lo, long long ldp,
+                                                          float2* __restrict__ stats) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const long long row = blockIdx.x * (long long)(blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (row >= rows) return;
+  const int lane = threadIdx.x & 31;
+  const int nchunk = C >> 5;
+  for (int c = lane * 4; c < C; c += 128) {
+    const float4 v = *reinterpret_cast<const float4*>(x + row * ldx + c);
+    float s1 = (v.x + v.y) + (v.z + v.w);
+    float s2 = fmaf(v.x, v.x, fmaf(v.y, v.y, fmaf(v.z, v.z, v.w * v.w)));
+#pragma unroll
+    for (int o = 1; o < 8; o <<= 1) {
+      s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+      s2 += __shfl_xor_sync(0xffffffffu, s2, o);
+    }
+    if ((lane & 7) == 0) stats[row * nchunk + (c >> 5)] = make_float2(s1, s2);
+    if (out) *reinterpret_cast<float4*>(out + row * ldo + c) = v;
+    __nv_bfloat16 h0, l0, h1, l1, h2, l2, h3, l3;
+    split_bf16(v.x, h0, l0); split_bf16(v.y, h1, l1); split_bf16(v.z, h2, l2); split_bf16(v.w, h3, l3);
+    const long long o = row * ldp + c;
+    *reinterpret_cast<uint2*>(hi + o) = make_uint2(pack_bf16(h0, h1), pack_bf16(h2, h3));
+    *reinterpret_cast<uint2*>(lo + o) = make_uint2(pack_bf16(l0, l1), pack_bf16(l2, l3));
+  }
+}
+
+int launch_split_stats(const float* x, long long ldx, long long rows, int C, float* out, long long ldo, __nv_bfloat16* hi,
+                       __nv_bfloat16* lo, long long ldp, float2* stats, cudaStream_t st) {
+  if (C <= 0 || C % 128 || C > 1024 || ldx % 4 || ldp % 4 || (out && ldo % 4)) {
+    set_error("split_stats: need C a multiple of 128 (<= 1024) and row strides multiples of 4 (C=%d)", C);
+    return -1;
+  }
+  if (rows == 0) return 0;
+  const int wpb = 8;
+  launch_pdl(split_stats_kernel, dim3((unsigned)((rows + wpb - 1) / wpb)), dim3(wpb * 32), 0, st, x, ldx, rows, C, out, ldo,
+             hi, lo, ldp, stats);
+  return cudaGetLastError() == cudaSuccess ? 0 : -6;
+}
+
+// ------------------------------------------------------------------------------------------------
 // LayerNorm over the last dim (nn.LayerNorm, eps 1e-6 in the ViT blocks croco.py:34, 1e-5 for
 // norm_q/k/v spann3r/model.py:245-247).  One warp per row, the row lives in registers, two-pass
 // mean / variance in fp32.  Emits fp32 and/or split-bf16 planes.  `swap_rows` > 0 writes row r of

@@ -225,28 +225,38 @@ struct s3r_engine {
 
   // ---- ViT blocks on X [nimg*N, D] (in place).  croco/models/blocks.py:127-130 ----
   // LayerNorms are folded into the GEMM that consumes them (s3r_lin.cs): P holds the planes of the block input x and St1
-  // its per-row chunk statistics (written by whichever GEMM produced x).  No LayerNorm kernel runs inside a block.
+  // its per-row chunk statistics (written by whichever GEMM -- or split_stats launch -- produced x).  No LayerNorm kernel
+  // runs inside a block.  D is the model width, Da the attention width (heads x 64).  They are equal except in the
+  // use_feat value encoder (D = 768; 16 heads of 48 packed into 64-wide slots, so Da = 1024), whose q / k / v and
+  // attention output carry zero columns.  cs = the RoPE (cos, sin) table of these blocks, q_scale = head_dim^-0.5 of the
+  // unpadded heads.
   // Launch structure per block: [qkv of block 0] then, per block, attention, proj, fc1, fc2 and the NEXT block's qkv.
-  int vit_qkv(PlanCache& pc, const s3r_block_w& bw, int D, int nimg, bool rope, cudaStream_t st, const int* pos_tab) {
+  struct VitCfg {
+    int D = 1024, Da = 1024;
+    const float* cs = nullptr;   // nullptr = w.rope_cs
+    float q_scale = 0.125f;
+  };
+  int vit_qkv(PlanCache& pc, const s3r_block_w& bw, const VitCfg& c, int nimg, bool rope, cudaStream_t st,
+              const int* pos_tab) {
     const int rows = nimg * N;
-    Geom g; g.W = rows; g.Kc = D; g.N = 3 * D;
-    Epi e; e.epi = EPI_QKV; e.bias = bw.qkv.b; e.q_C = D; e.q_role_base = 0; e.q_ntok = N; e.q_ntok_pad = Npad;
-    e.q_rope = rope ? 1 : 0; e.q_nb = nimg; e.q_pos = pos_tab; e.q_cs = (const float2*)w.rope_cs;
-    e.q_out = Qb; e.k_out = Kb; e.vt_out = Vtb; e.q_scale = 0.125f;
-    e.ln_stats = St1; e.ln_np = D / 32; e.ln_eps = 1e-6f; e.ln_cs = bw.qkv.cs;                       // norm1
+    Geom g; g.W = rows; g.Kc = c.D; g.N = 3 * c.Da;
+    Epi e; e.epi = EPI_QKV; e.bias = bw.qkv.b; e.q_C = c.Da; e.q_role_base = 0; e.q_ntok = N; e.q_ntok_pad = Npad;
+    e.q_rope = rope ? 1 : 0; e.q_nb = nimg; e.q_pos = pos_tab; e.q_cs = (const float2*)(c.cs ? c.cs : w.rope_cs);
+    e.q_out = Qb; e.k_out = Kb; e.vt_out = Vtb; e.q_scale = c.q_scale;
+    e.ln_stats = St1; e.ln_np = c.D / 32; e.ln_eps = 1e-6f; e.ln_cs = bw.qkv.cs;                       // norm1
     return gemm(pc, P, WP(bw.qkv.w), g, e, st);
   }
-  int vit_blocks(PlanCache& pc, const s3r_block_w* blocks, int depth, int D, int nimg, bool rope, float* Xp, cudaStream_t st,
-                 const int* pos_tab = nullptr) {
-    const int rows = nimg * N, heads = D / 64;
+  int vit_blocks(PlanCache& pc, const s3r_block_w* blocks, int depth, const VitCfg& c, int nimg, bool rope, float* Xp,
+                 cudaStream_t st, const int* pos_tab = nullptr) {
+    const int D = c.D, rows = nimg * N, heads = c.Da / 64;
     if (!pos_tab) pos_tab = pos;
     int r;
-    if ((r = vit_qkv(pc, blocks[0], D, nimg, rope, st, pos_tab))) return r;
+    if ((r = vit_qkv(pc, blocks[0], c, nimg, rope, st, pos_tab))) return r;
     for (int l = 0; l < depth; ++l) {
       const s3r_block_w& bw = blocks[l];
-      if ((r = attention(pc, Qb, Kb, Vtb, nimg * heads, heads, N, N, AO, D, st))) return r;
+      if ((r = attention(pc, Qb, Kb, Vtb, nimg * heads, heads, N, N, AO, c.Da, st))) return r;
       {
-        Geom g; g.W = rows; g.Kc = D; g.N = D;
+        Geom g; g.W = rows; g.Kc = c.Da; g.N = D;
         Epi e; e.bias = bw.proj.b; e.res1 = Xp; e.ldr1 = D; e.out = Xp; e.ldo = D;
         e.op = P2; e.ldp = D; e.stats_out = St2;
         if ((r = gemm(pc, AO, WP(bw.proj.w), g, e, st))) return r;
@@ -263,7 +273,7 @@ struct s3r_engine {
         e.op = P; e.ldp = D; e.stats_out = St1;
         if ((r = gemm(pc, Hb, WP(bw.fc2.w), g, e, st))) return r;
       }
-      if (l + 1 < depth && (r = vit_qkv(pc, blocks[l + 1], D, nimg, rope, st, pos_tab))) return r;
+      if (l + 1 < depth && (r = vit_qkv(pc, blocks[l + 1], c, nimg, rope, st, pos_tab))) return r;
     }
     return 0;
   }
@@ -305,6 +315,14 @@ extern "C" {
 s3r_engine* s3r_engine_create(const s3r_model_w* w, int batch, int height, int width, int max_images) {
   if (!w || batch <= 0 || height % 16 != 0 || width % 16 != 0 || height <= 0 || width <= 0) {
     set_error("s3r_engine_create: need batch > 0 and height, width multiples of 16 (got %d, %dx%d)", batch, height, width);
+    return nullptr;
+  }
+  if (w->value_dim != 0 && w->value_dim != 1024 && w->value_dim != 768) {
+    set_error("s3r_engine_create: value_dim must be 0, 1024 or 768 (got %d)", w->value_dim);
+    return nullptr;
+  }
+  if (w->value_dim == 768 && !w->rope_cs_v) {
+    set_error("s3r_engine_create: value_dim 768 needs the 48-wide RoPE table rope_cs_v");
     return nullptr;
   }
   if (max_images < 2 * batch) max_images = 2 * batch;
@@ -507,7 +525,7 @@ int s3r_engine_encode(s3r_engine* e, const float* img, int nimg, float* feat, vo
     ep.op = e->P; ep.ldp = 1024; ep.stats_out = e->St1;   // block 0's folded norm1 reads these
     if ((r = e->gemm(pc, e->Pim, WP(e->w.patch_embed.w), g, ep, st))) return r;
   }
-  if ((r = e->vit_blocks(pc, e->w.enc, 24, 1024, nimg, true, e->X, st))) return r;
+  if ((r = e->vit_blocks(pc, e->w.enc, 24, s3r_engine::VitCfg(), nimg, true, e->X, st))) return r;
   if ((r = e->ln(e->X, e->w.enc_norm, 0, 0, 1e-6f, rows, 1024, feat, 1024, Planes(), 0, 0, 0, st))) return r;
   pc.end();
   return 0;
@@ -758,43 +776,69 @@ int s3r_engine_heads(s3r_engine* e, float* pts, float* conf, void* stream) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// value encoder: spann3r/model.py:305-320 (pos_patch_embed on pts3d, 6 Blocks without RoPE, value_norm,
-// value_out) + `cur_v + feat_k1` (:519-521) fused as the residual of value_out.
+// value encoder: spann3r/model.py:305-320 (6 Blocks, RoPE with mem_pos_enc, value_norm, value_out) + `cur_v + feat_k1`
+// (:519-521) fused as the residual of value_out.  Default (value_dim 1024): pos_patch_embed on pts3d.  use_feat
+// (value_dim 768): the blocks run on dec1[-1] = dec_norm of head 1's last decoder layer, 16 heads of 48 in 64-wide slots.
 // ------------------------------------------------------------------------------------------------
 int s3r_engine_value(s3r_engine* e, const float* pts3d, const float* feat_k1, int flags, float* out, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
-  S3R_ENGINE_DEVICE(e, "s3r_engine_value");
-  if (flags & ~(S3R_VALUE_PTS_TRANSPOSED | S3R_VALUE_ROPE)) {
+  if (flags & ~(S3R_VALUE_PTS_TRANSPOSED | S3R_VALUE_ROPE | S3R_VALUE_DEC_TOKENS)) {
     set_error("s3r_engine_value: unknown flags 0x%x", flags);
     return -1;
   }
   const bool tr = (flags & S3R_VALUE_PTS_TRANSPOSED) != 0, rope = (flags & S3R_VALUE_ROPE) != 0;
+  const bool tokens = (flags & S3R_VALUE_DEC_TOKENS) != 0;
+  const bool use_feat = e->w.value_dim == 768;
+  if (tokens != use_feat) {
+    set_error(use_feat ? "s3r_engine_value: this engine's value encoder is 768 wide (use_feat); it takes decoder tokens "
+                         "(S3R_VALUE_DEC_TOKENS), not a pointmap"
+                       : "s3r_engine_value: S3R_VALUE_DEC_TOKENS needs a 768-wide value encoder (value_dim 768); this "
+                         "engine's is 1024 wide");
+    return -1;
+  }
+  if (tokens && tr) {
+    set_error("s3r_engine_value: S3R_VALUE_DEC_TOKENS reads the frame's own token grid; S3R_VALUE_PTS_TRANSPOSED does not "
+              "apply to it");
+    return -1;
+  }
+  S3R_ENGINE_DEVICE(e, "s3r_engine_value");
   // the cached plans do not depend on the flags: same launches, shapes and buffers; the flags only pick the im2col
   // strides and the per-call RoPE switch / position table of the qkv epilogue
   PlanCache& pc = e->pc_value;
   pc.begin();
   const int B = e->B;
   const int rows = B * e->N;
+  const int D = use_feat ? 768 : 1024;
   int r;
   ++e->launches;
-  // pts3d is the head's [B, H, W, 3] map: the reference permutes to NCHW first; here the im2col reads it with NHWC
-  // strides.  For a portrait frame the landscape wrapper (dust3r/utils/misc.py:66-94) hands encode_cur_value the
-  // map with axes 1 and 2 swapped, i.e. an image of W rows x H columns: same memory, row / column strides exchanged,
-  // patch grid gw x gh (S3R_VALUE_PTS_TRANSPOSED).
-  const long long srow = (long long)e->W * 3, spx = 3;
-  if ((r = launch_im2col_patch16(pts3d, (long long)e->H * e->W * 3, 1, tr ? spx : srow, tr ? srow : spx, B,
-                                 tr ? e->gw : e->gh, tr ? e->gh : e->gw, e->Pim.hi, e->Pim.lo, st)))
-    return r;
-  {
+  s3r_engine::VitCfg vc;
+  if (use_feat) {
+    // dec1[-1] (NULL: the engine's own dec_norm output of stream 1, D12 rows [0, R)) -> the fp32 residual stream Xv, its
+    // planes P and the chunk statistics St1 that block 0's folded norm1 reads
+    if ((r = launch_split_stats(pts3d ? pts3d : e->D12, 768, rows, 768, e->Xv, 768, e->P.hi, e->P.lo, 768, e->St1, st)))
+      return r;
+    vc.D = 768;
+    vc.Da = 1024;
+    vc.cs = e->w.rope_cs_v;
+    vc.q_scale = 0.14433756729740643f;   // 48^-0.5
+  } else {
+    // pts3d is the head's [B, H, W, 3] map: the reference permutes to NCHW first; here the im2col reads it with NHWC
+    // strides.  For a portrait frame the landscape wrapper (dust3r/utils/misc.py:66-94) hands encode_cur_value the
+    // map with axes 1 and 2 swapped, i.e. an image of W rows x H columns: same memory, row / column strides exchanged,
+    // patch grid gw x gh (S3R_VALUE_PTS_TRANSPOSED).
+    const long long srow = (long long)e->W * 3, spx = 3;
+    if ((r = launch_im2col_patch16(pts3d, (long long)e->H * e->W * 3, 1, tr ? spx : srow, tr ? srow : spx, B,
+                                   tr ? e->gw : e->gh, tr ? e->gh : e->gw, e->Pim.hi, e->Pim.lo, st)))
+      return r;
     Geom g; g.W = rows; g.Kc = 768; g.N = 1024;
     Epi ep; ep.bias = e->w.pos_patch_embed.b; ep.out = e->Xv; ep.ldo = 1024;
     ep.op = e->P; ep.ldp = 1024; ep.stats_out = e->St1;
     if ((r = e->gemm(pc, e->Pim, WP(e->w.pos_patch_embed.w), g, ep, st))) return r;
   }
-  if ((r = e->vit_blocks(pc, e->w.val, 6, 1024, B, rope, e->Xv, st, tr ? e->pos_t : e->pos))) return r;
-  if ((r = e->ln(e->Xv, e->w.value_norm, 0, 0, 1e-6f, rows, 1024, nullptr, 0, e->Pv, 1024, 0, 0, st))) return r;
+  if ((r = e->vit_blocks(pc, e->w.val, 6, vc, B, rope, e->Xv, st, tr ? e->pos_t : e->pos))) return r;
+  if ((r = e->ln(e->Xv, e->w.value_norm, 0, 0, 1e-6f, rows, D, nullptr, 0, e->Pv, D, 0, 0, st))) return r;
   {
-    Geom g; g.W = rows; g.Kc = 1024; g.N = 1024;
+    Geom g; g.W = rows; g.Kc = D; g.N = 1024;
     Epi ep; ep.bias = e->w.value_out.b; ep.res1 = feat_k1; ep.ldr1 = 1024; ep.out = out; ep.ldo = 1024;
     if ((r = e->gemm(pc, e->Pv, WP(e->w.value_out.w), g, ep, st))) return r;
   }

@@ -10,6 +10,9 @@ namespace s3r {
 
 int launch_split(const float* x, long long ldx, __nv_bfloat16* hi, __nv_bfloat16* lo, long long ldp, int col0,
                  long long rows, int C, int relu, cudaStream_t st);
+// fp32 rows -> planes + per-32-column (sum, sum of squares) in the GEMM producer's stats_out layout (+ optional fp32 copy)
+int launch_split_stats(const float* x, long long ldx, long long rows, int C, float* out, long long ldo, __nv_bfloat16* hi,
+                       __nv_bfloat16* lo, long long ldp, float2* stats, cudaStream_t st);
 int launch_layernorm(const float* x, long long ldx, const float* w, const float* b, long long wb_group_stride,
                      long long rows_per_group, float eps, long long rows, int C, float* out, long long ldo,
                      __nv_bfloat16* hi, __nv_bfloat16* lo, long long ldp, int col0, long long swap_rows,

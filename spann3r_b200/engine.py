@@ -1,6 +1,6 @@
 """Host side of the model-level C ABI: weight packing and the `Engine` wrapper.
 
-`PackedWeights` converts a reference-layout state dict (1101 keys, SURVEY.md §8b) ONCE into the
+`PackedWeights` converts a reference-layout state dict (1101 keys, SURVEY.md §8b; 1099 for use_feat) ONCE into the
 split-bf16 planes / fp32 tables of `s3r_model_w` (include/spann3r_b200.h); `Engine` owns one
 `s3r_engine` handle per (batch, height, width) and exposes its stages on torch tensors.
 Everything here is plumbing (pointers, shapes, one-time layout permutes); all arithmetic of the
@@ -60,7 +60,7 @@ class ModelW(C.Structure):
                 ("key_fc1", Lin), ("key_fc2", Lin), ("dpt", DptW),
                 ("pos_patch_embed", Lin), ("val", BlockW * 6), ("value_norm", LN), ("value_out", Lin),
                 ("norm_q", LN), ("norm_k", LN), ("norm_v", LN),
-                ("rope_cs", _vp), ("rope_maxpos", _i)]
+                ("rope_cs", _vp), ("rope_maxpos", _i), ("value_dim", _i), ("rope_cs_v", _vp)]
 
 
 class Bank(C.Structure):
@@ -88,17 +88,50 @@ _lib.register_protos({
 })
 
 ROPE_MAXPOS = 64
-VALUE_PTS_TRANSPOSED, VALUE_ROPE = 1, 2   # include/spann3r_b200.h: flags of s3r_engine_value
+VALUE_PTS_TRANSPOSED, VALUE_ROPE, VALUE_DEC_TOKENS = 1, 2, 4   # include/spann3r_b200.h: flags of s3r_engine_value
 
 
-def rope_cs_table(maxpos: int = ROPE_MAXPOS, base: float = 100.0) -> torch.Tensor:
-    """(cos, sin) of pos * base^(-j/16), j < 16: exactly the fp32 table the reference's PyTorch RoPE2D
-    builds (croco/models/pos_embed.py:120-129 with D = 32), as [maxpos, 16, 2]."""
-    D = 32
+def rope_cs_table(maxpos: int = ROPE_MAXPOS, base: float = 100.0, head_dim: int = 64) -> torch.Tensor:
+    """(cos, sin) of pos * base^(-j/P), j < P = head_dim / 4: exactly the fp32 table the reference's PyTorch RoPE2D
+    builds (croco/models/pos_embed.py:120-129 with D = head_dim / 2), as [maxpos, 16, 2].  The QKV epilogue rotates the
+    pairs (j, j + 16) of each 32-wide half of a 64-wide head slot; for 48-wide heads (P = 12, the use_feat value encoder)
+    entries 12..15 are (1, 0) and leave the zero padding pairs at zero."""
+    D = head_dim // 2
     inv_freq = 1.0 / (base ** (torch.arange(0, D, 2).float() / D))
     t = torch.arange(maxpos, dtype=inv_freq.dtype)
     freqs = torch.einsum("i,j->ij", t, inv_freq)
-    return torch.stack((freqs.cos(), freqs.sin()), dim=-1).contiguous()
+    cs = torch.stack((freqs.cos(), freqs.sin()), dim=-1)
+    if cs.shape[1] < 16:
+        pad = torch.zeros(maxpos, 16 - cs.shape[1], 2)
+        pad[..., 0] = 1.0
+        cs = torch.cat((cs, pad), dim=1)
+    return cs.contiguous()
+
+
+def head_slots(heads: int = 16, head_dim: int = 48) -> torch.Tensor:
+    """Column of every model feature c = h * head_dim + d in the 64-wide head slots the attention kernel runs on:
+    head h, half s (y / x), in-half index i -> 64 h + 32 s + (i < P ? i : 16 + (i - P)), P = head_dim / 4.  Each half's
+    RoPE pairs (i, i + P) land on the epilogue's pairs (j, j + 16); everything else in the slot is zero padding."""
+    half, P = head_dim // 2, head_dim // 4
+    c = torch.arange(heads * head_dim)
+    h, d = c // head_dim, c % head_dim
+    s, i = d // half, d % half
+    return 64 * h + 32 * s + torch.where(i < P, i, 16 + (i - P))
+
+
+def pad_qkv_rows(t: torch.Tensor, slots: torch.Tensor) -> torch.Tensor:
+    """qkv weight [3 C, K] / bias [3 C] -> [3 * 64 heads, K] / [3 * 64 heads] with each role's rows at their slots, zeros
+    elsewhere (any dtype / device)."""
+    C, width = slots.numel(), 64 * ((int(slots.max()) + 64) // 64)
+    out = t.new_zeros((3 * width,) + tuple(t.shape[1:]))
+    idx = torch.cat([r * width + slots for r in range(3)]).to(t.device)
+    return out.index_copy_(0, idx, t.reshape((3 * C,) + tuple(t.shape[1:])))
+
+
+def pad_proj_cols(w: torch.Tensor, slots: torch.Tensor) -> torch.Tensor:
+    """proj weight [N, C] -> [N, 64 * heads] reading the attention output's slot columns, zeros elsewhere."""
+    width = 64 * ((int(slots.max()) + 64) // 64)
+    return w.new_zeros(w.shape[0], width).index_copy_(1, slots.to(w.device), w)
 
 
 def fold_layernorm(w: torch.Tensor, b: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor):
@@ -201,16 +234,22 @@ class PackedWeights:
         n.b = self._f32(torch.stack([self._t(k + ".bias") for k in names]))
         return n
 
-    def _linear(self, names) -> Lin:
-        return self._lin([self._t(k + ".weight") for k in names], [self._t(k + ".bias") for k in names])
+    def _linear(self, names, slots=None) -> Lin:
+        """slots: read the input through the 64-wide head slots (`pad_proj_cols`) -- proj of the use_feat value blocks."""
+        ws = [self._t(k + ".weight") for k in names]
+        if slots is not None:
+            ws = [pad_proj_cols(w, slots) for w in ws]
+        return self._lin(ws, [self._t(k + ".bias") for k in names])
 
-    def _linear_ln(self, names, ln_names) -> Lin:
+    def _linear_ln(self, names, ln_names, slots=None) -> Lin:
         """Linear that follows a LayerNorm, with the LayerNorm folded in (include/spann3r_b200.h, s3r_lin.cs):
         LN(x) W^T + b = rstd (x W'^T - mean cs) + b'  with  W' = W diag(gamma), b' = b + W beta, cs = rowsum(W').
         Exact algebra; cs is summed over the split-bf16 planes the tensor core will actually multiply."""
         ws, bs = [], []
         for k, ln in zip(names, ln_names):
             wf, bf = fold_layernorm(self._t(k + ".weight"), self._t(k + ".bias"), self._t(ln + ".weight"), self._t(ln + ".bias"))
+            if slots is not None:   # qkv of the use_feat value blocks: rows into 64-wide head slots, zero weight / bias / cs
+                wf, bf = pad_qkv_rows(wf, slots), pad_qkv_rows(bf, slots)
             ws.append(wf)
             bs.append(bf)
         l = self._lin(ws, bs)
@@ -225,11 +264,11 @@ class PackedWeights:
         ws = [self._t(k + ".weight").permute(2, 3, 1, 0) for k in names]
         return self._lin([w.reshape(-1, w.shape[-1]) for w in ws], [self._t(k + ".bias") for k in names])
 
-    def _block(self, prefix) -> BlockW:
+    def _block(self, prefix, slots=None) -> BlockW:
         b = BlockW()
         b.norm1 = self._ln([prefix + ".norm1"])
-        b.qkv = self._linear_ln([prefix + ".attn.qkv"], [prefix + ".norm1"])
-        b.proj = self._linear([prefix + ".attn.proj"])
+        b.qkv = self._linear_ln([prefix + ".attn.qkv"], [prefix + ".norm1"], slots)
+        b.proj = self._linear([prefix + ".attn.proj"], slots)
         b.norm2 = self._ln([prefix + ".norm2"])
         b.fc1 = self._linear_ln([prefix + ".mlp.fc1"], [prefix + ".norm2"])
         b.fc2 = self._linear([prefix + ".mlp.fc2"])
@@ -288,14 +327,21 @@ class PackedWeights:
         d.head2 = self._conv3([p + ".head.2" for p in hp])
         d.head4_w = self._f32(torch.stack([self._t(p + ".head.4.weight").reshape(4, 128) for p in hp]))
         d.head4_b = self._f32(torch.stack([self._t(p + ".head.4.bias") for p in hp]))
-        s.pos_patch_embed = self._linear(["pos_patch_embed.proj"])
+        # value encoder: 1024 wide (default), or 768 wide with 48-wide heads (use_feat; no pos_patch_embed), packed into
+        # 64-wide head slots (include/spann3r_b200.h, s3r_model_w.value_dim)
+        s.value_dim = self.value_dim = int(self.sd["value_norm.weight"].shape[0])
+        slots = head_slots(16, self.value_dim // 16) if self.value_dim == 768 else None
+        if slots is None:
+            s.pos_patch_embed = self._linear(["pos_patch_embed.proj"])
         for i in range(6):
-            s.val[i] = self._block(f"value_encoder.{i}")
+            s.val[i] = self._block(f"value_encoder.{i}", slots)
         s.value_norm = self._ln(["value_norm"])
         s.value_out = self._linear(["value_out"])
         s.norm_q, s.norm_k, s.norm_v = self._ln(["norm_q"]), self._ln(["norm_k"]), self._ln(["norm_v"])
         s.rope_cs = self._f32(rope_cs_table())
         s.rope_maxpos = ROPE_MAXPOS
+        if slots is not None:
+            s.rope_cs_v = self._f32(rope_cs_table(head_dim=self.value_dim // 16))
 
 
 class MemoryBank:
@@ -398,12 +444,19 @@ class Engine:
         self._call("s3r_engine_heads", "heads", _lib.ptr(pts), _lib.ptr(conf))
         return pts, conf
 
-    def value(self, pts3d, feat_k1, transposed: bool = False, rope: bool = False):
+    def value(self, pts3d, feat_k1, transposed: bool = False, rope: bool = False, tokens: bool = False):
         """pts3d: head 1's map in the head's own [B, H, W, 3] layout; transposed=True reads it as the [B, W, H, 3]
-        landscape view the reference's head wrapper returns for portrait frames (S3R_VALUE_PTS_TRANSPOSED)."""
-        self._chk(pts3d, (self.B, self.H, self.W, 3)); self._chk(feat_k1, (self.B, self.N, 1024))
+        landscape view the reference's head wrapper returns for portrait frames (S3R_VALUE_PTS_TRANSPOSED).
+        tokens=True (use_feat weights, S3R_VALUE_DEC_TOKENS): the input is dec1[-1] [B, N, 768] instead, or None for the
+        engine's own copy from the last `decode`."""
+        if tokens:
+            if pts3d is not None:
+                self._chk(pts3d, (self.B, self.N, 768))
+        else:
+            self._chk(pts3d, (self.B, self.H, self.W, 3))
+        self._chk(feat_k1, (self.B, self.N, 1024))
         out = self._new(self.B, self.N, 1024)
-        flags = (VALUE_PTS_TRANSPOSED if transposed else 0) | (VALUE_ROPE if rope else 0)
+        flags = (VALUE_PTS_TRANSPOSED if transposed else 0) | (VALUE_ROPE if rope else 0) | (VALUE_DEC_TOKENS if tokens else 0)
         self._call("s3r_engine_value", "value", _lib.ptr(pts3d), _lib.ptr(feat_k1), flags, _lib.ptr(out))
         return out
 

@@ -1,7 +1,7 @@
 """Drop-in `Spann3R` / `SpatialMemory` / DUSt3R module for the reference's callers.
 
 Mirrors the reference's public surface (spann3r/model.py:11-226,473-539; dust3r/model.py:84-225) --
-same class names, constructor signature, `state_dict` keys (1101, strict-loadable both ways), the
+same class names, constructor signature, `state_dict` keys (1101, or 1099 with `use_feat=True`; strict-loadable both ways), the
 `.dust3r` attribute, `forward(frames, return_memory=False) -> (preds, preds_all[, sp_mem])` with the
 same dict keys / shapes -- so `demo.py` / `eval.py` run by changing one import (INTEGRATION.md).
 
@@ -10,7 +10,10 @@ The modules below hold parameters only.  All arithmetic runs in libspann3r_b200.
 GPU `forward` raises.  Training mode (`train.py`): the same CUDA forward with the reference's
 training branches (attn_thresh=0, memory dropout, ungated add_mem) and a PyTorch-recompute backward (SURVEY.md §8f rank 1, staged).
 `offline_reconstruction` (SURVEY.md §8f rank 2) is built on the same engine stages.  Portrait frames follow the
-reference's landscape wrapper (`_to_landscape`); `mem_pos_enc=True` is supported, `use_feat=True` is not.
+reference's landscape wrapper (`_to_landscape`).  Every constructor option is supported: `mem_pos_enc=True` puts RoPE into the
+value encoder; `use_feat=True` builds the reference's 768-wide value encoder (16 heads of 48, no `pos_patch_embed`), fed
+with head 1's last decoder tokens instead of the pointmap.  The library runs its 48-wide heads zero-padded to 64-wide slots
+(include/spann3r_b200.h, s3r_model_w.value_dim), an exact repacking of the same arithmetic.
 """
 from __future__ import annotations
 
@@ -260,11 +263,9 @@ class Spann3R(ParamModule):
     def __init__(self, dus3r_name="./checkpoints/DUSt3R_ViTLarge_BaseDecoder_512_dpt.pth", use_feat=False,
                  mem_pos_enc=False, memory_dropout=0.15, max_encode_batch: int = 16):
         super().__init__()
-        if use_feat:
-            raise NotImplementedError("use_feat=True (a 768-wide value encoder fed with decoder tokens, 48-wide heads) is "
-                                      "not built; the released checkpoints and demo.py / eval.py use the default")
-        self.use_feat, self.mem_pos_enc = use_feat, mem_pos_enc
-        spec = synth.load_spec()
+        self.use_feat, self.mem_pos_enc = bool(use_feat), mem_pos_enc
+        # use_feat (spann3r/model.py:225-242): a 768-wide value encoder and no pos_patch_embed
+        spec = synth.usefeat_spec() if self.use_feat else synth.load_spec()
         self.dust3r = AsymmetricCroCo3DStereo(spec)
         object.__setattr__(self.dust3r, "_owner", self)
         rest = {k: v for k, v in spec["spann3r"].items() if not k.startswith("dust3r.")}
@@ -294,9 +295,10 @@ class Spann3R(ParamModule):
                 raise ValueError(f"unsupported DUSt3R architecture (need {need}): {args}")
         print("... loading model from", path)
         print(self.dust3r.load_state_dict(ckpt["model"], strict=False))
-        # spann3r/model.py:240-241: pos_patch_embed starts as a copy of dust3r.patch_embed
-        self.pos_patch_embed.proj.weight.data.copy_(self.dust3r.patch_embed.proj.weight.data)
-        self.pos_patch_embed.proj.bias.data.copy_(self.dust3r.patch_embed.proj.bias.data)
+        if not self.use_feat:
+            # spann3r/model.py:240-242: pos_patch_embed (default value encoder only) starts as a copy of dust3r.patch_embed
+            self.pos_patch_embed.proj.weight.data.copy_(self.dust3r.patch_embed.proj.weight.data)
+            self.pos_patch_embed.proj.bias.data.copy_(self.dust3r.patch_embed.proj.bias.data)
 
     @torch.no_grad()
     def _init_like_reference(self):
@@ -428,7 +430,7 @@ class Spann3R(ParamModule):
 
     def _frame_loop(self, F_, H, W, eng, sp_mem, feat_of, return_memory):
         """The frame loop of spann3r/model.py:484-533 over the already encoded frames."""
-        portrait = H > W        # heads run at (H, W); outputs and the value encoder's input are the landscape views
+        portrait = H > W        # heads run at (H, W); outputs and the pointmap value encoder's input are the landscape views
         feat_k2 = None
         preds, preds_all = None, []
         for i in range(F_ - 1):
@@ -440,8 +442,7 @@ class Spann3R(ParamModule):
             pts, conf = eng.heads()
             res1 = {"pts3d": _to_landscape(pts[0], H, W), "conf": _to_landscape(conf[0], H, W)}
             res2 = {"pts3d": _to_landscape(pts[1], H, W), "conf": _to_landscape(conf[1], H, W)}
-            # encode_cur_value(res1['pts3d']) + feat_k1; the engine reads pts[0] through the landscape view's strides
-            mem_v = eng.value(pts[0], feat_k1, transposed=portrait, rope=self.mem_pos_enc)
+            mem_v = self._value(eng, pts[0], feat_k1, portrait)
             sp_mem.add_mem_check(feat_k1, mem_v, sim_pending=sim)
             res2["pts3d_in_other_view"] = res2.pop("pts3d")
             if preds is None:
@@ -455,6 +456,14 @@ class Spann3R(ParamModule):
         if return_memory:
             return preds, preds_all, sp_mem
         return preds, preds_all
+
+    def _value(self, eng, pts1, feat_k1, portrait):
+        """encode_cur_value(res1, dec1, pos1, shape1) + feat_k1 (spann3r/model.py:312-320, 519-521) after the engine's last
+        decode / heads.  Default: the pointmap of head 1, which the engine reads through the landscape view's strides.
+        use_feat: dec1[-1], the engine's resident dec_norm tokens of stream 1, on the frame's own grid."""
+        if self.use_feat:
+            return eng.value(None, feat_k1, rope=self.mem_pos_enc, tokens=True)
+        return eng.value(pts1, feat_k1, transposed=portrait, rope=self.mem_pos_enc)
 
     # -- offline mode (SURVEY.md §8f rank 2) ------------------------------------------------------------
     def find_initial_pair(self, graph, n_frames):
@@ -526,7 +535,7 @@ class Spann3R(ParamModule):
                 feat2 = feats[best_id]
                 res1, res2 = decode_heads(feat_fuse, feat2)          # restores the engine's hooks for the winner
             feat_k1, feat_k2 = eng.keyheads(feat1, feat2)
-            mem_v = eng.value(res1.pop("_raw"), feat_k1, transposed=portrait, rope=self.mem_pos_enc)
+            mem_v = self._value(eng, res1.pop("_raw"), feat_k1, portrait)
             sp_mem.add_mem_check(feat_k1, mem_v)
             res2["pts3d_in_other_view"] = res2.pop("pts3d")
             if preds is None:

@@ -39,6 +39,29 @@ def load_spec(path: str = _SPEC_PATH) -> dict:
         return json.load(f)
 
 
+USE_FEAT_DIM = 768   # Spann3R(use_feat=True): the value encoder runs at the decoder's width (spann3r/model.py:225)
+
+
+def usefeat_spec(spec: dict | None = None) -> dict:
+    """The state-dict inventory of `Spann3R(use_feat=True)`, derived from the default one (spann3r/model.py:225-242):
+    `pos_patch_embed` is not created, and the value encoder (6 Blocks, 16 heads of 48), `value_norm` and `value_out`'s
+    input are 768 wide.  Every other key keeps its shape and its place in the order (1099 keys)."""
+    spec = spec or load_spec()
+    D = USE_FEAT_DIM
+    out = {}
+    for key, shape in spec["spann3r"].items():
+        if key.startswith("pos_patch_embed."):
+            continue
+        if key.startswith("value_encoder."):
+            shape = [D if s == 1024 else 4 * D if s == 4096 else 3 * D if s == 3072 else s for s in shape]
+        elif key.startswith("value_norm."):
+            shape = [D]
+        elif key == "value_out.weight":
+            shape = [shape[0], D]
+        out[key] = list(shape)
+    return {**{k: v for k, v in spec.items() if k != "spann3r"}, "spann3r": out}
+
+
 def _gen(seed: int, key: str) -> torch.Generator:
     g = torch.Generator(device="cpu")
     g.manual_seed((seed * 1000003 + zlib.crc32(key.encode())) & 0x7FFFFFFFFFFFFFFF)

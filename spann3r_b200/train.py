@@ -17,7 +17,9 @@ What is native and what is not (said once, here):
   (`spann3r/training.py:322-325`) all-reduces them over NCCL like the reference's.
 
 Stages (= Functions): encoder (per chunk of frames), memory read, frame step (twin decoder + key heads + DPT heads), value
-encoder.  Square / landscape frames only (the reference trains at 224 x 224).
+encoder.  Square / landscape frames only (the reference trains at 224 x 224).  With `use_feat=True` the frame step also
+returns dec1[-1] (dec_norm of head 1's last decoder layer) and the value stage reads it, so the memory values' gradients
+reach the decoder as in the reference (spann3r/model.py:312-314).
 """
 from __future__ import annotations
 
@@ -158,10 +160,14 @@ def forward_train(model, frames, return_memory=False):
     val_names, val_params = stage_params(model, "value")
     rope_v = bool(model.mem_pos_enc)
 
+    use_feat = bool(model.use_feat)
+
     def native_step(feat_fuse, feat1, feat2):
-        eng.decode(feat_fuse.contiguous(), feat2.contiguous())
+        dec_all = eng.decode(feat_fuse.contiguous(), feat2.contiguous(), want_all=use_feat)
         k1, k2 = eng.keyheads(feat1.contiguous(), feat2.contiguous())
         pts, conf = eng.heads()
+        if use_feat:                  # dec1[-1]: the last (normed) layer of stream 1
+            return k1, k2, pts, conf, dec_all[11, 0].clone()
         return k1, k2, pts, conf
 
     feat_k2 = None
@@ -169,12 +175,17 @@ def forward_train(model, frames, return_memory=False):
     for i in range(F_ - 1):
         feat1, feat2 = feats[i], feats[i + 1]
         feat_fuse = mem.memory_read(feat_k2) if feat_k2 is not None else feat1
-        feat_k1, feat_k2, pts, conf = _apply(native_step, lambda P, a, b, c: R.step(P, a, b, c, H, W), step_names,
-                                             step_params, feat_fuse, feat1, feat2)
+        outs = _apply(native_step, lambda P, a, b, c: R.step(P, a, b, c, H, W, dec_tokens=use_feat), step_names,
+                      step_params, feat_fuse, feat1, feat2)
+        feat_k1, feat_k2, pts, conf = outs[:4]
         res1 = {"pts3d": pts[0], "conf": conf[0]}
         res2 = {"pts3d_in_other_view": pts[1], "conf": conf[1]}
-        mem_v = _apply(lambda p3, k1: eng.value(p3.contiguous(), k1.contiguous(), transposed=False, rope=rope_v),
-                       lambda P, p3, k1: R.value(P, p3, k1, rope_v), val_names, val_params, pts[0], feat_k1)
+        if use_feat:
+            mem_v = _apply(lambda d1, k1: eng.value(d1.contiguous(), k1.contiguous(), rope=rope_v, tokens=True),
+                           lambda P, d1, k1: R.value_tokens(P, d1, k1, rope_v, H, W), val_names, val_params, outs[4], feat_k1)
+        else:
+            mem_v = _apply(lambda p3, k1: eng.value(p3.contiguous(), k1.contiguous(), transposed=False, rope=rope_v),
+                           lambda P, p3, k1: R.value(P, p3, k1, rope_v), val_names, val_params, pts[0], feat_k1)
         mem.add_mem(feat_k1, mem_v)                         # training: no similarity gate (spann3r/model.py:518-519)
         if preds is None:
             preds = [res1]

@@ -19,6 +19,11 @@ Outputs
   tests/golden/seq_224_3f_sharp_mempos.npz  3 x 224x224 with Spann3R(mem_pos_enc=True) (RoPE inside the value encoder)
   tests/golden/cfg2_384x512_10f_sharp.npz  BASELINE config 2 exactly (10 x 384x512, sharpened ckpt), outputs (::16, ::16), bank rows ::4   [--only cfg2]
   tests/golden/cfg2_384x512_10f_raw.npz    the same on the RAW random-init checkpoint (SURVEY 8d: report both)            [--only cfg2]
+  Spann3R(use_feat=True), sharpened weights of synth.usefeat_spec()                                                     [--only usefeat]
+  tests/golden/state_dict_spec_usefeat.json  key -> shape of the reference's use_feat state dict, in order
+  tests/golden/seq_224_3f_sharp_usefeat.npz  3 x 224x224, with the value_out hook, outputs (::2, ::2)
+  tests/golden/seq_288x224_3f_sharp_usefeat_mempos.npz  PORTRAIT 3 x (H=288, W=224) with mem_pos_enc=True, outputs (::4, ::4)
+  tests/golden/offline_224_4f_sharp_usefeat.npz  offline mode, 4 x 224x224, outputs (::4, ::4)
 The hooked runs also store the sub-sampled per-stage activations the tests compare (GOLDEN_ACTS).
 """
 import argparse
@@ -36,7 +41,7 @@ sys.path.insert(0, REPO)
 GOLD = os.path.join(REPO, "tests", "golden")
 
 
-def build_reference(seed=0, sharpen=False, mem_pos_enc=False):
+def build_reference(seed=0, sharpen=False, mem_pos_enc=False, use_feat=False):
     sys.path.insert(0, REF)
     torch.serialization.add_safe_globals([argparse.Namespace])
     from spann3r.model import Spann3R  # noqa  (reference)
@@ -57,11 +62,16 @@ def build_reference(seed=0, sharpen=False, mem_pos_enc=False):
             json.dump(spec, f, indent=0)
         print("wrote", spec_path, len(spec["spann3r"]), "keys")
     spec = synth.load_spec(spec_path)
+    if use_feat:
+        spec = synth.usefeat_spec(spec)
     dust3r_sd = synth.make_state_dict(spec, seed=seed, prefix="dust3r.")
     torch.save({"args": argparse.Namespace(model=synth.DUST3R_ARGS), "model": dust3r_sd}, tmp)
     t0 = time.time()
-    m = Spann3R(dus3r_name=tmp, use_feat=False, mem_pos_enc=mem_pos_enc)
+    m = Spann3R(dus3r_name=tmp, use_feat=use_feat, mem_pos_enc=mem_pos_enc)
     sd = synth.make_state_dict(spec, seed=seed, sharpen=sharpen)
+    ref_spec = {k: list(v.shape) for k, v in m.state_dict().items()}
+    if list(ref_spec.items()) != list(spec["spann3r"].items()):
+        raise RuntimeError("the synthetic key inventory differs from the reference's (keys, order or shapes)")
     missing = m.load_state_dict(sd, strict=True)
     print("reference built in %.1fs" % (time.time() - t0), missing)
     return m.eval()
@@ -110,6 +120,8 @@ def run(model, frames, out_path, px_stride=1, hooks=True, mem_stride=1):
         }
         mods = dict(model.named_modules())
         for name, pick in watch.items():
+            if name not in mods:      # pos_patch_embed does not exist with use_feat=True
+                continue
             def mk(name, pick):
                 def hook(_m, _i, o):
                     k = "act/" + name
@@ -204,6 +216,17 @@ def main():
             run(m, synth.make_frames(4, 224, 224), os.path.join(GOLD, "seq_224_4f_sharp.npz"), px_stride=4)
         if args.only in ("all", "seq512"):
             run(m, synth.make_frames(3, 384, 512), os.path.join(GOLD, "seq_384x512_3f_sharp.npz"), px_stride=8)
+    if args.only in ("all", "usefeat"):
+        m = build_reference(sharpen=True, use_feat=True)
+        with open(os.path.join(GOLD, "state_dict_spec_usefeat.json"), "w") as f:
+            json.dump({k: list(v.shape) for k, v in m.state_dict().items()}, f, indent=0)
+        run(m, synth.make_frames(3, 224, 224), os.path.join(GOLD, "seq_224_3f_sharp_usefeat.npz"), px_stride=2)
+        run_offline(m, synth.make_frames(4, 224, 224), os.path.join(GOLD, "offline_224_4f_sharp_usefeat.npz"))
+        del m
+        m = build_reference(sharpen=True, use_feat=True, mem_pos_enc=True)
+        run(m, synth.make_frames(3, 288, 224), os.path.join(GOLD, "seq_288x224_3f_sharp_usefeat_mempos.npz"), px_stride=4,
+            hooks=False)
+        del m
 
 
 if __name__ == "__main__":
