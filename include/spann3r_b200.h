@@ -30,8 +30,8 @@ enum { S3R_EPI_PLAIN = 0, S3R_EPI_PIXSHUF = 1, S3R_EPI_QKV = 2, S3R_EPI_HEADTAIL
 enum { S3R_ACT_NONE = 0, S3R_ACT_GELU = 1, S3R_ACT_RELU = 2 };
 
 int s3r_version(void);
-/* sizeof(s3r_gemm_desc / s3r_model_w / s3r_bank) as compiled: bindings check their mirrors against these */
-int s3r_abi_sizeof(int which /* 0 gemm_desc, 1 model_w, 2 bank */);
+/* sizeof(s3r_gemm_desc / s3r_model_w / s3r_bank / s3r_loss_desc) as compiled: bindings check their mirrors against these */
+int s3r_abi_sizeof(int which /* 0 gemm_desc, 1 model_w, 2 bank, 3 loss_desc */);
 /* last error text of the calling thread ("" if none) */
 const char* s3r_last_error(void);
 /* 1 if a CUDA device of compute capability 9.0 (H100, sm_90a) is visible, else 0 (never falls back to CPU) */
@@ -229,6 +229,46 @@ size_t s3r_pcl_stats_workspace_bytes(void);
 int s3r_pcl_stats(const double* x, int64_t n, double threshold, void* workspace, double* out, void* stream);
 /* out[i] = |a[i] . b[idx[i]]| for a [n, 3], b [*, 3] fp64, idx [n] int64 (eval_recon.py's normal consistency). */
 int s3r_pcl_abs_dot(const double* a, const double* b, const int64_t* idx, int64_t n, double* out, void* stream);
+
+/* ---- training / test criteria: spann3r/loss.py:129-369 (Regr3D_t, its ShiftInv / ScaleInv / ScaleShiftInv variants,
+ * ConfLoss_t) with L21 (dust3r/losses.py:52-59), forward and backward --------------------------------------------------
+ * F >= 2 views of B sequences of H x W pixels.  Pred slot k < F-1 is preds_all[k][0] (frame k: 'pts3d' for k = 0, else
+ * 'pts3d_in_other_view'), slot F-1+i is preds_all[i][1]['pts3d_in_other_view'] (frame i+1); every map is a contiguous
+ * fp32 [B, H, W, 3] (conf [B, H, W]) device tensor.  gt_pts / valid / pred / conf are HOST arrays of device pointers
+ * (F, F, 2(F-1), 2(F-1) entries); the library copies them into the workspace.
+ *   norm_mode 0 (False), 1 'avg_dis', 2 'avg_log1p'; gt_scale, fix_first as Regr3D_t; shift_inv / scale_inv select the
+ *   variant (both = Regr3D_t_ScaleShiftInv); conf_loss = ConfLoss_t(alpha) over the criterion (needs conf), else the
+ *   per-term means are summed ('mean' reduction); conf may be NULL without conf_loss (details conf_left/right then 0);
+ *   has_dist_clip: valid &= |pts3d| <= dist_clip (untransformed points). */
+typedef struct s3r_loss_desc {
+  int frames, batch, height, width;
+  int norm_mode, gt_scale, fix_first, shift_inv, scale_inv, conf_loss, has_dist_clip;
+  float alpha, dist_clip;
+  const float* pose0;                /* device [B, 4, 4] camera_pose of view 0 (cam-to-world) */
+  const float* const* gt_pts;        /* [F] -> [B, H, W, 3] pts3d (world) */
+  const uint8_t* const* valid;       /* [F] -> [B, H, W] bool valid_mask */
+  const float* const* pred;          /* [2(F-1)] -> [B, H, W, 3] */
+  const float* const* conf;          /* [2(F-1)] -> [B, H, W], or NULL */
+} s3r_loss_desc;
+/* results (fp64, device): S3R_LOSS_RES_HEADER values, then S3R_LOSS_RES_PER_B per batch element.
+ * Header: loss, factor_loss, pts3d_1, pts3d_2, loss_left, loss_right, conf_left, conf_right, conf_loss_1, conf_loss2,
+ * conf_mean, then the batch means of gt_shift_z, pred_shift_z, gt_scale, pred_scale (clipped), the count k of
+ * pr_factor > gt_factor (-1: no factor_loss), the number of terms without a valid pixel; zeros up to the header size.
+ * Per b: gt_factor (1 without), pr_factor (1 without), gt_shift_z, pred_shift_z, gt_scale, pred_scale (clipped). */
+#define S3R_LOSS_RES_HEADER 20
+#define S3R_LOSS_RES_PER_B 6
+/* bytes of caller-owned device workspace (256-byte aligned) for one forward + its backward; 0 = invalid descriptor */
+size_t s3r_loss_workspace_bytes(const s3r_loss_desc* d);
+/* One criterion evaluation.  Optional outputs (NULL = not written): gt_out [F, B, H, W, 3] and pred_out [2(F-1), B, H,
+ * W, 3], the aligned maps get_all_pts3d_t returns; valid_out [F, B, H, W] uint8 masks.  No host synchronisation; sums
+ * in fp64 in a fixed order (bitwise reproducible); medians exact (torch.nanmedian's lower median). */
+int s3r_loss_forward(const s3r_loss_desc* d, void* workspace, size_t workspace_bytes, float* gt_out, float* pred_out,
+                     uint8_t* valid_out, double* results, void* stream);
+/* Gradients of upstream[0] * loss + upstream[1] * factor_loss (upstream: device fp32 [2]) with respect to every pred slot
+ * -> grad_pred [2(F-1), B, H, W, 3] and, with conf_loss, every conf slot -> grad_conf [2(F-1), B, H, W] (else unused).
+ * The workspace is the forward's, unchanged since, with the same descriptor. */
+int s3r_loss_backward(const s3r_loss_desc* d, const void* workspace, size_t workspace_bytes, const float* upstream,
+                      float* grad_pred, float* grad_conf, void* stream);
 
 /* ---- model level: the per-frame forward path -------------------------------------------------
  * Packed weights.  The host (spann3r_b200/weights.py) converts the reference state dict ONCE into

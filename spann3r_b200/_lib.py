@@ -41,6 +41,19 @@ class GemmDesc(C.Structure):
     ]
 
 
+class LossDesc(C.Structure):
+    """Mirror of s3r_loss_desc; the pointer arrays are host arrays of device pointers."""
+    _fields_ = [
+        ("frames", _i), ("batch", _i), ("height", _i), ("width", _i),
+        ("norm_mode", _i), ("gt_scale", _i), ("fix_first", _i), ("shift_inv", _i), ("scale_inv", _i), ("conf_loss", _i),
+        ("has_dist_clip", _i), ("alpha", _f), ("dist_clip", _f),
+        ("pose0", _vp), ("gt_pts", C.POINTER(_vp)), ("valid", C.POINTER(_vp)), ("pred", C.POINTER(_vp)),
+        ("conf", C.POINTER(_vp)),
+    ]
+
+
+LOSS_RES_HEADER, LOSS_RES_PER_B = 20, 6
+
 _PROTOS = {
     "s3r_version": (_i, []),
     "s3r_abi_sizeof": (_i, [_i]),
@@ -75,6 +88,9 @@ _PROTOS = {
     "s3r_pcl_stats_workspace_bytes": (C.c_size_t, []),
     "s3r_pcl_stats": (_i, [_vp, _i64, C.c_double, _vp, _vp, _vp]),
     "s3r_pcl_abs_dot": (_i, [_vp, _vp, _vp, _i64, _vp, _vp]),
+    "s3r_loss_workspace_bytes": (C.c_size_t, [C.POINTER(LossDesc)]),
+    "s3r_loss_forward": (_i, [C.POINTER(LossDesc), _vp, C.c_size_t, _vp, _vp, _vp, _vp, _vp]),
+    "s3r_loss_backward": (_i, [C.POINTER(LossDesc), _vp, C.c_size_t, _vp, _vp, _vp, _vp]),
     "s3r_resample_h_u8": (_i, [_vp, _i64, _i, _i, _vp, _vp, _i, _i, _vp, _vp]),
     "s3r_resample_v_u8_norm": (_i, [_vp, _i, _i, _vp, _vp, _i, _vp, _vp]),
 }

@@ -20,6 +20,7 @@ int s3r_abi_sizeof(int which) {
     case 0: return (int)sizeof(s3r_gemm_desc);
     case 1: return (int)sizeof(s3r_model_w);
     case 2: return (int)sizeof(s3r_bank);
+    case 3: return (int)sizeof(s3r_loss_desc);
   }
   return -1;
 }
@@ -214,6 +215,16 @@ int s3r_pcl_stats(const double* x, int64_t n, double threshold, void* workspace,
 }
 int s3r_pcl_abs_dot(const double* a, const double* b, const int64_t* idx, int64_t n, double* out, void* stream) {
   return launch_pcl_abs_dot(a, b, reinterpret_cast<const long long*>(idx), n, out, S(stream));
+}
+
+size_t s3r_loss_workspace_bytes(const s3r_loss_desc* d) { return loss_workspace_bytes(d); }
+int s3r_loss_forward(const s3r_loss_desc* d, void* workspace, size_t workspace_bytes, float* gt_out, float* pred_out,
+                     uint8_t* valid_out, double* results, void* stream) {
+  return launch_loss_forward(d, workspace, workspace_bytes, gt_out, pred_out, valid_out, results, S(stream));
+}
+int s3r_loss_backward(const s3r_loss_desc* d, const void* workspace, size_t workspace_bytes, const float* upstream,
+                      float* grad_pred, float* grad_conf, void* stream) {
+  return launch_loss_backward(d, workspace, workspace_bytes, upstream, grad_pred, grad_conf, S(stream));
 }
 
 int s3r_conf_score(const float* conf, int64_t n, float* scratch256, float* out, void* stream) {

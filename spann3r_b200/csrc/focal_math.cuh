@@ -57,5 +57,13 @@ S3R_FHD uint32_t order_key(float f) {
 }
 S3R_FHD float key_value(uint32_t k) { return bits_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k); }
 
+// one digit of an 8-bit radix select: the bin of the 256-bin histogram that holds the element of rank k (0-based,
+// ascending); k becomes that element's rank inside the bin.  Ranks beyond the total land in bin 255.
+S3R_FHD int radix_pick(const int* hist, long long& k) {
+  int bin = 0;
+  while (bin < 255 && k >= hist[bin]) k -= hist[bin++];
+  return bin;
+}
+
 }  // namespace focal
 }  // namespace s3r

@@ -147,8 +147,7 @@ __global__ void __launch_bounds__(32) focal_median_pick_kernel(int* __restrict__
       k = (n - 1) / 2;
     }
     if (sc[259] >= 0) {
-      int bin = 0;
-      while (bin < 255 && k >= sc[bin]) k -= sc[bin++];
+      const int bin = focal::radix_pick(sc, k);
       sc[256] = (int)((((uint32_t)sc[256]) << 8) | (uint32_t)bin);
       sc[257] = (int)(uint32_t)(k & 0xffffffffll);
       sc[258] = (int)(uint32_t)(k >> 32);

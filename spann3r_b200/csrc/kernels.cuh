@@ -6,6 +6,8 @@
 #include "gemm.cuh"
 #include <cuda.h>
 
+struct s3r_loss_desc;   // include/spann3r_b200.h
+
 namespace s3r {
 
 int launch_split(const float* x, long long ldx, __nv_bfloat16* hi, __nv_bfloat16* lo, long long ldp, int col0,
@@ -104,6 +106,13 @@ int launch_conv_wgrad(const __nv_bfloat16* dy_hi, const __nv_bfloat16* dy_lo, lo
                       const __nv_bfloat16* x_lo, long long ldx, int NB, int H, int W, int N, int Kc, int taps,
                       void* workspace, size_t workspace_bytes, float* dw, cudaStream_t st);
 int launch_col2im_3x3s2(const float* cols, int NB, int H, int W, int C, int Ho, int Wo, float* out, cudaStream_t st);
+
+// training / test criteria (loss.cu): validate the descriptor before any CUDA call
+size_t loss_workspace_bytes(const s3r_loss_desc* d);
+int launch_loss_forward(const s3r_loss_desc* d, void* ws, size_t ws_bytes, float* gt_out, float* pred_out,
+                        uint8_t* valid_out, double* results, cudaStream_t st);
+int launch_loss_backward(const s3r_loss_desc* d, const void* ws, size_t ws_bytes, const float* upstream,
+                         float* grad_pred, float* grad_conf, cudaStream_t st);
 
 // fused attention (attention.cu): O = softmax(Q K^T) V per (batch*head), tf32 wgmma, split-bf16 output
 int launch_attention(const float* q, const float* k, const float* vt, int BH, int heads, int nq, int nk, int nk_pad,

@@ -284,3 +284,80 @@ PNP_CASES = [
     (384, 512, 420.0, (-0.2, 0.4, 0.3), (0.1, 0.6, -0.3), 0.003, 0.3, 4),
     (384, 512, 380.0, (0.05, 1.2, -0.4), (1.0, -0.3, 0.8), 0.004, 0.45, 5),
 ]
+
+
+def make_loss_case(batch: int, frames: int, height: int, width: int, invalid: float = 0.3, seed: int = 0,
+                   device="cpu"):
+    """Views and `preds_all` for the criteria (spann3r_b200.loss / tests/golden/loss_*.npz): a wavy surface per frame
+    in world coordinates seen through a non-identity camera_pose per view; `invalid` of the pixels in irregular blobs
+    (0: all valid); predictions = the ground truth in view 0's camera frame, scaled per sequence, plus noise, with the
+    keys Spann3R.forward returns (pair 0 left: 'pts3d', every other map: 'pts3d_in_other_view'), conf = 1 + exp(x).
+    fp32 CPU tensors (moved to `device`)."""
+    g = torch.Generator().manual_seed(seed)
+    B, F, H, W = batch, frames, height, width
+    v, u = torch.meshgrid(torch.linspace(-1, 1, H), torch.linspace(-1, 1, W), indexing="ij")
+    poses = []
+    for f in range(F):
+        ang = 0.05 * torch.randn(B, 3, generator=g, dtype=torch.float64) + torch.tensor([0.02 * f, -0.01 * f, 0.0],
+                                                                                          dtype=torch.float64)
+        R = torch.stack([torch.as_tensor(_rotation(a.tolist())) for a in ang])
+        P = torch.eye(4, dtype=torch.float64).repeat(B, 1, 1)
+        P[:, :3, :3] = R
+        P[:, :3, 3] = 0.3 * torch.randn(B, 3, generator=g, dtype=torch.float64) + torch.tensor([0.1 * f, 0.0, 0.05 * f])
+        poses.append(P)
+    inv0 = torch.linalg.inv(poses[0])
+    gts, cam0 = [], []
+    for f in range(F):
+        z = 2.0 + 0.3 * torch.rand(B, 1, 1, generator=g, dtype=torch.float64) \
+            + 0.2 * torch.sin(3 * u + f)[None] * torch.cos(2 * v)[None]
+        cam = torch.stack((u[None] * z, v[None] * z * (H / W), z), -1)                   # in camera f
+        world = torch.einsum("bij,bhwj->bhwi", poses[f][:, :3, :3], cam) + poses[f][:, None, None, :3, 3]
+        if invalid > 0:
+            low = torch.rand(B, 1, max(2, H // 24), max(2, W // 24), generator=g)
+            blob = torch.nn.functional.interpolate(low, size=(H, W), mode="bicubic", align_corners=False)[:, 0]
+            noise = torch.rand(B, H, W, generator=g)
+            valid = (blob + 0.15 * noise) > torch.quantile(blob.flatten(1) + 0.15 * noise.flatten(1), invalid, dim=1)[:, None, None]
+        else:
+            valid = torch.ones(B, H, W, dtype=torch.bool)
+        gts.append({"pts3d": world.float(), "valid_mask": valid, "camera_pose": poses[f].float()})
+        cam0.append(torch.einsum("bij,bhwj->bhwi", inv0[:, :3, :3], world) + inv0[:, None, None, :3, 3])
+    s = 0.5 + torch.rand(B, 1, 1, 1, generator=g, dtype=torch.float64)
+
+    def pred(f):
+        return (cam0[f] * s + 0.05 * torch.randn(cam0[f].shape, generator=g, dtype=torch.float64)).float()
+
+    def conf():
+        return (1 + torch.exp(0.5 * torch.randn(B, H, W, generator=g))).float()
+
+    preds = []
+    for k in range(F - 1):
+        left = {("pts3d" if k == 0 else "pts3d_in_other_view"): pred(k), "conf": conf()}
+        right = {"pts3d_in_other_view": pred(k + 1), "conf": conf()}
+        preds.append((left, right))
+    if device != "cpu":
+        gts = [{k: t.to(device) for k, t in d.items()} for d in gts]
+        preds = [tuple({k: t.to(device) for k, t in d.items()} for d in p) for p in preds]
+    return gts, preds
+
+
+# the cases of tests/golden/loss_<name>.npz: criterion string, call ("loss" = compute_frame_loss, "pts" =
+# get_all_pts3d_t), keyword arguments, data (make_loss_case arguments)
+LOSS_CASES = {
+    "train": {"criterion": "ConfLoss_t(Regr3D_t(L21, norm_mode='avg_dis', fix_first=False), alpha=0.4)", "call": "loss",
+              "data": {"batch": 2, "frames": 5, "height": 224, "width": 224, "invalid": 0.3, "seed": 1}},
+    "test": {"criterion": "Regr3D_t_ScaleShiftInv(L21, gt_scale=True)", "call": "loss",
+             "data": {"batch": 2, "frames": 4, "height": 224, "width": 224, "invalid": 0.3, "seed": 2}},
+    "eval": {"criterion": "Regr3D_t_ScaleShiftInv(L21, norm_mode=False, gt_scale=True)", "call": "pts",
+             "data": {"batch": 1, "frames": 4, "height": 224, "width": 224, "invalid": 0.2, "seed": 3}},
+    "log1p_fixfirst_clip": {"criterion": "ConfLoss_t(Regr3D_t(L21, norm_mode='avg_log1p', fix_first=True), alpha=0.2)",
+                            "call": "loss", "kw": {"dist_clip": 3.0},
+                            "data": {"batch": 2, "frames": 3, "height": 64, "width": 96, "invalid": 0.3, "seed": 4}},
+    "scaleinv": {"criterion": "Regr3D_t_ScaleInv(L21, gt_scale=False, fix_first=False)", "call": "loss",
+                 "data": {"batch": 3, "frames": 3, "height": 64, "width": 64, "invalid": 0.3, "seed": 5}},
+    "regr_mean": {"criterion": "Regr3D_t(L21, norm_mode='avg_dis')", "call": "loss",
+                  "data": {"batch": 2, "frames": 3, "height": 48, "width": 64, "invalid": 0.3, "seed": 6}},
+    "landscape": {"criterion": "ConfLoss_t(Regr3D_t(L21, norm_mode='avg_dis', fix_first=False), alpha=0.4)", "call": "loss",
+                  "data": {"batch": 1, "frames": 3, "height": 384, "width": 512, "invalid": 0.3, "seed": 7}},
+    "even_pts": {"criterion": "Regr3D_t_ScaleShiftInv(L21, gt_scale=False)", "call": "pts",
+                 "data": {"batch": 2, "frames": 3, "height": 32, "width": 48, "invalid": 0.0, "seed": 8}},
+}

@@ -2,11 +2,12 @@
 """BASELINE config[4] / SURVEY.md §8d config 5: the reference's DDP training step on synthetic views.
 
     torchrun --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P tools/train_step_bench.py \
-        [--impl ours|reference] [--batch 4] [--frames 10] [--res 224] [--steps 5] [--warmup 2] [--native-linear] [--native-conv]
+        [--impl ours|reference] [--batch 4] [--frames 10] [--res 224] [--steps 5] [--warmup 2] [--native-linear] [--native-conv] [--native-criterion]
 
 One step = `spann3r/training.py:216-228`: forward of a batch of `--batch` sequences per rank -> `ConfLoss_t(Regr3D_t(L21,
 norm_mode='avg_dis', fix_first=False), alpha=0.4).compute_frame_loss` (the REFERENCE's criterion, imported from the staged
-copy under oracle/_ref: losses are callers of the path, SURVEY.md §2) -> backward -> DDP gradient all-reduce (NCCL, 2.63 GB
+copy under oracle/_ref: losses are callers of the path, SURVEY.md §2; --native-criterion: the same criterion on the
+library's kernels, spann3r_b200.loss; the JSON line records which) -> backward -> DDP gradient all-reduce (NCCL, 2.63 GB
 fp32 per rank, `DistributedDataParallel(find_unused_parameters=True, static_graph=True)` as `training.py:322-325`) -> AdamW.
 
 --impl ours: `spann3r_b200.Spann3R` in training mode = the sm_90a kernels forward (attn_thresh=0, Philox memory dropout,
@@ -60,6 +61,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--native-linear", action="store_true", help="train.set_native_linear(True)")
     ap.add_argument("--native-conv", action="store_true", help="train.set_native_conv(True)")
+    ap.add_argument("--native-criterion", action="store_true", help="the criterion of spann3r_b200.loss (sm_90a kernels)")
     a = ap.parse_args()
     rank, world, local = (int(os.environ.get(k, d)) for k, d in (("RANK", 0), ("WORLD_SIZE", 1), ("LOCAL_RANK", 0)))
     torch.cuda.set_device(local)
@@ -82,8 +84,11 @@ def main():
             model = Spann3R(dus3r_name=None)
             model.load_state_dict(sd, strict=True)
             model = model.to(dev)
-    from dust3r.losses import L21          # noqa: the reference's criterion (staged copy)
-    from spann3r.loss import ConfLoss_t, Regr3D_t   # noqa
+    if a.native_criterion:
+        from spann3r_b200.loss import L21, ConfLoss_t, Regr3D_t
+    else:
+        from dust3r.losses import L21          # noqa: the reference's criterion (staged copy)
+        from spann3r.loss import ConfLoss_t, Regr3D_t   # noqa
     criterion = ConfLoss_t(Regr3D_t(L21, norm_mode="avg_dis", fix_first=False), alpha=0.4).to(dev)
     from spann3r_b200 import _native_conv, _native_linear, train
     if a.native_linear:
@@ -145,6 +150,7 @@ def main():
             "gradient_bytes_per_rank": 4 * nparam, "loss_first": l0, "loss_last": l1,
             "backward": "recompute (spann3r_b200/train.py)" if a.impl == "ours" else "PyTorch autograd (reference)",
             "native_backward": native,
+            "criterion": "spann3r_b200.loss (sm_90a)" if a.native_criterion else "reference spann3r/loss.py",
             "forward": "sm_90a kernels (libspann3r_b200.so)" if a.impl == "ours" else "PyTorch eager (reference)",
             "wall_s": time.time() - t0}), flush=True)
     if world > 1:
