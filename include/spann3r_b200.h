@@ -30,8 +30,9 @@ enum { S3R_EPI_PLAIN = 0, S3R_EPI_PIXSHUF = 1, S3R_EPI_QKV = 2, S3R_EPI_HEADTAIL
 enum { S3R_ACT_NONE = 0, S3R_ACT_GELU = 1, S3R_ACT_RELU = 2 };
 
 int s3r_version(void);
-/* sizeof(s3r_gemm_desc / s3r_model_w / s3r_bank / s3r_loss_desc) as compiled: bindings check their mirrors against these */
-int s3r_abi_sizeof(int which /* 0 gemm_desc, 1 model_w, 2 bank, 3 loss_desc */);
+/* sizeof(s3r_gemm_desc / s3r_model_w / s3r_bank / s3r_loss_desc / s3r_attn_train_desc) as compiled: bindings check their
+ * mirrors against these */
+int s3r_abi_sizeof(int which /* 0 gemm_desc, 1 model_w, 2 bank, 3 loss_desc, 4 attn_train_desc */);
 /* last error text of the calling thread ("" if none) */
 const char* s3r_last_error(void);
 /* 1 if a CUDA device of compute capability 9.0 (H100, sm_90a) is visible, else 0 (never falls back to CPU) */
@@ -269,6 +270,29 @@ int s3r_loss_forward(const s3r_loss_desc* d, void* workspace, size_t workspace_b
  * The workspace is the forward's, unchanged since, with the same descriptor. */
 int s3r_loss_backward(const s3r_loss_desc* d, const void* workspace, size_t workspace_bytes, const float* upstream,
                       float* grad_pred, float* grad_conf, void* stream);
+
+/* ---- attention of the training backward: O = softmax(scale Q K^T) V and its gradients (croco/models/blocks.py:106-110,
+ * 162-166 under training), split-bf16 (~fp32-accurate) with no materialised scores: the forward keeps O and one
+ * log-sum-exp per row, the backward rebuilds the probabilities from it.  No float atomics: bitwise reproducible.
+ *   q [batch, heads, nq, dh], k / v [batch, heads, nk, dh]: device fp32, element strides of (batch, head, token) below,
+ *   non-negative multiples of 4, dh contiguous; dh 48 or 64; nq, nk >= 1 (may differ); batch * heads <= 65535. */
+typedef struct s3r_attn_train_desc {
+  int batch, heads, nq, nk, dh;
+  float scale;                       /* softmax scale, dh^-0.5 for the model's attentions */
+  const float* q;
+  const float* k;
+  const float* v;
+  int64_t q_stride[3], k_stride[3], v_stride[3];
+} s3r_attn_train_desc;
+/* bytes of caller-owned device workspace s3r_attn_train_backward needs (a multiple of 256); 0 = invalid descriptor */
+size_t s3r_attn_train_workspace_bytes(const s3r_attn_train_desc* d);
+/* o: fp32 [batch, nq, heads * dh] (head h in columns [h dh, h dh + dh)); lse: fp32 [batch * heads, nq], the natural log
+ * of each row's sum of exp(scale q.k) */
+int s3r_attn_train_forward(const s3r_attn_train_desc* d, float* o, float* lse, void* stream);
+/* d_o: the gradient of o, same layout; o, lse: the forward's outputs -> dq [batch, heads, nq, dh], dk / dv [batch,
+ * heads, nk, dh], contiguous fp32 */
+int s3r_attn_train_backward(const s3r_attn_train_desc* d, const float* o, const float* lse, const float* d_o,
+                            void* workspace, size_t workspace_bytes, float* dq, float* dk, float* dv, void* stream);
 
 /* ---- model level: the per-frame forward path -------------------------------------------------
  * Packed weights.  The host (spann3r_b200/weights.py) converts the reference state dict ONCE into

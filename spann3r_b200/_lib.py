@@ -54,6 +54,15 @@ class LossDesc(C.Structure):
 
 LOSS_RES_HEADER, LOSS_RES_PER_B = 20, 6
 
+
+class AttnTrainDesc(C.Structure):
+    """Mirror of s3r_attn_train_desc."""
+    _fields_ = [
+        ("batch", _i), ("heads", _i), ("nq", _i), ("nk", _i), ("dh", _i), ("scale", _f),
+        ("q", _vp), ("k", _vp), ("v", _vp),
+        ("q_stride", _i64 * 3), ("k_stride", _i64 * 3), ("v_stride", _i64 * 3),
+    ]
+
 _PROTOS = {
     "s3r_version": (_i, []),
     "s3r_abi_sizeof": (_i, [_i]),
@@ -91,6 +100,9 @@ _PROTOS = {
     "s3r_loss_workspace_bytes": (C.c_size_t, [C.POINTER(LossDesc)]),
     "s3r_loss_forward": (_i, [C.POINTER(LossDesc), _vp, C.c_size_t, _vp, _vp, _vp, _vp, _vp]),
     "s3r_loss_backward": (_i, [C.POINTER(LossDesc), _vp, C.c_size_t, _vp, _vp, _vp, _vp]),
+    "s3r_attn_train_workspace_bytes": (C.c_size_t, [C.POINTER(AttnTrainDesc)]),
+    "s3r_attn_train_forward": (_i, [C.POINTER(AttnTrainDesc), _vp, _vp, _vp]),
+    "s3r_attn_train_backward": (_i, [C.POINTER(AttnTrainDesc), _vp, _vp, _vp, _vp, C.c_size_t, _vp, _vp, _vp, _vp]),
     "s3r_resample_h_u8": (_i, [_vp, _i64, _i, _i, _vp, _vp, _i, _i, _vp, _vp]),
     "s3r_resample_v_u8_norm": (_i, [_vp, _i, _i, _vp, _vp, _i, _vp, _vp]),
 }

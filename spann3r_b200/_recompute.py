@@ -3,12 +3,13 @@
 This is NOT a forward path: `Spann3R.forward` always runs the sm_90a kernels (training mode included), and nothing here
 is reachable from eval-mode code.  `torch.autograd.Function.backward` of every stage re-evaluates that stage with these
 differentiable restatements (activation checkpointing at stage granularity) and lets autograd produce the gradients --
-labelled "PyTorch recompute backward" wherever a number from it is reported.  Two switches put the GEMM-shaped ops of the
+labelled "PyTorch recompute backward" wherever a number from it is reported.  Three switches put the tensor-core ops of the
 recompute and of its backward on the library's kernels: every Linear goes through `_lin` (`_native_linear`,
-`train.set_native_linear`), every convolution through `_conv` / `_convT` (`_native_conv`, `train.set_native_conv`).  Both
-are off by default.  Attention, the memory read, LayerNorm, GELU, the upsample, ReLU and the elementwise glue stay PyTorch
-autograd, as do `head.4` (128 -> 4 channels) and anything on the CPU.  Each function cites the reference lines it restates
-(paths relative to the reference root); `tests/test_train_cpu.py` pins them to the oracle on the CPU.
+`train.set_native_linear`), every convolution through `_conv` / `_convT` (`_native_conv`, `train.set_native_conv`), every
+self- and cross-attention through `_attn` (`_native_attn`, `train.set_native_attention`).  All are off by default.  The
+memory read, RoPE, LayerNorm, GELU, the upsample, ReLU and the elementwise glue stay PyTorch autograd, as do `head.4`
+(128 -> 4 channels) and anything on the CPU.  Each function cites the reference lines it restates (paths relative to the
+reference root); `tests/test_train_cpu.py` pins them to the oracle on the CPU.
 
 P: dict parameter name (the reference's state-dict keys) -> tensor.
 """
@@ -17,7 +18,7 @@ from __future__ import annotations
 import torch
 import torch.nn.functional as F
 
-from . import _native_conv, _native_linear
+from . import _native_attn, _native_conv, _native_linear
 
 ENC_HEADS, DEC_HEADS, VAL_HEADS = 16, 12, 16
 
@@ -71,6 +72,15 @@ def _sdpa(q, k, v):
     return a @ v
 
 
+def _attn(q, k, v):
+    """softmax(q k^T / sqrt(dh)) v of q [B, heads, nq, dh], k / v [B, heads, nk, dh], heads merged: -> [B, nq, heads * dh].
+    `_sdpa` and PyTorch autograd by default; with the switch on, the split-bf16 flash kernels (`_native_attn`)."""
+    B, H, N, dh = q.shape
+    if _native_attn.use(q):
+        return _native_attn.attention(q, k, v, dh ** -0.5)
+    return _sdpa(q, k, v).transpose(1, 2).reshape(B, N, H * dh)
+
+
 def _self_attn(P, n, x, heads, cs):
     """croco/models/blocks.py:94-112."""
     B, N, C = x.shape
@@ -78,8 +88,7 @@ def _self_attn(P, n, x, heads, cs):
     q, k, v = qkv[0], qkv[1], qkv[2]
     if cs is not None:
         q, k = _rope(q, cs), _rope(k, cs)
-    o = _sdpa(q, k, v)
-    return _lin(P, n + ".proj", o.transpose(1, 2).reshape(B, N, C))
+    return _lin(P, n + ".proj", _attn(q, k, v))
 
 
 def _cross_attn(P, n, xq, y, heads, cs):
@@ -89,8 +98,7 @@ def _cross_attn(P, n, xq, y, heads, cs):
     q = _lin(P, n + ".projq", xq).view(B, N, heads, dh).transpose(1, 2)
     k = _lin(P, n + ".projk", y).view(B, -1, heads, dh).transpose(1, 2)
     v = _lin(P, n + ".projv", y).view(B, -1, heads, dh).transpose(1, 2)
-    o = _sdpa(_rope(q, cs), _rope(k, cs), v)
-    return _lin(P, n + ".proj", o.transpose(1, 2).reshape(B, N, C))
+    return _lin(P, n + ".proj", _attn(_rope(q, cs), _rope(k, cs), v))
 
 
 def _mlp(P, n, x):

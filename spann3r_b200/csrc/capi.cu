@@ -21,6 +21,7 @@ int s3r_abi_sizeof(int which) {
     case 1: return (int)sizeof(s3r_model_w);
     case 2: return (int)sizeof(s3r_bank);
     case 3: return (int)sizeof(s3r_loss_desc);
+    case 4: return (int)sizeof(s3r_attn_train_desc);
   }
   return -1;
 }
@@ -225,6 +226,15 @@ int s3r_loss_forward(const s3r_loss_desc* d, void* workspace, size_t workspace_b
 int s3r_loss_backward(const s3r_loss_desc* d, const void* workspace, size_t workspace_bytes, const float* upstream,
                       float* grad_pred, float* grad_conf, void* stream) {
   return launch_loss_backward(d, workspace, workspace_bytes, upstream, grad_pred, grad_conf, S(stream));
+}
+
+size_t s3r_attn_train_workspace_bytes(const s3r_attn_train_desc* d) { return attn_train_workspace_bytes(d); }
+int s3r_attn_train_forward(const s3r_attn_train_desc* d, float* o, float* lse, void* stream) {
+  return launch_attn_train_forward(d, o, lse, S(stream));
+}
+int s3r_attn_train_backward(const s3r_attn_train_desc* d, const float* o, const float* lse, const float* d_o,
+                            void* workspace, size_t workspace_bytes, float* dq, float* dk, float* dv, void* stream) {
+  return launch_attn_train_backward(d, o, lse, d_o, workspace, workspace_bytes, dq, dk, dv, S(stream));
 }
 
 int s3r_conf_score(const float* conf, int64_t n, float* scratch256, float* out, void* stream) {

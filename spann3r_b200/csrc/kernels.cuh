@@ -7,6 +7,7 @@
 #include <cuda.h>
 
 struct s3r_loss_desc;   // include/spann3r_b200.h
+struct s3r_attn_train_desc;
 
 namespace s3r {
 
@@ -117,5 +118,12 @@ int launch_loss_backward(const s3r_loss_desc* d, const void* ws, size_t ws_bytes
 // fused attention (attention.cu): O = softmax(Q K^T) V per (batch*head), tf32 wgmma, split-bf16 output
 int launch_attention(const float* q, const float* k, const float* vt, int BH, int heads, int nq, int nk, int nk_pad,
                      __nv_bfloat16* o_hi, __nv_bfloat16* o_lo, float* o_f32, long long ldo, cudaStream_t st);
+
+// attention of the training backward (attention_train.cu): split-bf16 flash forward / backward; validate before any
+// CUDA call
+size_t attn_train_workspace_bytes(const s3r_attn_train_desc* d);
+int launch_attn_train_forward(const s3r_attn_train_desc* d, float* o, float* lse, cudaStream_t st);
+int launch_attn_train_backward(const s3r_attn_train_desc* d, const float* o, const float* lse, const float* d_o,
+                               void* workspace, size_t workspace_bytes, float* dq, float* dk, float* dv, cudaStream_t st);
 
 }  // namespace s3r

@@ -11,8 +11,10 @@ What is native and what is not (said once, here):
   re-evaluates the stage with the differentiable restatement in `_recompute.py` and calls `torch.autograd.grad`.  By
   default that is eager PyTorch throughout.  `set_native_linear(True)` runs every Linear's recompute, dgrad and wgrad on
   the split-bf16 GEMM engine; `set_native_conv(True)` does the same for the convolutions of the DPT heads and the two patch
-  embeddings (wgrad on `s3r_conv_wgrad`).  The two switches are independent and combine.  Attention, the memory read,
-  LayerNorm, GELU, the upsample, ReLU and the elementwise glue stay PyTorch autograd either way.
+  embeddings (wgrad on `s3r_conv_wgrad`); `set_native_attention(True)` runs every self- and cross-attention forward and
+  backward on split-bf16 flash kernels that keep no score matrix (`s3r_attn_train_*`).  The three switches are
+  independent and combine.  The memory read, RoPE, LayerNorm, GELU, the upsample, ReLU and the elementwise glue stay
+  PyTorch autograd either way.
   Gradients reach the `nn.Parameter`s through the Function's parameter inputs, so `DistributedDataParallel`
   (`spann3r/training.py:322-325`) all-reduces them over NCCL like the reference's.
 
@@ -91,6 +93,14 @@ def set_native_conv(on: bool = True):
     instead of `F.conv2d` / `F.conv_transpose2d` + PyTorch autograd.  Independent of `set_native_linear`."""
     from . import _native_conv
     _native_conv.ENABLED = bool(on)
+
+
+def set_native_attention(on: bool = True):
+    """Run the attentions of the backward (recompute forward and its gradients) on the library's split-bf16 flash kernels
+    (`_native_attn.py`) instead of `_sdpa` + PyTorch autograd: fp32-grade whatever `allow_tf32` says, and no
+    [images * heads, N, N] probabilities kept for the backward.  Independent of the other two switches."""
+    from . import _native_attn
+    _native_attn.ENABLED = bool(on)
 
 
 def _apply(native, torch_fn, names, params, *acts):

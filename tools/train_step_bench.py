@@ -2,7 +2,8 @@
 """BASELINE config[4] / SURVEY.md §8d config 5: the reference's DDP training step on synthetic views.
 
     torchrun --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P tools/train_step_bench.py \
-        [--impl ours|reference] [--batch 4] [--frames 10] [--res 224] [--steps 5] [--warmup 2] [--native-linear] [--native-conv] [--native-criterion]
+        [--impl ours|reference] [--batch 4] [--frames 10] [--res 224] [--steps 5] [--warmup 2] [--native-linear] [--native-conv] [--native-attn]
+        [--native-criterion]
 
 One step = `spann3r/training.py:216-228`: forward of a batch of `--batch` sequences per rank -> `ConfLoss_t(Regr3D_t(L21,
 norm_mode='avg_dis', fix_first=False), alpha=0.4).compute_frame_loss` (the REFERENCE's criterion, imported from the staged
@@ -12,8 +13,9 @@ fp32 per rank, `DistributedDataParallel(find_unused_parameters=True, static_grap
 
 --impl ours: `spann3r_b200.Spann3R` in training mode = the sm_90a kernels forward (attn_thresh=0, Philox memory dropout,
 ungated add_mem) + the recompute backward of `spann3r_b200/train.py`: eager PyTorch, except the Linears with --native-linear
-(or S3R_TRAIN_NATIVE_LINEAR=1) and the convolutions with --native-conv (or S3R_TRAIN_NATIVE_CONV=1), which then run on the
-library's kernels.  The JSON line records both switches.  --impl reference: the unmodified reference module, eager PyTorch
+(or S3R_TRAIN_NATIVE_LINEAR=1), the convolutions with --native-conv (or S3R_TRAIN_NATIVE_CONV=1) and the attentions with
+--native-attn (or S3R_TRAIN_NATIVE_ATTN=1), which then run on the library's kernels.  The JSON line records all three
+switches and the step's peak allocated memory.  --impl reference: the unmodified reference module, eager PyTorch
 both ways.
 
 Rank 0 prints one JSON line: steps/s (device time, max over ranks), forward / backward split, and the EXPOSED all-reduce time
@@ -61,6 +63,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--native-linear", action="store_true", help="train.set_native_linear(True)")
     ap.add_argument("--native-conv", action="store_true", help="train.set_native_conv(True)")
+    ap.add_argument("--native-attn", action="store_true", help="train.set_native_attention(True)")
     ap.add_argument("--native-criterion", action="store_true", help="the criterion of spann3r_b200.loss (sm_90a kernels)")
     a = ap.parse_args()
     rank, world, local = (int(os.environ.get(k, d)) for k, d in (("RANK", 0), ("WORLD_SIZE", 1), ("LOCAL_RANK", 0)))
@@ -90,12 +93,15 @@ def main():
         from dust3r.losses import L21          # noqa: the reference's criterion (staged copy)
         from spann3r.loss import ConfLoss_t, Regr3D_t   # noqa
     criterion = ConfLoss_t(Regr3D_t(L21, norm_mode="avg_dis", fix_first=False), alpha=0.4).to(dev)
-    from spann3r_b200 import _native_conv, _native_linear, train
+    from spann3r_b200 import _native_attn, _native_conv, _native_linear, train
     if a.native_linear:
         train.set_native_linear(True)
     if a.native_conv:
         train.set_native_conv(True)
-    native = {"linear": bool(_native_linear.ENABLED), "conv": bool(_native_conv.ENABLED)} if a.impl == "ours" else None
+    if a.native_attn:
+        train.set_native_attention(True)
+    native = ({"linear": bool(_native_linear.ENABLED), "conv": bool(_native_conv.ENABLED),
+               "attention": bool(_native_attn.ENABLED)} if a.impl == "ours" else None)
     model.train()
     ddp = model
     if world > 1:
@@ -137,7 +143,9 @@ def main():
     t0 = time.time()
     for _ in range(a.warmup):
         l0 = float(step(True))
+    torch.cuda.reset_peak_memory_stats(dev)
     (ms, fwd, bwd), l1 = timed(a.steps, True)
+    peak = torch.cuda.max_memory_allocated(dev)
     (ms_ns, _, _), _ = timed(max(2, a.steps // 2), False) if world > 1 else ((ms, 0, 0), 0)
     if rank == 0:
         nparam = sum(p.numel() for p in model.parameters())
@@ -149,7 +157,7 @@ def main():
             "ms_per_step_no_sync": ms_ns, "exposed_allreduce_ms": max(0.0, ms - ms_ns) if world > 1 else None,
             "gradient_bytes_per_rank": 4 * nparam, "loss_first": l0, "loss_last": l1,
             "backward": "recompute (spann3r_b200/train.py)" if a.impl == "ours" else "PyTorch autograd (reference)",
-            "native_backward": native,
+            "native_backward": native, "peak_allocated_gb": peak / 2 ** 30,
             "criterion": "spann3r_b200.loss (sm_90a)" if a.native_criterion else "reference spann3r/loss.py",
             "forward": "sm_90a kernels (libspann3r_b200.so)" if a.impl == "ours" else "PyTorch eager (reference)",
             "wall_s": time.time() - t0}), flush=True)
