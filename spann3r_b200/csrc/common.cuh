@@ -181,6 +181,20 @@ __device__ __forceinline__ uint64_t wgmma_desc_sw128_kmajor(uint32_t smem_addr) 
   return d;
 }
 
+// The same for rows of exactly one 64-byte swizzle span (32 bf16), stored as TMA SWIZZLE_64B wrote it:
+//   stride offset  = 8 rows x 64 B = 512 B >> 4 = 32
+//   layout type    = 2 (SWIZZLE_64B)
+// Tiles start on 512-byte boundaries (base offset 0).  Each k16 step adds 32 bytes (2 in the start field); stepping
+// 64 rows = adding 4 KB.
+__device__ __forceinline__ uint64_t wgmma_desc_sw64_kmajor(uint32_t smem_addr) {
+  uint64_t d = 0;
+  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
+  d |= (uint64_t)1 << 16;
+  d |= (uint64_t)32 << 32;
+  d |= (uint64_t)2 << 62;
+  return d;
+}
+
 // ----------------------------------------------------------------------------------------------
 // Programmatic dependent launch (PDL): every kernel of the library is launched with
 // cudaLaunchAttributeProgrammaticStreamSerialization, signals its dependents at once and waits for

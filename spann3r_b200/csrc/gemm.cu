@@ -9,10 +9,11 @@
 //
 // Structure: persistent, warp-specialised, one CTA per SM, 128 x BN output tiles.
 //   warpgroup 0   TMA producer (one warp; registers handed to the consumers with setmaxnreg): per k-block four
-//                 SWIZZLE_128B boxes (A_hi, A_lo: 128 pixels x 64 ch; B_hi, B_lo: BN x 64) into a STAGES-deep smem
-//                 ring; a 3x3 conv is 9 taps whose A box is the same 4-D tensor map at (w+dx, h+dy) -- out-of-bounds
-//                 pixels are zero-filled by TMA, which is exactly the conv's zero padding.
-//   warpgroups 1, 2  consumers: each owns 64 rows of the tile and issues per k-block 4 K-steps x 3 wgmma (hi*lo,
+//                 SWIZZLE_64B boxes (A_hi, A_lo: 128 pixels x 32 ch; B_hi, B_lo: BN x 32) into a STAGES-deep smem
+//                 ring (5 stages at BN = 128, 7 at BN = 64); a 3x3 conv is 9 taps whose A box is the same 4-D tensor
+//                 map at (w+dx, h+dy) -- out-of-bounds pixels are zero-filled by TMA, which is exactly the conv's zero
+//                 padding.
+//   warpgroups 1, 2  consumers: each owns 64 rows of the tile and issues per k-block 2 K-steps x 3 wgmma (hi*lo,
 //                 lo*hi, hi*hi) into a 64 x BN fp32 register accumulator, one k-block in flight.  The epilogue is run
 //                 by the same 8 warps: the accumulator goes through shared memory 2 x 32 columns at a time into the
 //                 thread = tile row layout of gemm_epilogue.cuh (fused bias / GELU / ReLU / residual adds / split-bf16
@@ -32,7 +33,11 @@
 namespace s3r {
 
 static constexpr int BM = 128;
-static constexpr int BK = 64;
+// 32-channel k-blocks: one 64-byte swizzle span per row.  A stage is then 32 KB at BN = 128, so the ring is 5 deep;
+// the consumers hold 2 stages (the k-block being issued and the one retiring), which leaves 3 k-blocks of loads in
+// flight to cover the TMA / L2 latency (64-channel k-blocks fit only 2 stages at BN = 128: at most 1 in flight).
+static constexpr int BK = 32;
+static constexpr CUtensorMapSwizzle kSwizzle = CU_TENSOR_MAP_SWIZZLE_64B;   // BK * 2 bytes per row
 static constexpr int kEpiWarps = 8;     // the two consumer warpgroups
 static constexpr int kNumThreads = 128 + 32 * kEpiWarps;
 static constexpr int kSmemMax = 227 * 1024;
@@ -49,7 +54,7 @@ struct GemmCfg {
   static constexpr int FIXED = 1024 /*align slack*/ + 256 /*barriers*/ + kAccBytes + COLV + HT;
   static constexpr int STAGES = (kSmemMax - FIXED) / STAGE;
   static constexpr int SMEM = STAGES * STAGE + FIXED;
-  static_assert(STAGES >= 2, "smem ring");
+  static_assert(STAGES == (BN == 128 ? 5 : 7), "ring depth (DESIGN.md §4)");
   static_assert(Stg<32>::WARP_BYTES == 32 * kAccLD * 4, "a warp's staging tile is its own rows of the accumulator chunk");
 };
 
@@ -206,9 +211,9 @@ __global__ void __launch_bounds__(kNumThreads, 1) gemm_bf16x3_kernel(const __gri
       EpiRow er;
       EpiTRows tr;
       epi_tile_pre<EPI, 32>(args, tg, quad, lane, er, tr);
-      float4 rcur[8], rnxt[8];
+      float4 res[8];
       const int cfirst = nt * BN + half * CH * 32;
-      if (cfirst < args.N) epi_prefetch_res<EPI, 32>(args, tr, rcur, cfirst, lane);
+      if (cfirst < args.N) epi_prefetch_res<EPI, 32>(args, tr, res, cfirst, lane);
       // staged columns visible to all consumer warps; every warp is also done with the previous tile's staging buffer
       asm volatile("bar.sync 1, %0;" ::"n"(32 * kEpiWarps) : "memory");
 
@@ -220,10 +225,10 @@ __global__ void __launch_bounds__(kNumThreads, 1) gemm_bf16x3_kernel(const __gri
         mbar_wait(&full_bar[stage], phase);
         if (trace && kb == 0 && it == 0 && threadIdx.x == 128) trace[3] = globaltimer_ns();
         const uint32_t sa = smem_u + stage * Cfg::STAGE;
-        const uint64_t da_hi = wgmma_desc_sw128_kmajor(sa + wg * (64 * BK * 2));
-        const uint64_t da_lo = wgmma_desc_sw128_kmajor(sa + Cfg::A_TILE + wg * (64 * BK * 2));
-        const uint64_t db_hi = wgmma_desc_sw128_kmajor(sa + 2 * Cfg::A_TILE);
-        const uint64_t db_lo = wgmma_desc_sw128_kmajor(sa + 2 * Cfg::A_TILE + Cfg::B_TILE);
+        const uint64_t da_hi = wgmma_desc_sw64_kmajor(sa + wg * (64 * BK * 2));
+        const uint64_t da_lo = wgmma_desc_sw64_kmajor(sa + Cfg::A_TILE + wg * (64 * BK * 2));
+        const uint64_t db_hi = wgmma_desc_sw64_kmajor(sa + 2 * Cfg::A_TILE);
+        const uint64_t db_lo = wgmma_desc_sw64_kmajor(sa + 2 * Cfg::A_TILE + Cfg::B_TILE);
         wgmma_fence();
 #pragma unroll
         for (int kk = 0; kk < BK / 16; ++kk) {
@@ -283,10 +288,8 @@ __global__ void __launch_bounds__(kNumThreads, 1) gemm_bf16x3_kernel(const __gri
         const int c = half * CH + cc;
         const int col0 = nt * BN + c * 32;
         if (col0 < args.N) {   // warp-uniform
-          if (cc + 1 < CH && col0 + 32 < args.N) epi_prefetch_res<EPI, 32>(args, tr, rnxt, col0 + 32, lane);
-          epi_chunk<EPI, 32>(args, v, sb + c * 32, scs + c * 32, myrows, tg, er, tr, rcur, col0, lane, ht_acc);
-#pragma unroll
-          for (int q = 0; q < 8; ++q) rcur[q] = rnxt[q];
+          const int res_next = (cc + 1 < CH && col0 + 32 < args.N) ? col0 + 32 : -1;
+          epi_chunk<EPI, 32>(args, v, sb + c * 32, scs + c * 32, myrows, tg, er, tr, res, col0, res_next, lane, ht_acc);
         }
       }
 
@@ -336,9 +339,9 @@ static PFN_encodeTiled get_encode() {
   return fn;
 }
 
-// dims/box innermost-first; strides_bytes has rank-1 entries (dims 1..rank-1). Always SWIZZLE_128B.
+// dims/box innermost-first; strides_bytes has rank-1 entries (dims 1..rank-1).
 int encode_tmap(CUtensorMap* out, CUtensorMapDataType dt, int rank, const void* base, const uint64_t* dims,
-                const uint64_t* strides_bytes, const uint32_t* box) {
+                const uint64_t* strides_bytes, const uint32_t* box, CUtensorMapSwizzle swizzle) {
   PFN_encodeTiled enc = get_encode();
   if (!enc) {
     set_error("cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
@@ -353,7 +356,7 @@ int encode_tmap(CUtensorMap* out, CUtensorMapDataType dt, int rank, const void* 
   }
   for (int i = 0; i + 1 < rank; ++i) s[i] = strides_bytes[i];
   CUresult r = enc(out, dt, (cuuint32_t)rank, const_cast<void*>(base), d, s, b, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                   swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_error("cuTensorMapEncodeTiled failed: %d (rank %d dims %llu %llu %llu %llu box %u %u %u %u base %p)", (int)r,
               rank, (unsigned long long)d[0], (unsigned long long)(rank > 1 ? d[1] : 0),
@@ -413,7 +416,7 @@ int gemm_plan_init(GemmPlan* plan, const __nv_bfloat16* a_hi, const __nv_bfloat1
   a.tiles_h = (H + a.bh - 1) / a.bh;
   a.out_group_rows = (long long)NB * H * W;
   // Tile shape: 128 x 64 or 128 x 128, the cheaper under makespan = waves x (bytes staged per k-block), with waves =
-  // ceil(tiles / SMs) for the persistent static schedule and 48 KB (128 x 64) / 64 KB (128 x 128) staged per k-block.
+  // ceil(tiles / SMs) for the persistent static schedule and 24 KB (128 x 64) / 32 KB (128 x 128) staged per k-block.
   // A 64-row warpgroup holds a 64 x BN fp32 accumulator in registers next to the epilogue's working set, so 128 is the
   // widest tile; wider requests (force_bn 256, and 2064 / 2128 / 2256, the tile widths of CTA-pair kernels on other
   // architectures) run at the nearest width the kernel has.
@@ -421,8 +424,8 @@ int gemm_plan_init(GemmPlan* plan, const __nv_bfloat16* a_hi, const __nv_bfloat1
   const int sms = num_sms();
   auto waves = [](long long tiles, long long slots) { return (double)((tiles + slots - 1) / slots); };
   const long long nt64 = (N + 63) / 64, nt128 = (N + 127) / 128;
-  const double c64 = waves(m_tiles * nt64, sms) * 48.0;
-  const double c128 = (N > 64) ? waves(m_tiles * nt128, sms) * 64.0 : 1e30;
+  const double c64 = waves(m_tiles * nt64, sms) * 24.0;
+  const double c128 = (N > 64) ? waves(m_tiles * nt128, sms) * 32.0 : 1e30;
   int bn = (c128 <= c64) ? 128 : 64;
   int fb = force_bn >= 2000 ? force_bn - 2000 : force_bn == 1128 ? 128 : force_bn;
   if (fb > 0) {
@@ -440,8 +443,8 @@ int gemm_plan_init(GemmPlan* plan, const __nv_bfloat16* a_hi, const __nv_bfloat1
     uint64_t str[3] = {(uint64_t)lda * esz, (uint64_t)lda * W * esz, (uint64_t)lda * W * H * esz};
     uint32_t box[4] = {(uint32_t)BK, (uint32_t)a.bw, (uint32_t)a.bh, 1};
     int r;
-    if ((r = encode_tmap(&a.tmA_hi, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, a_hi, dims, str, box))) return r;
-    if ((r = encode_tmap(&a.tmA_lo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, a_lo, dims, str, box))) return r;
+    if ((r = encode_tmap(&a.tmA_hi, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, a_hi, dims, str, box, kSwizzle))) return r;
+    if ((r = encode_tmap(&a.tmA_lo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, a_lo, dims, str, box, kSwizzle))) return r;
   }
   {
     uint64_t dims[3] = {(uint64_t)Kc, (uint64_t)taps, (uint64_t)(b_group_rows * (groups - 1) + N)};
@@ -449,8 +452,8 @@ int gemm_plan_init(GemmPlan* plan, const __nv_bfloat16* a_hi, const __nv_bfloat1
     uint64_t str[2] = {(uint64_t)(taps == 1 ? ldb : Kc) * esz, (uint64_t)ldb * esz};
     uint32_t box[3] = {(uint32_t)BK, 1, (uint32_t)bn};
     int r;
-    if ((r = encode_tmap(&a.tmB_hi, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, b_hi, dims, str, box))) return r;
-    if ((r = encode_tmap(&a.tmB_lo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, b_lo, dims, str, box))) return r;
+    if ((r = encode_tmap(&a.tmB_hi, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, b_hi, dims, str, box, kSwizzle))) return r;
+    if ((r = encode_tmap(&a.tmB_lo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, b_lo, dims, str, box, kSwizzle))) return r;
   }
   const long long n_tiles = (N + bn - 1) / bn;
   const long long total = m_tiles * n_tiles;

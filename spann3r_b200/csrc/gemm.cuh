@@ -29,7 +29,7 @@ struct GemmArgs {
   int bw, bh;          // tile box, bw*bh == 128
   int tiles_w, tiles_h;
   int N;               // output columns per group
-  int Kc, taps, kpt;   // channels per tap, 1 or 9 taps, k-blocks (of 64) per tap
+  int Kc, taps, kpt;   // channels per tap, 1 or 9 taps, k-blocks (of 32) per tap
   int b_group_rows;    // B rows between groups
   // epilogue
   int epi, act, plane_relu;
@@ -98,7 +98,8 @@ Options& options();
 int num_sms();
 
 int encode_tmap(CUtensorMap* out, CUtensorMapDataType dt, int rank, const void* base, const uint64_t* dims,
-                const uint64_t* strides_bytes, const uint32_t* box);
+                const uint64_t* strides_bytes, const uint32_t* box,
+                CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B);
 const char* last_error();
 void set_error(const char* fmt, ...);
 

@@ -172,7 +172,8 @@ __device__ __forceinline__ void epi_tile_pre(const GemmArgs& args, const TileGeo
   }
 }
 
-// Residual values of one 32-column chunk in the transposed layout (EPI_PLAIN; requested one chunk ahead).
+// Residual values of a tile's first 32-column chunk in the transposed layout (EPI_PLAIN; epi_chunk requests each
+// following chunk's values as it consumes the current ones).
 template <int EPI, int SW>
 __device__ __forceinline__ void epi_prefetch_res(const GemmArgs& args, const EpiTRows& tr, float4 (&rp)[8], int col0,
                                                  int lane) {
@@ -191,11 +192,13 @@ __device__ __forceinline__ void epi_prefetch_res(const GemmArgs& args, const Epi
 }
 
 // One 32-column chunk.  v: this thread's accumulator row; sb / scs: the chunk's staged bias / colsum values; stg: the
-// warp's staging tile; rp: prefetched residual (transposed layout); ht_acc: running dot products of EPI_HEADTAIL.
+// warp's staging tile; rp: prefetched residual (transposed layout), refilled slot by slot with the residual of the
+// chunk at column res_next (EPI_PLAIN; -1 = none), so one buffer serves every chunk with the next one's loads in flight;
+// ht_acc: running dot products of EPI_HEADTAIL.
 template <int EPI, int SW>
 __device__ __forceinline__ void epi_chunk(const GemmArgs& args, float (&v)[32], const float* sb, const float* scs,
                                           float* stg, const TileGeom& tg, const EpiRow& er, const EpiTRows& tr,
-                                          const float4 (&rp)[8], int col0, int lane, float (&ht_acc)[4]) {
+                                          float4 (&rp)[8], int col0, int res_next, int lane, float (&ht_acc)[4]) {
   // ---------------------------------------------------------------- row domain
   if (args.ln_stats != nullptr) {
     const float4* c4 = reinterpret_cast<const float4*>(scs);
@@ -332,8 +335,12 @@ __device__ __forceinline__ void epi_chunk(const GemmArgs& args, float (&v)[32], 
         if (ok) {
           if (args.res1 != nullptr) {
             float4 t;
-            if constexpr (EPI == EPI_PLAIN) t = rp[p * S::NIT + it];
-            else t = ld_f4(args.res1 + orow * args.ldr1 + ocol);
+            if constexpr (EPI == EPI_PLAIN) {
+              t = rp[p * S::NIT + it];
+              if (res_next >= 0) rp[p * S::NIT + it] = ld_f4(args.res1 + orow * args.ldr1 + res_next + p * SW + cq);
+            } else {
+              t = ld_f4(args.res1 + orow * args.ldr1 + ocol);
+            }
             x.x += t.x; x.y += t.y; x.z += t.z; x.w += t.w;
           }
           if (args.res2 != nullptr) {
