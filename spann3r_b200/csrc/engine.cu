@@ -869,6 +869,11 @@ int s3r_engine_memory_read_train(s3r_engine* e, const s3r_bank* bank, const floa
     set_error("s3r_engine_memory_read: bad bank (len=%d cap=%d; cap must be a multiple of 8)", M, cap);
     return -1;
   }
+  if (M > MEM_SOFTMAX_MAX_LEN) {  // before any allocation or launch: the softmax keeps a whole score row in shared memory
+    set_error("s3r_engine_memory_read: bank of %d tokens exceeds the %d-token row buffer of the softmax", M,
+              MEM_SOFTMAX_MAX_LEN);
+    return -1;
+  }
   if (cap > e->mem_cap) {  // (re)size the score / probability scratch for this bank capacity (rare)
     e->release(e->Sm); e->release(e->Pm.hi); e->release(e->Pm.lo);   // the old scratch is dead: no stage is in flight on it
     e->Sm = e->alloc<float>((size_t)B * N * cap);                    // that a later launch of this stream could overtake

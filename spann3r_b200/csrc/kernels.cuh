@@ -51,6 +51,8 @@ int attn_launch(const AttnPlan& plan, __nv_bfloat16* o_hi, __nv_bfloat16* o_lo, 
                 cudaStream_t st);
 
 // spatial memory (memory.cu)
+// longest bank the softmax takes: one fp32 score row in shared memory, up to 200 KB of it
+constexpr int MEM_SOFTMAX_MAX_LEN = 200 * 1024 / 4;
 int launch_mem_softmax(const float* S, long long ldS, long long rows, int M, int Mpad, float scale, float thresh,
                        __nv_bfloat16* phi, __nv_bfloat16* plo, long long ldP, cudaStream_t st, float drop_p = 0.f,
                        unsigned long long seed = 0);

@@ -169,18 +169,25 @@ int launch_mem_softmax(const float* S, long long ldS, long long rows, int M, int
                        unsigned long long seed) {
   if (rows == 0 || M == 0) return 0;
   const size_t smem = (size_t)M * sizeof(float);
-  if (smem > 200 * 1024) {
-    set_error("mem_softmax: bank of %d tokens exceeds the 51200-token row buffer", M);
+  if (M > MEM_SOFTMAX_MAX_LEN) {
+    set_error("mem_softmax: bank of %d tokens exceeds the %d-token row buffer", M, MEM_SOFTMAX_MAX_LEN);
     return -1;
   }
+  // Opt in to the large row buffer on first use, whatever this call's size: the kernel's static shared memory counts
+  // against the same 48 KB default, so a row of exactly 48 KB (12288 tokens) already needs it.
   static PerDeviceOnce once;
-  if (smem > 48 * 1024 && !once.cur()) {
-    cudaFuncSetAttribute(mem_softmax_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+  if (!once.cur()) {
+    cudaFuncSetAttribute(mem_softmax_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, MEM_SOFTMAX_MAX_LEN * 4);
     once.cur() = true;
   }
   launch_pdl(mem_softmax_kernel, dim3((unsigned)rows), dim3(256), smem, st, S, ldS, M, Mpad, scale, thresh, phi, plo, ldP,
              drop_p, (float)(1.0 / (1.0 - (double)drop_p)), seed);
-  return cudaGetLastError() == cudaSuccess ? 0 : -6;
+  const cudaError_t err = cudaGetLastError();
+  if (err != cudaSuccess) {
+    set_error("mem_softmax: launch of %d rows x %d tokens failed: %s", (int)rows, M, cudaGetErrorString(err));
+    return -6;
+  }
+  return 0;
 }
 
 // ------------------------------------------------------------------------------------------------

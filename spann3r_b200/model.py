@@ -203,7 +203,9 @@ class SpatialMemory:
         not change in between), same value, same decision."""
         if self.bank is None or self.bank.len == 0 or thresh == 1.0:
             return None
-        mean_corr = self.engine.check_sim(self.bank, feat_k, self.wm)
+        # the window is the last wm * P tokens, or the whole bank when a prune to long_mem_size < wm * P tokens left
+        # fewer (mem_k[:, -wm * P:] of the reference)
+        mean_corr = self.engine.check_sim(self.bank, feat_k, min(self.wm, self.bank.len // self.num_patches))
         if self._sim_host is None:
             self._sim_host = torch.empty(1, dtype=torch.float32, pin_memory=True)
         self._sim_host.copy_(mean_corr.max().reshape(1), non_blocking=True)
