@@ -41,6 +41,7 @@ int s3r_device_ok(void);
 /* ---- op level ------------------------------------------------------------------------------ */
 
 /* fp32 [rows, c] (row stride ldx) -> planes [rows, ldp] at column col0, optional ReLU first.
+ * c, ldx, ldp and col0 are multiples of 4 (16-byte loads, 8-byte stores).
  * Replaces nothing in the reference; it is the format conversion at the head of a GEMM chain. */
 int s3r_split(const float* x, int64_t ldx, void* hi, void* lo, int64_t ldp, int col0, int64_t rows, int c, int relu,
               void* stream);
@@ -49,8 +50,9 @@ int s3r_split(const float* x, int64_t ldx, void* hi, void* lo, int64_t ldp, int 
  * croco/models/blocks.py:116-130,176-191 (norm1/2/3/norm_y, eps 1e-6), dust3r/model.py:151,203
  * (enc_norm, dec_norm), spann3r/model.py:245-247 (norm_q/k/v, eps 1e-5).
  * Groups: row r uses weight set (r / rows_per_group) at w + set*wb_group_stride (0 = one set).
- * swap_rows > 0: two groups of swap_rows rows; output rows and weight sets are exchanged between
- * the groups (the twin decoders' norm_y, dust3r/model.py:197-199). */
+ * swap_rows > 0: two groups of swap_rows rows (rows == 2 * swap_rows, rows_per_group == swap_rows); output rows
+ * and weight sets are exchanged between the groups (the twin decoders' norm_y, dust3r/model.py:197-199).
+ * ldx, wb_group_stride, ldo (with out), ldp and col0 (with planes) are multiples of 4. */
 int s3r_layernorm(const float* x, int64_t ldx, const float* w, const float* b, int64_t wb_group_stride,
                   int64_t rows_per_group, float eps, int64_t rows, int c, float* out, int64_t ldo, void* hi, void* lo,
                   int64_t ldp, int col0, int64_t swap_rows, void* stream);
@@ -65,7 +67,7 @@ int s3r_rope2d_inplace(float* tokens, const int64_t* pos, int64_t bn, int h, int
  * planes [b*gh*gw, 768], k = c*256 + i*16 + j.  dust3r/patch_embed.py:19-29. */
 int s3r_im2col_patch16(const float* img, int64_t sb, int64_t sc, int64_t sy, int64_t sx, int b, int gh, int gw,
                        void* hi, void* lo, void* stream);
-/* im2col for Conv2d(C, C, 3, stride 2, pad 1): planes [nb,h,w,c] -> planes [nb*ho*wo, 9*c].
+/* im2col for Conv2d(C, C, 3, stride 2, pad 1): planes [nb,h,w,c] -> planes [nb*ho*wo, 9*c], c a multiple of 8.
  * croco/models/dpt_block.py:396-408 (act_4_postprocess). */
 int s3r_im2col_3x3s2(const void* ihi, const void* ilo, int nb, int h, int w, int c, int ho, int wo, void* ohi,
                      void* olo, void* stream);
@@ -96,7 +98,11 @@ int s3r_col2im_3x3s2(const float* cols, int nb, int h, int w, int c, int ho, int
  *   A planes [groups*nb, h, w, kc] (a linear layer is h = 1, w = rows), B planes [groups*n, taps, kc],
  *   taps = 1 (linear / 1x1 conv / ConvTranspose with kernel == stride) or 9 (3x3, stride 1, pad 1).
  * Replaces nn.Linear / Conv2d / ConvTranspose2d calls of croco/models/blocks.py:73-79,94-112,149-169,
- * dust3r/model.py:189-190, spann3r/model.py:250-261,310 and croco/models/dpt_block.py (all convs). */
+ * dust3r/model.py:189-190, spann3r/model.py:250-261,310 and croco/models/dpt_block.py (all convs).
+ * n is a multiple of 32 (the epilogue stores whole 32-column chunks).  ldr1, ldr2, ldo, ldp and plane_col0 are
+ * non-negative multiples of 4 below 2^31 (16-byte residual / fp32 accesses, 8-byte plane stores); res1 may be
+ * out_f32 with ldr1 == ldo (in-place residual, as the engine's proj / cproj / fc2 launches).  Every rule is
+ * checked before the driver is touched: a rejected descriptor returns -1 and names the field in s3r_last_error(). */
 typedef struct s3r_gemm_desc {
   const void* a_hi; const void* a_lo;
   const void* b_hi; const void* b_lo;
@@ -112,7 +118,11 @@ typedef struct s3r_gemm_desc {
   /* S3R_EPI_QKV: columns are q_c-wide roles starting at q_role_base (0 q, 1 k, 2 v); q,k get 2-D RoPE
    * from q_pos ([groups*rows, 2] int32 (y, x)) and the (cos, sin) table q_cs [maxpos, 16, 2]; q is scaled by
    * q_scale; outputs q_out/k_out [groups*q_nb, heads, q_ntok, 64], vt_out [groups*q_nb, heads, 64, q_ntok_pad],
-   * all rounded to tf32.  croco/models/blocks.py:97-104,154-160 + models/pos_embed.py:112-159. */
+   * all rounded to tf32.  n is a multiple of q_c with q_role_base + n/q_c <= 5, and the output of every role the
+   * columns reach is non-NULL; q_ntok <= q_ntok_pad, a multiple of 4 (columns q_ntok.. of V^T are left untouched);
+   * q_rope needs q_pos and q_cs.  Under a_swap the positions of a row follow its A operand: columns >= swap_col0 of
+   * group g are rotated by the positions of group groups-1-g (the other stream's tokens, as the cross-attention k).
+   * croco/models/blocks.py:97-104,154-160 + models/pos_embed.py:112-159. */
   int q_c, q_role_base, q_ntok, q_ntok_pad, q_rope, q_nb;
   const int32_t* q_pos; const float* q_cs;
   float* q_out; float* k_out; float* vt_out; float q_scale;
@@ -123,7 +133,11 @@ typedef struct s3r_gemm_desc {
   /* Folded LayerNorm (croco/models/blocks.py:127-130,186-191: every Linear that follows a LayerNorm).  Consumer:
    * A = planes of the RAW residual stream x, B = planes of W diag(gamma), bias = b + W beta, ln_cs [groups*n] = row
    * sums of the B planes (hi + lo), ln_stats [A rows, ln_np] float2 (sum, sum of squares) per 32-column chunk of x
-   * (ln_np = kc/32); the epilogue applies rstd_r * (acc - mean_r * ln_cs[col]) + bias = LN(x) W^T + b.
+   * (ln_np = kc/32, even and <= 32: kc % 64 == 0, kc <= 1024, taps == 1); the epilogue applies
+   * rstd_r * (acc - mean_r * ln_cs[col]) + bias = LN(x) W^T + b.  The variance is E[x^2] - mean^2 in fp32 from these
+   * one-pass sums, and the GEMM runs on the raw x, so the error grows with |mean_r| / std_r: rows up to 3 are held to
+   * the GEMM's 3e-5 relative error (tests/test_epilogue_gpu.py); every folded LayerNorm input of the model stays
+   * below 0.11 (both synthetic checkpoints).
    * a_swap = 1: group g reads A rows / statistics of group groups-1-g (norm_y of the twin decoders,
    * dust3r/model.py:197-199).  Producer (EPI_PLAIN, n % 32 == 0): stats_out [rows, n/32] float2 receives the chunk
    * sums of the rows it writes.  All NULL / 0 = plain GEMM. */
@@ -143,7 +157,8 @@ int s3r_gemm_tile_n(const s3r_gemm_desc* d);
 
 /* Fused multi-head attention core, head dim 64: O = softmax(Q K^T) V per (batch*head) on tf32 wgmma.
  *   q [bh, nq, 64], k [bh, nk, 64] (already RoPE'd / scaled by the QKV epilogue), vt [bh, 64, nk_pad];
- *   output [b*nq, heads*64] as planes and/or fp32 (row stride ldo).
+ *   output [b*nq, heads*64] as planes and/or fp32 (row stride ldo, even); bh a multiple of heads; nk_pad >= nk, a
+ *   multiple of 4: columns nk .. nk_pad-1 of vt are never read.
  * croco/models/blocks.py:106-110 (self), :162-166 (cross). */
 int s3r_attention(const float* q, const float* k, const float* vt, int bh, int heads, int nq, int nk, int nk_pad,
                   void* o_hi, void* o_lo, float* o_f32, int64_t ldo, void* stream);

@@ -285,6 +285,10 @@ int attn_launch(const AttnPlan& plan, __nv_bfloat16* o_hi, __nv_bfloat16* o_lo, 
 
 int launch_attention(const float* q, const float* k, const float* vt, int BH, int heads, int nq, int nk, int nk_pad,
                      __nv_bfloat16* o_hi, __nv_bfloat16* o_lo, float* o_f32, long long ldo, cudaStream_t st) {
+  if (heads <= 0 || BH % heads != 0 || ldo % 2 != 0) {
+    set_error("attention: bh=%d must be a multiple of heads=%d, and ldo=%lld even (paired stores)", BH, heads, ldo);
+    return -1;
+  }
   if (nq <= 0 || nk <= 0 || BH <= 0) return 0;
   AttnPlan plan;
   int r = attn_plan_init(&plan, q, k, vt, BH, heads, nq, nk, nk_pad);

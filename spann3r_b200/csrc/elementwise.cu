@@ -38,6 +38,10 @@ __global__ void split_kernel(const float* __restrict__ x, long long ldx, __nv_bf
 int launch_split(const float* x, long long ldx, __nv_bfloat16* hi, __nv_bfloat16* lo, long long ldp, int col0,
                  long long rows, int C, int relu, cudaStream_t st) {
   if (C % 4) { set_error("split: C %% 4 != 0"); return -1; }
+  if (ldx % 4 || ldp % 4 || col0 < 0 || col0 % 4) {
+    set_error("split: ldx=%lld, ldp=%lld and col0=%d must be non-negative multiples of 4 (vector accesses)", ldx, ldp, col0);
+    return -1;
+  }
   const long long total = rows * (C / 4);
   if (total == 0) return 0;
   int blocks = (int)((total + 255) / 256);
@@ -165,6 +169,16 @@ int launch_layernorm(const float* x, long long ldx, const float* w, const float*
                      long long rows_per_group, float eps, long long rows, int C, float* out, long long ldo,
                      __nv_bfloat16* hi, __nv_bfloat16* lo, long long ldp, int col0, long long swap_rows,
                      cudaStream_t st) {
+  if (swap_rows > 0 && (rows != 2 * swap_rows || rows_per_group != swap_rows)) {
+    set_error("layernorm: swap_rows=%lld needs rows == 2*swap_rows and rows_per_group == swap_rows (rows=%lld, "
+              "rows_per_group=%lld)", swap_rows, rows, rows_per_group);
+    return -1;
+  }
+  if (ldx % 4 || wb_group_stride % 4 || (out && ldo % 4) || (hi && (ldp % 4 || col0 < 0 || col0 % 4))) {
+    set_error("layernorm: ldx=%lld, wb_group_stride=%lld, ldo=%lld, ldp=%lld and col0=%d must be multiples of 4 (vector "
+              "accesses)", ldx, wb_group_stride, ldo, ldp, col0);
+    return -1;
+  }
   if (rows == 0) return 0;
   const int wpb = 8;
   dim3 grid((unsigned)((rows + wpb - 1) / wpb)), block(wpb * 32);
@@ -268,6 +282,7 @@ __global__ void im2col_3x3s2_kernel(const __nv_bfloat16* __restrict__ ihi, const
 
 int launch_im2col_3x3s2(const __nv_bfloat16* ihi, const __nv_bfloat16* ilo, int NB, int H, int W, int C, int Ho, int Wo,
                         __nv_bfloat16* ohi, __nv_bfloat16* olo, cudaStream_t st) {
+  if (C <= 0 || C % 8) { set_error("im2col_3x3s2: C=%d must be a positive multiple of 8 (16-byte copies)", C); return -1; }
   const long long total = (long long)NB * Ho * Wo * 9 * (C / 8);
   if (total == 0) return 0;
   int blocks = (int)((total + 255) / 256);

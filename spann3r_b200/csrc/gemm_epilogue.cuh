@@ -142,9 +142,10 @@ __device__ __forceinline__ void epi_tile_pre(const GemmArgs& args, const TileGeo
     er.rm = er.rstd * mean;
   }
   if constexpr (EPI == EPI_QKV) {
-    if (args.q_rope && er.valid) {
-      er.py = args.q_pos[er.grow * 2];
-      er.px = args.q_pos[er.grow * 2 + 1];
+    if (args.q_rope && er.valid) {   // positions of the token whose row is the A operand (group ga under a_swap)
+      const long long prow = (long long)tg.ga * args.out_group_rows + er.pix;
+      er.py = args.q_pos[prow * 2];
+      er.px = args.q_pos[prow * 2 + 1];
     }
   }
   if constexpr (EPI != EPI_HEADTAIL) {
