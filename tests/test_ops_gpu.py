@@ -183,8 +183,8 @@ def test_qkv_rope_attention(L, B, gh, gw, heads, groups):
 
 @pytest.mark.parametrize("BH,heads,nq,nk", [
     (6, 3, 196, 300),
-    # many-wave launches take the query-tile-pair variant (two tiles per CTA, no merge): full / ragged key blocks,
-    # ragged last query tile, a single key block
+    # many-wave launches (one CTA per 128-query tile and head): full / ragged key blocks, ragged last query tile, a
+    # single key block.  tests/test_attention_core_gpu.py holds the kernel to a per-element bound.
     (96, 16, 768, 768), (128, 16, 512, 300), (160, 16, 700, 768), (256, 16, 256, 100),
 ])
 def test_cross_attention_shapes(L, BH, heads, nq, nk):
