@@ -10,6 +10,8 @@
  * Number format.  Every weight GEMM / convolution on the path consumes fp32 values carried as two
  * bf16 planes (hi = bf16(x), lo = bf16(x - hi)) and issues three wgmma tensor-core MMAs per product
  * (DESIGN.md section 3).  "planes" below always means such a (hi, lo) pair of identical layout.
+ * Opt-in bf16 precision (s3r_gemm_desc.precision = 1, s3r_engine_create_ex): a GEMM multiplies the hi planes only,
+ * one MMA per product; producers still write both planes.
  *
  * Each entry point cites the reference code it replaces (paths relative to the reference root).
  */
@@ -150,6 +152,10 @@ typedef struct s3r_gemm_desc {
    * roles 3 / 4 (columns 3*q_c .. 5*q_c) are a second K / V^T pair written to k2_out / vt2_out -- the decoder's
    * self-attention qkv and cross-attention k, v projections (croco/models/blocks.py:186-189) as ONE launch */
   int swap_col0; float* k2_out; float* vt2_out;
+  /* 0: split bf16, three MMAs per product (hi*lo + lo*hi + hi*hi), fp32-grade.  1: bf16, one MMA (hi*hi) with fp32
+   * accumulation; a_lo and b_lo are not read and may be NULL, and a folded LayerNorm's ln_cs must then be the row sums of
+   * the hi plane alone (s3r_lin.cs_hi); S3R_EPI_HEADTAIL is split only.  Any other value is rejected. */
+  int precision;
 } s3r_gemm_desc;
 int s3r_gemm(const s3r_gemm_desc* d, void* stream);
 /* tile width the planner would pick (64/128), for tests */
@@ -319,8 +325,10 @@ int s3r_attn_train_backward(const s3r_attn_train_desc* d, const float* o, const 
 typedef struct s3r_planes { const void* hi; const void* lo; } s3r_planes;
 typedef struct s3r_ln { const float* w; const float* b; } s3r_ln;      /* grouped: [G, C] contiguous */
 /* b may be NULL.  cs != NULL marks a LayerNorm-folded linear: w = planes of W diag(gamma), b = b + W beta,
- * cs [G*N] = row sums of the planes (see s3r_gemm_desc.ln_cs); the preceding s3r_ln is then unused by the engine. */
-typedef struct s3r_lin { s3r_planes w; const float* b; const float* cs; } s3r_lin;
+ * cs [G*N] = row sums of the planes (see s3r_gemm_desc.ln_cs); the preceding s3r_ln is then unused by the engine.
+ * cs_hi [G*N] = row sums of the hi plane alone: what a bf16-precision GEMM's tensor core sees (required with cs by
+ * engines of precision 1). */
+typedef struct s3r_lin { s3r_planes w; const float* b; const float* cs; const float* cs_hi; } s3r_lin;
 
 typedef struct s3r_block_w {       /* croco/models/blocks.py:114-130 */
   s3r_ln norm1; s3r_lin qkv; s3r_lin proj; s3r_ln norm2; s3r_lin fc1; s3r_lin fc2;
@@ -379,6 +387,10 @@ typedef struct s3r_engine s3r_engine;
 /* One engine per (device, batch of sequences, image size).  Allocates its own activation workspace
  * (freed by destroy); `max_images` bounds the images one encode call may batch (>= 2*batch). */
 s3r_engine* s3r_engine_create(const s3r_model_w* w, int batch, int height, int width, int max_images);
+/* The same with a GEMM precision (s3r_gemm_desc.precision): 0 is s3r_engine_create.  1 runs every GEMM of encode, decode,
+ * keyheads and value on one bf16 product; heads, the memory read / append / similarity gate and the attention cores keep
+ * their arithmetic.  Other values: NULL, with the reason in s3r_last_error(). */
+s3r_engine* s3r_engine_create_ex(const s3r_model_w* w, int batch, int height, int width, int max_images, int precision);
 void s3r_engine_destroy(s3r_engine* e);
 /* dust3r/model.py:131-154 _encode_image: img [nimg,3,H,W] fp32 -> feat [nimg, N, 1024] fp32 */
 int s3r_engine_encode(s3r_engine* e, const float* img, int nimg, float* feat, void* stream);
@@ -430,7 +442,8 @@ double s3r_engine_take_flops(s3r_engine* e);
  * profile_read synchronises the device; out = {gemm_ms, gemm_flops, gemm_launches, attn_ms, attn_flops, attn_launches} */
 void s3r_engine_profile(s3r_engine* e, int on);
 /* per-launch list (in launch order) of the recorded tensor-core launches: duration [ms], algorithmic FLOPs, kind
- * (0 GEMM / conv, 1 attention); returns the count (call before profile_read, which consumes the records) */
+ * (0 split GEMM / conv, 1 attention, 2 one-product bf16 GEMM); returns the count (call before profile_read, which consumes
+ * the records).  profile_read counts kinds 0 and 2 as GEMMs. */
 int s3r_engine_profile_list(s3r_engine* e, double* ms, double* flops, int* kind, int cap);
 int s3r_engine_profile_read(s3r_engine* e, double* out);
 /* number of kernel launches since the last call; resets the counter */

@@ -14,6 +14,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("S3R_LIB", os.path.join(_HERE, "libspann3r_b200.so"))   # S3R_LIB: A/B an older build
 
 EPI_PLAIN, EPI_PIXSHUF, EPI_QKV, EPI_HEADTAIL = 0, 1, 2, 3
+PRECISION_SPLIT, PRECISION_BF16 = 0, 1     # s3r_gemm_desc.precision: three split-bf16 products, or one bf16 product
 ACT_NONE, ACT_GELU, ACT_RELU = 0, 1, 2
 
 _vp, _i, _i64, _f = C.c_void_p, C.c_int, C.c_int64, C.c_float
@@ -38,6 +39,7 @@ class GemmDesc(C.Structure):
         ("stats_out", _vp),
         ("trace", _vp),
         ("swap_col0", _i), ("k2_out", _vp), ("vt2_out", _vp),
+        ("precision", _i),
     ]
 
 

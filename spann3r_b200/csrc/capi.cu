@@ -91,6 +91,14 @@ static bool bad_ld(int64_t ld) { return ld < 0 || ld > INT32_MAX || ld % 4 != 0;
 
 // Every descriptor rule the epilogue relies on, checked before anything touches the driver.
 static int check_desc(const s3r_gemm_desc* d) {
+  if (d->precision != GEMM_SPLIT && d->precision != GEMM_BF16) {
+    set_error("s3r_gemm: precision=%d must be 0 (split bf16) or 1 (one bf16 product)", d->precision);
+    return -1;
+  }
+  if (d->precision == GEMM_BF16 && d->epi == S3R_EPI_HEADTAIL) {
+    set_error("s3r_gemm: precision=1 does not support EPI_HEADTAIL (the DPT head tail is split-only)");
+    return -1;
+  }
   if (d->n <= 0 || d->n % 32 != 0) {
     set_error("s3r_gemm: n=%d must be a positive multiple of 32 (the epilogue stores whole 32-column chunks)", d->n);
     return -1;
@@ -171,7 +179,7 @@ static int fill_plan(const s3r_gemm_desc* d, GemmPlan* plan) {
   if (r) return r;
   const int force_bn = d->epi == S3R_EPI_HEADTAIL ? (d->force_bn == 128 ? 128 : 1128) : d->force_bn;
   r = gemm_plan_init(plan, B(d->a_hi), B(d->a_lo), B(d->b_hi), B(d->b_lo), d->groups, d->nb, d->h, d->w, d->kc,
-                     d->taps, d->n, force_bn);
+                     d->taps, d->n, force_bn, 0, 0, 0, d->precision);
   if (r) return r;
   GemmArgs& a = plan->args;
   a.epi = d->epi; a.act = d->act; a.plane_relu = d->plane_relu;

@@ -53,15 +53,18 @@ struct Epi {
   const float *ht_w = nullptr, *ht_b = nullptr; float *ht_pts = nullptr, *ht_conf = nullptr;
   // folded LayerNorm: consumer side (statistics of the A rows + column sums of the gamma-folded weights) ...
   const float2* ln_stats = nullptr; int ln_np = 0; float ln_eps = 0.f; const float* ln_cs = nullptr; int a_swap = 0;
+  const float* ln_cs_hi = nullptr;   // column sums of the hi plane alone: the ones a GEMM_BF16 launch subtracts
   float2* stats_out = nullptr;   // ... and producer side (chunk sums of the rows this GEMM writes)
 };
 
-// Plans are created on the first pass through a stage and replayed afterwards (same call order).
+// Plans are created on the first pass through a stage and replayed afterwards (same call order).  `precision` is the
+// GemmPrecision of every GEMM of the stage: the engine's for encode / decode / keyheads / value, split for the rest.
 struct PlanCache {
   std::vector<GemmPlan> gemms;
   std::vector<AttnPlan> attns;
   size_t gc = 0, ac = 0;
   bool building = true;
+  int precision = GEMM_SPLIT;
   void begin() {
     gc = ac = 0;
     if (building) {   // a previous first pass failed half way (e.g. a plan_init error): start the plan list over
@@ -82,9 +85,10 @@ struct s3r_engine {
   double flops = 0;
   long long launches = 0;
   int status = 0;
+  int precision = GEMM_SPLIT;   // of the encode / decode / keyheads / value GEMMs (s3r_engine_create_ex)
   // optional per-launch timing of the tensor-core kernels (bench.py roofline leg)
   bool profiling = false;
-  struct Timed { cudaEvent_t a, b; double flops; int kind; };   // kind 0 = GEMM/conv, 1 = attention
+  struct Timed { cudaEvent_t a, b; double flops; int kind; };   // kind 0 = split GEMM/conv, 1 = attention, 2 = bf16 GEMM
   std::vector<Timed> timed;
   std::vector<cudaEvent_t> ev_pool;
   cudaEvent_t get_event() {
@@ -154,7 +158,7 @@ struct s3r_engine {
     if (pc.building) {
       pc.gemms.emplace_back();
       int r = gemm_plan_init(&pc.gemms.back(), A.hi, A.lo, Bw.hi, Bw.lo, g.groups, g.NB, g.H, g.W, g.Kc, g.taps, g.N,
-                             e.epi == EPI_HEADTAIL ? 1128 : g.force_bn, g.lda, g.ldb, g.b_group_rows);
+                             e.epi == EPI_HEADTAIL ? 1128 : g.force_bn, g.lda, g.ldb, g.b_group_rows, pc.precision);
       if (r) return r;
       pc.gemms.back().b_static = (g.b_static && options().prefetch_b) ? 1 : 0;   // decided when the plan is built
     }
@@ -178,14 +182,20 @@ struct s3r_engine {
     } else if (e.epi == EPI_HEADTAIL) {
       a.ht_w = e.ht_w; a.ht_b = e.ht_b; a.ht_pts = e.ht_pts; a.ht_conf = e.ht_conf;
     }
-    a.ln_stats = e.ln_stats; a.ln_np = e.ln_np; a.ln_eps = e.ln_eps; a.ln_cs = e.ln_cs; a.a_swap = e.a_swap;
+    // a folded LayerNorm subtracts mean * (column sums of exactly the planes the tensor core multiplies)
+    const float* cs = p.precision == GEMM_BF16 ? e.ln_cs_hi : e.ln_cs;
+    if (e.ln_stats && !cs) {
+      set_error("engine: a LayerNorm-folded linear lacks its %s column sums", p.precision == GEMM_BF16 ? "cs_hi" : "cs");
+      return -1;
+    }
+    a.ln_stats = e.ln_stats; a.ln_np = e.ln_np; a.ln_eps = e.ln_eps; a.ln_cs = cs; a.a_swap = e.a_swap;
     a.swap_col0 = e.swap_col0;
     a.stats_out = e.stats_out;
     a.b_static = p.b_static;
     flops += p.flops;
     ++launches;
     if (!profiling) return gemm_launch(p, st);
-    Timed t; t.a = get_event(); t.b = get_event(); t.flops = p.flops; t.kind = 0;
+    Timed t; t.a = get_event(); t.b = get_event(); t.flops = p.flops; t.kind = p.precision == GEMM_BF16 ? 2 : 0;
     cudaEventRecord(t.a, st);
     int r = gemm_launch(p, st);
     cudaEventRecord(t.b, st);
@@ -243,7 +253,7 @@ struct s3r_engine {
     Epi e; e.epi = EPI_QKV; e.bias = bw.qkv.b; e.q_C = c.Da; e.q_role_base = 0; e.q_ntok = N; e.q_ntok_pad = Npad;
     e.q_rope = rope ? 1 : 0; e.q_nb = nimg; e.q_pos = pos_tab; e.q_cs = (const float2*)(c.cs ? c.cs : w.rope_cs);
     e.q_out = Qb; e.k_out = Kb; e.vt_out = Vtb; e.q_scale = c.q_scale;
-    e.ln_stats = St1; e.ln_np = c.D / 32; e.ln_eps = 1e-6f; e.ln_cs = bw.qkv.cs;                       // norm1
+    e.ln_stats = St1; e.ln_np = c.D / 32; e.ln_eps = 1e-6f; e.ln_cs = bw.qkv.cs; e.ln_cs_hi = bw.qkv.cs_hi;   // norm1
     return gemm(pc, P, WP(bw.qkv.w), g, e, st);
   }
   int vit_blocks(PlanCache& pc, const s3r_block_w* blocks, int depth, const VitCfg& c, int nimg, bool rope, float* Xp,
@@ -264,7 +274,7 @@ struct s3r_engine {
       {
         Geom g; g.W = rows; g.Kc = D; g.N = 4 * D;
         Epi e; e.bias = bw.fc1.b; e.act = ACT_GELU; e.op = Hb; e.ldp = 4 * D;
-        e.ln_stats = St2; e.ln_np = D / 32; e.ln_eps = 1e-6f; e.ln_cs = bw.fc1.cs;                       // norm2
+        e.ln_stats = St2; e.ln_np = D / 32; e.ln_eps = 1e-6f; e.ln_cs = bw.fc1.cs; e.ln_cs_hi = bw.fc1.cs_hi;   // norm2
         if ((r = gemm(pc, P2, WP(bw.fc1.w), g, e, st))) return r;
       }
       {
@@ -313,6 +323,14 @@ static __global__ void bank_bump_kernel(float* count, float* attn, long long ld,
 extern "C" {
 
 s3r_engine* s3r_engine_create(const s3r_model_w* w, int batch, int height, int width, int max_images) {
+  return s3r_engine_create_ex(w, batch, height, width, max_images, GEMM_SPLIT);
+}
+
+s3r_engine* s3r_engine_create_ex(const s3r_model_w* w, int batch, int height, int width, int max_images, int precision) {
+  if (precision != GEMM_SPLIT && precision != GEMM_BF16) {
+    set_error("s3r_engine_create_ex: precision must be 0 (split bf16) or 1 (one bf16 product), got %d", precision);
+    return nullptr;
+  }
   if (!w || batch <= 0 || height % 16 != 0 || width % 16 != 0 || height <= 0 || width <= 0) {
     set_error("s3r_engine_create: need batch > 0 and height, width multiples of 16 (got %d, %dx%d)", batch, height, width);
     return nullptr;
@@ -334,6 +352,8 @@ s3r_engine* s3r_engine_create(const s3r_model_w* w, int batch, int height, int w
   e->N = e->gh * e->gw;
   e->Npad = (e->N + 3) / 4 * 4;
   e->max_images = max_images;
+  e->precision = precision;
+  e->pc_decode.precision = e->pc_keys.precision = e->pc_value.precision = precision;   // pc_heads, pc_memread: split
   if (e->gh > w->rope_maxpos || e->gw > w->rope_maxpos) {
     set_error("s3r_engine_create: patch grid %dx%d exceeds the RoPE table (%d positions)", e->gh, e->gw, w->rope_maxpos);
     delete e;
@@ -484,7 +504,7 @@ int s3r_engine_profile_read(s3r_engine* e, double* out) {
   for (auto& t : e->timed) {
     float ms = 0.f;
     cudaEventElapsedTime(&ms, t.a, t.b);
-    const int o = t.kind == 0 ? 0 : 3;
+    const int o = t.kind == 1 ? 3 : 0;
     out[o] += ms;
     out[o + 1] += t.flops;
     out[o + 2] += 1;
@@ -512,6 +532,7 @@ int s3r_engine_encode(s3r_engine* e, const float* img, int nimg, float* feat, vo
     return -1;
   }
   PlanCache& pc = e->pc_encode[nimg];
+  pc.precision = e->precision;
   pc.begin();
   const int rows = nimg * e->N;
   int r;
@@ -568,7 +589,8 @@ int s3r_engine_decode(s3r_engine* e, const float* f1, const float* f2, float* de
     Epi ep; ep.epi = EPI_QKV; ep.bias = bw.qkv.b; ep.q_C = 768; ep.q_role_base = 0; ep.q_ntok = N; ep.q_ntok_pad = e->Npad;
     ep.q_rope = 1; ep.q_nb = B; ep.q_pos = e->pos; ep.q_cs = cs;
     ep.q_out = e->Qd; ep.k_out = e->Kd; ep.vt_out = e->Vtd; ep.k2_out = e->Kd2; ep.vt2_out = e->Vtd2; ep.q_scale = 0.125f;
-    ep.ln_stats = e->Sa; ep.ln_np = 24; ep.ln_eps = 1e-6f; ep.ln_cs = bw.qkv.cs; ep.a_swap = 1; ep.swap_col0 = 2304;
+    ep.ln_stats = e->Sa; ep.ln_np = 24; ep.ln_eps = 1e-6f; ep.ln_cs = bw.qkv.cs; ep.ln_cs_hi = bw.qkv.cs_hi;
+    ep.a_swap = 1; ep.swap_col0 = 2304;
     return e->gemm(pc, xin, WP(bw.qkv.w), g, ep, st);
   };
   Planes xin = e->Pa;
@@ -588,7 +610,7 @@ int s3r_engine_decode(s3r_engine* e, const float* f1, const float* f2, float* de
       Epi ep; ep.epi = EPI_QKV; ep.bias = bw.q.b; ep.q_C = 768; ep.q_role_base = 0; ep.q_ntok = N; ep.q_ntok_pad = e->Npad;
       ep.q_rope = 1; ep.q_nb = B; ep.q_pos = e->pos; ep.q_cs = cs;
       ep.q_out = e->Qd; ep.k_out = e->Kd; ep.vt_out = e->Vtd; ep.q_scale = 0.125f;
-      ep.ln_stats = e->Sb; ep.ln_np = 24; ep.ln_eps = 1e-6f; ep.ln_cs = bw.q.cs;                        // norm2
+      ep.ln_stats = e->Sb; ep.ln_np = 24; ep.ln_eps = 1e-6f; ep.ln_cs = bw.q.cs; ep.ln_cs_hi = bw.q.cs_hi;     // norm2
       if ((r = e->gemm(pc, e->Pb, WP(bw.q.w), g, ep, st))) return r;
     }
     if ((r = e->attention(pc, e->Qd, e->Kd2, e->Vtd2, 2 * B * 12, 12, N, N, e->AOd, 768, st))) return r;
@@ -602,7 +624,7 @@ int s3r_engine_decode(s3r_engine* e, const float* f1, const float* f2, float* de
     {
       Geom g; g.groups = 2; g.W = (int)R; g.Kc = 768; g.N = 3072;
       Epi ep; ep.bias = bw.fc1.b; ep.act = ACT_GELU; ep.op = e->Hd; ep.ldp = 3072;
-      ep.ln_stats = e->Sc; ep.ln_np = 24; ep.ln_eps = 1e-6f; ep.ln_cs = bw.fc1.cs;                      // norm3
+      ep.ln_stats = e->Sc; ep.ln_np = 24; ep.ln_eps = 1e-6f; ep.ln_cs = bw.fc1.cs; ep.ln_cs_hi = bw.fc1.cs_hi; // norm3
       if ((r = e->gemm(pc, e->Pc, WP(bw.fc1.w), g, ep, st))) return r;
     }
     {

@@ -44,17 +44,24 @@ static constexpr int kSmemMax = 227 * 1024;
 static constexpr int kAccLD = 36;       // accumulator staging row stride (floats): 16-byte rows, conflict-free row reads
 static constexpr int kAccBytes = 2 * BM * kAccLD * 4;   // two 32-column chunks (one per column half) of all 128 rows
 
-template <int BN>
+// NP = tensor-core products per k16 step: 3 (split bf16: hi*lo, lo*hi, hi*hi) or 1 (hi*hi only, the bf16 precision).
+// A stage holds the planes the products read: A_hi [A_lo] B_hi [B_lo].
+template <int BN, int NP>
 struct GemmCfg {
+  static constexpr int PLANES = NP == 3 ? 2 : 1;
   static constexpr int A_TILE = BM * BK * 2;  // bytes, one plane
   static constexpr int B_TILE = BN * BK * 2;
-  static constexpr int STAGE = 2 * A_TILE + 2 * B_TILE;
+  static constexpr int B_OFF = PLANES * A_TILE;   // first B plane in a stage
+  static constexpr int STAGE = PLANES * (A_TILE + B_TILE);
   static constexpr int COLV = 2 * 2 * BN * 4;  // per tile parity: staged bias + LN-fold column sums of the tile
   static constexpr int HT = 4 * 2 * 32 * 16;   // EPI_HEADTAIL hand-over slots (per lane quadrant, two tile parities)
   static constexpr int FIXED = 1024 /*align slack*/ + 256 /*barriers*/ + kAccBytes + COLV + HT;
   static constexpr int STAGES = (kSmemMax - FIXED) / STAGE;
   static constexpr int SMEM = STAGES * STAGE + FIXED;
-  static_assert(STAGES == (BN == 128 ? 5 : 7), "ring depth (DESIGN.md §4)");
+  static_assert(NP == 3 || NP == 1, "split (3 products) or bf16 (1 product)");
+  // split: 32 KB / 24 KB stages; one product: 16 KB / 12 KB stages, the same 32-channel k-blocks (DESIGN.md §4)
+  static_assert(STAGES == (NP == 3 ? (BN == 128 ? 5 : 7) : (BN == 128 ? 11 : 15)), "ring depth (DESIGN.md §4)");
+  static_assert(2 * STAGES * 8 <= 256, "full + empty barriers fit their 256-byte slot");
   static_assert(Stg<32>::WARP_BYTES == 32 * kAccLD * 4, "a warp's staging tile is its own rows of the accumulator chunk");
 };
 
@@ -64,9 +71,9 @@ __device__ __forceinline__ void wgmma_bf16(float (&d)[BN / 2], uint64_t da, uint
   else wgmma_bf16_n128(d, da, db, scale_d);
 }
 
-template <int BN, int EPI>
+template <int BN, int EPI, int NP>
 __global__ void __launch_bounds__(kNumThreads, 1) gemm_bf16x3_kernel(const __grid_constant__ GemmArgs args) {
-  using Cfg = GemmCfg<BN>;
+  using Cfg = GemmCfg<BN, NP>;
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment by pointer arithmetic on the __shared__ array (an integer round trip would lose the address
   // space and turn every access through `smem` into a generic LD / ST)
@@ -91,9 +98,11 @@ __global__ void __launch_bounds__(kNumThreads, 1) gemm_bf16x3_kernel(const __gri
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&args.tmA_hi);
-    tma_prefetch_desc(&args.tmA_lo);
     tma_prefetch_desc(&args.tmB_hi);
-    tma_prefetch_desc(&args.tmB_lo);
+    if constexpr (NP == 3) {
+      tma_prefetch_desc(&args.tmA_lo);
+      tma_prefetch_desc(&args.tmB_lo);
+    }
     for (int i = 0; i < Cfg::STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], kEpiWarps);
@@ -118,8 +127,8 @@ __global__ void __launch_bounds__(kNumThreads, 1) gemm_bf16x3_kernel(const __gri
         const int tap = kb / args.kpt, kc = (kb - tap * args.kpt) * BK;
         uint8_t* s = smem + kb * Cfg::STAGE;
         mbar_arrive_expect_tx(&full_bar[kb], Cfg::STAGE);
-        tma_load_3d(s + 2 * Cfg::A_TILE, &args.tmB_hi, &full_bar[kb], kc, tap, brow);
-        tma_load_3d(s + 2 * Cfg::A_TILE + Cfg::B_TILE, &args.tmB_lo, &full_bar[kb], kc, tap, brow);
+        tma_load_3d(s + Cfg::B_OFF, &args.tmB_hi, &full_bar[kb], kc, tap, brow);
+        if constexpr (NP == 3) tma_load_3d(s + Cfg::B_OFF + Cfg::B_TILE, &args.tmB_lo, &full_bar[kb], kc, tap, brow);
       }
     }
     __syncwarp();
@@ -156,10 +165,10 @@ __global__ void __launch_bounds__(kNumThreads, 1) gemm_bf16x3_kernel(const __gri
             const uint32_t fb = full_u + stage * 8;
             if (!b_done) mbar_arrive_expect_tx_u(fb, Cfg::STAGE);
             tma_load_4d_u(s, &args.tmA_hi, fb, kc, w0 + dx, h0 + dy, img);
-            tma_load_4d_u(s + Cfg::A_TILE, &args.tmA_lo, fb, kc, w0 + dx, h0 + dy, img);
+            if constexpr (NP == 3) tma_load_4d_u(s + Cfg::A_TILE, &args.tmA_lo, fb, kc, w0 + dx, h0 + dy, img);
             if (!b_done) {
-              tma_load_3d_u(s + 2 * Cfg::A_TILE, &args.tmB_hi, fb, kc, tap, brow);
-              tma_load_3d_u(s + 2 * Cfg::A_TILE + Cfg::B_TILE, &args.tmB_lo, fb, kc, tap, brow);
+              tma_load_3d_u(s + Cfg::B_OFF, &args.tmB_hi, fb, kc, tap, brow);
+              if constexpr (NP == 3) tma_load_3d_u(s + Cfg::B_OFF + Cfg::B_TILE, &args.tmB_lo, fb, kc, tap, brow);
             }
           }
           __syncwarp();
@@ -226,16 +235,24 @@ __global__ void __launch_bounds__(kNumThreads, 1) gemm_bf16x3_kernel(const __gri
         if (trace && kb == 0 && it == 0 && threadIdx.x == 128) trace[3] = globaltimer_ns();
         const uint32_t sa = smem_u + stage * Cfg::STAGE;
         const uint64_t da_hi = wgmma_desc_sw64_kmajor(sa + wg * (64 * BK * 2));
-        const uint64_t da_lo = wgmma_desc_sw64_kmajor(sa + Cfg::A_TILE + wg * (64 * BK * 2));
-        const uint64_t db_hi = wgmma_desc_sw64_kmajor(sa + 2 * Cfg::A_TILE);
-        const uint64_t db_lo = wgmma_desc_sw64_kmajor(sa + 2 * Cfg::A_TILE + Cfg::B_TILE);
+        const uint64_t db_hi = wgmma_desc_sw64_kmajor(sa + Cfg::B_OFF);
         wgmma_fence();
+        if constexpr (NP == 3) {
+          const uint64_t da_lo = wgmma_desc_sw64_kmajor(sa + Cfg::A_TILE + wg * (64 * BK * 2));
+          const uint64_t db_lo = wgmma_desc_sw64_kmajor(sa + Cfg::B_OFF + Cfg::B_TILE);
 #pragma unroll
-        for (int kk = 0; kk < BK / 16; ++kk) {
-          const uint64_t ko = (uint64_t)(kk * 32 >> 4);  // 16 bf16 = 32 bytes along K inside the swizzle span
-          wgmma_bf16<BN>(acc, da_hi + ko, db_lo + ko, 1);
-          wgmma_bf16<BN>(acc, da_lo + ko, db_hi + ko, 1);
-          wgmma_bf16<BN>(acc, da_hi + ko, db_hi + ko, 1);
+          for (int kk = 0; kk < BK / 16; ++kk) {
+            const uint64_t ko = (uint64_t)(kk * 32 >> 4);  // 16 bf16 = 32 bytes along K inside the swizzle span
+            wgmma_bf16<BN>(acc, da_hi + ko, db_lo + ko, 1);
+            wgmma_bf16<BN>(acc, da_lo + ko, db_hi + ko, 1);
+            wgmma_bf16<BN>(acc, da_hi + ko, db_hi + ko, 1);
+          }
+        } else {
+#pragma unroll
+          for (int kk = 0; kk < BK / 16; ++kk) {
+            const uint64_t ko = (uint64_t)(kk * 32 >> 4);
+            wgmma_bf16<BN>(acc, da_hi + ko, db_hi + ko, 1);
+          }
         }
         wgmma_commit();
         wgmma_wait<1>();   // the previous k-block's MMAs have retired: its stage goes back to the producer
@@ -396,8 +413,13 @@ int num_sms() {
 
 int gemm_plan_init(GemmPlan* plan, const __nv_bfloat16* a_hi, const __nv_bfloat16* a_lo,
                    const __nv_bfloat16* b_hi, const __nv_bfloat16* b_lo, int groups, int NB, int H, int W, int Kc,
-                   int taps, int N, int force_bn, long long lda, long long ldb, long long b_group_rows) {
+                   int taps, int N, int force_bn, long long lda, long long ldb, long long b_group_rows, int precision) {
   memset(plan, 0, sizeof(*plan));
+  if (precision != GEMM_SPLIT && precision != GEMM_BF16) {
+    set_error("gemm_plan_init: precision %d (0 = split bf16, 1 = one bf16 product)", precision);
+    return -1;
+  }
+  plan->precision = precision;
   GemmArgs& a = plan->args;
   if (lda == 0) lda = Kc;
   if (ldb == 0) ldb = (long long)Kc * taps;
@@ -444,7 +466,9 @@ int gemm_plan_init(GemmPlan* plan, const __nv_bfloat16* a_hi, const __nv_bfloat1
     uint32_t box[4] = {(uint32_t)BK, (uint32_t)a.bw, (uint32_t)a.bh, 1};
     int r;
     if ((r = encode_tmap(&a.tmA_hi, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, a_hi, dims, str, box, kSwizzle))) return r;
-    if ((r = encode_tmap(&a.tmA_lo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, a_lo, dims, str, box, kSwizzle))) return r;
+    if (precision == GEMM_SPLIT &&
+        (r = encode_tmap(&a.tmA_lo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, a_lo, dims, str, box, kSwizzle)))
+      return r;
   }
   {
     uint64_t dims[3] = {(uint64_t)Kc, (uint64_t)taps, (uint64_t)(b_group_rows * (groups - 1) + N)};
@@ -453,7 +477,9 @@ int gemm_plan_init(GemmPlan* plan, const __nv_bfloat16* a_hi, const __nv_bfloat1
     uint32_t box[3] = {(uint32_t)BK, 1, (uint32_t)bn};
     int r;
     if ((r = encode_tmap(&a.tmB_hi, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, b_hi, dims, str, box, kSwizzle))) return r;
-    if ((r = encode_tmap(&a.tmB_lo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, b_lo, dims, str, box, kSwizzle))) return r;
+    if (precision == GEMM_SPLIT &&
+        (r = encode_tmap(&a.tmB_lo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, b_lo, dims, str, box, kSwizzle)))
+      return r;
   }
   const long long n_tiles = (N + bn - 1) / bn;
   const long long total = m_tiles * n_tiles;
@@ -463,21 +489,21 @@ int gemm_plan_init(GemmPlan* plan, const __nv_bfloat16* a_hi, const __nv_bfloat1
   return 0;
 }
 
-template <int BN, int EPI>
+template <int BN, int EPI, int NP>
 static int launch_bn(const GemmPlan& plan, cudaStream_t stream) {
-  using Cfg = GemmCfg<BN>;
+  using Cfg = GemmCfg<BN, NP>;
   static PerDeviceOnce once;
   bool& attr_set = once.cur();
   if (!attr_set) {
     cudaError_t e =
-        cudaFuncSetAttribute(gemm_bf16x3_kernel<BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
+        cudaFuncSetAttribute(gemm_bf16x3_kernel<BN, EPI, NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
     if (e != cudaSuccess) {
       set_error("cudaFuncSetAttribute(smem=%d): %s", Cfg::SMEM, cudaGetErrorString(e));
       return -5;
     }
     attr_set = true;
   }
-  cudaError_t e = launch_pdl(gemm_bf16x3_kernel<BN, EPI>, plan.grid, dim3(kNumThreads), Cfg::SMEM, stream, plan.args);
+  cudaError_t e = launch_pdl(gemm_bf16x3_kernel<BN, EPI, NP>, plan.grid, dim3(kNumThreads), Cfg::SMEM, stream, plan.args);
   if (e != cudaSuccess) {
     set_error("gemm launch failed: %s", cudaGetErrorString(e));
     return -6;
@@ -485,24 +511,37 @@ static int launch_bn(const GemmPlan& plan, cudaStream_t stream) {
   return 0;
 }
 
-template <int BN>
+template <int BN, int NP>
 static int launch_epi(const GemmPlan& plan, cudaStream_t stream) {
   switch (plan.args.epi) {
-    case EPI_PLAIN: return launch_bn<BN, EPI_PLAIN>(plan, stream);
-    case EPI_PIXSHUF: return launch_bn<BN, EPI_PIXSHUF>(plan, stream);
-    case EPI_QKV: return launch_bn<BN, EPI_QKV>(plan, stream);
-    case EPI_HEADTAIL: return launch_bn<BN, EPI_HEADTAIL>(plan, stream);
+    case EPI_PLAIN: return launch_bn<BN, EPI_PLAIN, NP>(plan, stream);
+    case EPI_PIXSHUF: return launch_bn<BN, EPI_PIXSHUF, NP>(plan, stream);
+    case EPI_QKV: return launch_bn<BN, EPI_QKV, NP>(plan, stream);
+    case EPI_HEADTAIL:
+      // the DPT head tail runs in heads(), which is always split; not instantiated at one product (it would spill)
+      if constexpr (NP == 3) return launch_bn<BN, EPI_HEADTAIL, NP>(plan, stream);
+      break;
   }
   set_error("gemm_launch: bad epilogue mode %d", plan.args.epi);
   return -1;
 }
 
-int gemm_launch(const GemmPlan& plan, cudaStream_t stream) {
+template <int NP>
+static int launch_np(const GemmPlan& plan, cudaStream_t stream) {
   switch (plan.bn) {
-    case 64: return launch_epi<64>(plan, stream);
-    case 128: return launch_epi<128>(plan, stream);
+    case 64: return launch_epi<64, NP>(plan, stream);
+    case 128: return launch_epi<128, NP>(plan, stream);
   }
   set_error("gemm_launch: bad bn %d", plan.bn);
+  return -1;
+}
+
+int gemm_launch(const GemmPlan& plan, cudaStream_t stream) {
+  switch (plan.precision) {
+    case GEMM_SPLIT: return launch_np<3>(plan, stream);
+    case GEMM_BF16: return launch_np<1>(plan, stream);
+  }
+  set_error("gemm_launch: bad precision %d", plan.precision);
   return -1;
 }
 

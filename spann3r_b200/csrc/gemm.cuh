@@ -1,4 +1,4 @@
-// Host-visible description of one launch of the split-bf16 wgmma GEMM / implicit-GEMM conv engine.
+// Host-visible description of one launch of the bf16 wgmma GEMM / implicit-GEMM conv engine (split or one-product).
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -14,6 +14,9 @@ enum EpiMode : int {
   EPI_HEADTAIL = 3,   // DPT head tail: ReLU -> 1x1 conv (128->4) -> postprocess (pts3d, conf)
 };
 enum Act : int { ACT_NONE = 0, ACT_GELU = 1, ACT_RELU = 2 };
+// Tensor-core products per k16 step.  GEMM_SPLIT: hi*lo + lo*hi + hi*hi of the split planes (fp32-grade).  GEMM_BF16: hi*hi
+// only -- the lo planes are neither loaded nor needed (their tensor maps stay unencoded).
+enum GemmPrecision : int { GEMM_SPLIT = 0, GEMM_BF16 = 1 };
 
 // A operand: activations as two bf16 planes laid out [G*NB, H, W, C] (C contiguous).  A plain
 // linear layer is the degenerate image H=1, W=rows.  B operand: weights as two bf16 planes laid
@@ -73,11 +76,13 @@ struct GemmPlan {
   GemmArgs args;
   dim3 grid;
   int bn;          // 64 / 128
+  int precision;   // GemmPrecision
   int b_static;    // engine: B is a packed weight and the prefetch option was on when the plan was built
   double flops;    // algorithmic 2*M*N*K (all groups), for roofline accounting
 };
 
-// Encodes the four tensor maps and picks the tile shape.  Returns 0 or a negative error.
+// Encodes the tensor maps (four; two -- the hi planes -- at GEMM_BF16, where a_lo / b_lo may be null) and picks the tile
+// shape.  Returns 0 or a negative error.
 // lda / ldb: row strides (elements) of A pixels / B rows (0 = dense: Kc resp. taps*Kc);
 // b_group_rows: rows between consecutive groups of B (0 = N).
 // force_bn: 0 = planner's choice; 64 / 128 = that tile width; 256, 1128, 2064, 2128, 2256 = the nearest width the kernel has
@@ -86,7 +91,7 @@ int gemm_plan_init(GemmPlan* plan,
                    const __nv_bfloat16* a_hi, const __nv_bfloat16* a_lo,   // [G*NB, H, W, Kc]
                    const __nv_bfloat16* b_hi, const __nv_bfloat16* b_lo,   // [G*N, taps, Kc]
                    int groups, int NB, int H, int W, int Kc, int taps, int N, int force_bn = 0,
-                   long long lda = 0, long long ldb = 0, long long b_group_rows = 0);
+                   long long lda = 0, long long ldb = 0, long long b_group_rows = 0, int precision = GEMM_SPLIT);
 int gemm_launch(const GemmPlan& plan, cudaStream_t stream);
 
 // Tuning knobs of the tile planner / producers (s3r_set_option): read when a plan is BUILT, so two engines of one

@@ -28,7 +28,7 @@ class LN(C.Structure):
 
 
 class Lin(C.Structure):
-    _fields_ = [("w", Planes), ("b", _vp), ("cs", _vp)]
+    _fields_ = [("w", Planes), ("b", _vp), ("cs", _vp), ("cs_hi", _vp)]
 
 
 class BlockW(C.Structure):
@@ -70,6 +70,7 @@ class Bank(C.Structure):
 
 _lib.register_protos({
     "s3r_engine_create": (_vp, [C.POINTER(ModelW), _i, _i, _i, _i]),
+    "s3r_engine_create_ex": (_vp, [C.POINTER(ModelW), _i, _i, _i, _i, _i]),
     "s3r_engine_destroy": (None, [_vp]),
     "s3r_engine_encode": (_i, [_vp, _vp, _i, _vp, _vp]),
     "s3r_engine_decode": (_i, [_vp, _vp, _vp, _vp, _vp]),
@@ -152,6 +153,12 @@ def split_bf16_host_rowsum(w: torch.Tensor) -> torch.Tensor:
     hi = w.to(torch.bfloat16)
     lo = (w - hi.float()).to(torch.bfloat16)
     return (hi.double() + lo.double()).sum(dim=1).float()
+
+
+def bf16_hi_rowsum(w: torch.Tensor) -> torch.Tensor:
+    """Row sums of the hi plane bf16(w) alone, in fp64: the `cs_hi` of a LayerNorm-folded Linear, which a bf16-precision
+    GEMM (one product, hi x hi) subtracts instead of `cs`."""
+    return w.to(torch.bfloat16).double().sum(dim=1).float()
 
 
 class PackedWeights:
@@ -244,7 +251,8 @@ class PackedWeights:
     def _linear_ln(self, names, ln_names, slots=None) -> Lin:
         """Linear that follows a LayerNorm, with the LayerNorm folded in (include/spann3r_b200.h, s3r_lin.cs):
         LN(x) W^T + b = rstd (x W'^T - mean cs) + b'  with  W' = W diag(gamma), b' = b + W beta, cs = rowsum(W').
-        Exact algebra; cs is summed over the split-bf16 planes the tensor core will actually multiply."""
+        Exact algebra; cs is summed over the split-bf16 planes the tensor core will actually multiply, cs_hi over the hi
+        plane alone (bf16 precision)."""
         ws, bs = [], []
         for k, ln in zip(names, ln_names):
             wf, bf = fold_layernorm(self._t(k + ".weight"), self._t(k + ".bias"), self._t(ln + ".weight"), self._t(ln + ".bias"))
@@ -254,6 +262,7 @@ class PackedWeights:
             bs.append(bf)
         l = self._lin(ws, bs)
         l.cs = self._f32(torch.cat([split_bf16_host_rowsum(w.reshape(w.shape[0], -1)) for w in ws], dim=0))
+        l.cs_hi = self._f32(torch.cat([bf16_hi_rowsum(w.reshape(w.shape[0], -1)) for w in ws], dim=0))
         return l
 
     def _conv3(self, names, bias=True) -> Lin:   # [Cout, Cin, 3, 3] -> [Cout, tap, Cin]
@@ -382,16 +391,26 @@ class MemoryBank:
         self.len = k
 
 
+PRECISIONS = {"fp32": 0, "bf16": 1}   # Spann3R(precision=...) -> s3r_engine_create_ex's GEMM precision
+
+
 class Engine:
-    def __init__(self, weights: PackedWeights, batch: int, height: int, width: int, max_images: int = 0):
+    def __init__(self, weights: PackedWeights, batch: int, height: int, width: int, max_images: int = 0,
+                 precision: str = "fp32"):
+        """precision "bf16": the GEMMs of encode / decode / keyheads / value multiply the hi planes only (one tensor-core
+        product); everything else runs as in "fp32" (include/spann3r_b200.h, s3r_engine_create_ex)."""
+        if precision not in PRECISIONS:
+            raise ValueError(f"precision must be one of {sorted(PRECISIONS)}, got {precision!r}")
         self.weights = weights   # keeps the packed tensors alive
+        self.precision = precision
         self.B, self.H, self.W = batch, height, width
         self.N = (height // 16) * (width // 16)
         self.max_images = max(max_images, 2 * batch)
         self.device = weights.device
         L = _lib.lib()
         with torch.cuda.device(self.device):     # the engine allocates its workspace on the CURRENT device
-            self._h = L.s3r_engine_create(C.byref(weights.struct), batch, height, width, self.max_images)
+            self._h = L.s3r_engine_create_ex(C.byref(weights.struct), batch, height, width, self.max_images,
+                                             PRECISIONS[precision])
         if not self._h:
             raise _lib.S3RError("s3r_engine_create failed: " + L.s3r_last_error().decode())
 
@@ -501,7 +520,8 @@ class Engine:
                     attn_launches=int(out[5]))
 
     def profile_list(self, cap: int = 4096):
-        """[(ms, flops, kind)] of the launches recorded since profile(True), in launch order (kind 0 GEMM, 1 attention)."""
+        """[(ms, flops, kind)] of the launches recorded since profile(True), in launch order (kind 0 split GEMM,
+        1 attention, 2 one-product bf16 GEMM)."""
         ms, fl, kd = (C.c_double * cap)(), (C.c_double * cap)(), (C.c_int * cap)()
         with self._on():
             n = _lib.lib().s3r_engine_profile_list(self._h, ms, fl, kd, cap)

@@ -14,6 +14,12 @@ reference's landscape wrapper (`_to_landscape`).  Every constructor option is su
 value encoder; `use_feat=True` builds the reference's 768-wide value encoder (16 heads of 48, no `pos_patch_embed`), fed
 with head 1's last decoder tokens instead of the pointmap.  The library runs its 48-wide heads zero-padded to 64-wide slots
 (include/spann3r_b200.h, s3r_model_w.value_dim), an exact repacking of the same arithmetic.
+
+Precision: `Spann3R(precision="fp32")` (default) holds the forward within 1e-3 of the fp32 reference: every GEMM multiplies
+split-bf16 operands with three tensor-core products.  `precision="bf16"` (or `set_precision("bf16")`) is an opt-in for speed
+over parity, inference only: the GEMMs of the encoder, decoder, key heads and value encoder multiply bf16 operands once,
+with fp32 accumulation; the DPT heads, the spatial memory and the attention cores are unchanged (the reference's own
+`use_amp` inference likewise keeps its heads in fp32).
 """
 from __future__ import annotations
 
@@ -25,7 +31,7 @@ import torch.nn as nn
 
 from . import synth
 from ._lib import conf_score as _conf_score
-from .engine import Engine, MemoryBank, PackedWeights
+from .engine import PRECISIONS, Engine, MemoryBank, PackedWeights
 
 
 # ------------------------------------------------------------------------------------------------
@@ -263,8 +269,9 @@ class SpatialMemory:
 # ------------------------------------------------------------------------------------------------
 class Spann3R(ParamModule):
     def __init__(self, dus3r_name="./checkpoints/DUSt3R_ViTLarge_BaseDecoder_512_dpt.pth", use_feat=False,
-                 mem_pos_enc=False, memory_dropout=0.15, max_encode_batch: int = 16):
+                 mem_pos_enc=False, memory_dropout=0.15, max_encode_batch: int = 16, precision: str = "fp32"):
         super().__init__()
+        self.set_precision(precision)
         self.use_feat, self.mem_pos_enc = bool(use_feat), mem_pos_enc
         # use_feat (spann3r/model.py:225-242): a 768-wide value encoder and no pos_patch_embed
         spec = synth.usefeat_spec() if self.use_feat else synth.load_spec()
@@ -282,6 +289,13 @@ class Spann3R(ParamModule):
         if dus3r_name is not None:
             self._init_like_reference()
             self._load_dust3r(dus3r_name)
+
+    def set_precision(self, precision: str):
+        """"fp32" (default): fp32-grade GEMMs everywhere.  "bf16": one bf16 tensor-core product per GEMM in the encoder,
+        decoder, key heads and value encoder (inference only).  Engines of both precisions share the packed weights."""
+        if precision not in PRECISIONS:
+            raise ValueError(f"precision must be one of {sorted(PRECISIONS)}, got {precision!r}")
+        self.precision = precision
 
     # -- checkpoint plumbing -----------------------------------------------------------------------
     def _load_dust3r(self, path):
@@ -367,13 +381,16 @@ class Spann3R(ParamModule):
         return self._packed
 
     def _engine_for(self, B, H, W, n_frames=2, encode_only=False, training=False) -> Engine:
+        if training and self.precision != "fp32":
+            raise NotImplementedError(f"precision {self.precision!r} is inference only: the training backward recomputes the "
+                                      "fp32-grade forward, not this one (set_precision('fp32') to train)")
         w = self._weights_train() if training else self._weights()
         max_images = max(2 * B, min(n_frames * B, self.max_encode_batch * B))
-        key = (B, H, W)
+        key = (B, H, W, self.precision)
         eng = self._engines.get(key)
         if eng is None or eng.max_images < max_images:
             self._engines.pop(key, None)
-            eng = Engine(w, B, H, W, max_images=max_images)
+            eng = Engine(w, B, H, W, max_images=max_images, precision=self.precision)
             self._engines[key] = eng
         return eng
 
@@ -405,6 +422,8 @@ class Spann3R(ParamModule):
         """spann3r/model.py:473-539.  Eval mode: the inference path below.  Training mode (`self.training`): the same CUDA
         forward with the reference's training branches and a PyTorch-recompute backward (`train.py`)."""
         if self.training:      # also under torch.no_grad(): the training BRANCHES are what .train() selects, as in the reference
+            if self.precision != "fp32":
+                raise NotImplementedError(f"precision {self.precision!r} is inference only (set_precision('fp32') to train)")
             from .train import forward_train
             return forward_train(self, frames, return_memory)
         return self._forward_eval(frames, return_memory)
