@@ -436,6 +436,25 @@ int s3r_engine_memory_append(s3r_engine* e, const s3r_bank* bank, const float* f
                              void* stream);
 /* spann3r/model.py:97-118 check_sim: out[b, t] = mean cosine vs each of the last wm frames (device array [B, wm]) */
 int s3r_engine_check_sim(s3r_engine* e, const s3r_bank* bank, const float* feat_k, int wm, float* out, void* stream);
+/* Per-slot memory stages: independent sequences in one batch.  Slot b is batch item b of the engine and owns its region
+ * of the bank buffers; its length is lens[b] (host array of e's batch size; bank->len is not read).  The engine's batch
+ * must be at most S3R_MAX_SLOTS.  Every argument is validated before anything is launched.
+ * Tail contract: in every slot, the K_n rows and V_n^T columns in [lens[b], max(lens)) must hold finite values (the
+ * probabilities there are zero, and 0 * NaN is NaN on the tensor core); a zero-initialised bank whose resets and prunes
+ * zero what they leave behind satisfies it. */
+#define S3R_MAX_SLOTS 64
+/* memory_read with per-slot lengths (eval mode: no dropout).  A slot of length 0 reads nothing: out[b] = feat[b] exactly.
+ * bank.attn of slot b gains the column sums of its columns < lens[b] only.  0 <= lens[b] <= cap. */
+int s3r_engine_memory_read_slots(s3r_engine* e, const s3r_bank* bank, const int* lens, const float* feat, float thresh,
+                                 float* out, void* stream);
+/* add_mem per slot: slot b with append[b] != 0 takes its N tokens at offset lens[b] (lens[b] + N <= cap; the caller then
+ * adds N to its length); a slot with append[b] == 0 is left untouched. */
+int s3r_engine_memory_append_slots(s3r_engine* e, const s3r_bank* bank, const int* lens, const int* append,
+                                   const float* feat_k, const float* feat_v, void* stream);
+/* check_sim per slot: out[b, t] (device array [B, 8]) = mean cosine vs frame t of the last wm[b] frames ending at lens[b]
+ * (0 <= wm[b] <= 8, wm[b] * N <= lens[b]); entries t >= wm[b] are -inf, so a row's max is the slot's gate value. */
+int s3r_engine_check_sim_slots(s3r_engine* e, const s3r_bank* bank, const int* lens, const int* wm, const float* feat_k,
+                               float* out, void* stream);
 /* algorithmic FLOPs (2*M*N*K of every tensor-core launch) issued since the last call; resets the counter */
 double s3r_engine_take_flops(s3r_engine* e);
 /* Per-launch CUDA-event timing of the tensor-core kernels (bench.py roofline leg): switch on, run, read.

@@ -310,9 +310,13 @@ static __global__ void fill_pos_kernel(int* pos, long long rows, int N, int gw) 
   pos[2 * r] = t / gw;
   pos[2 * r + 1] = t % gw;
 }
-static __global__ void bank_bump_kernel(float* count, float* attn, long long ld, int len, int n_new) {
+// slot b (on[b] != 0) of length lens[b] takes n_new tokens
+static __global__ void bank_bump_kernel(float* count, float* attn, long long ld, const SlotInts lens, const SlotInts on,
+                                        int n_new) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   const int b = blockIdx.y;
+  if (!on[b]) return;
+  const int len = lens[b];
   if (i < len) count[b * ld + i] += 1.0f;           // mem_count += 1   (spann3r/model.py:88)
   else if (i < len + n_new) {                        // new tokens: count = attn = 0   (:89-90)
     count[b * ld + i] = 0.f;
@@ -871,30 +875,16 @@ int s3r_engine_value(s3r_engine* e, const float* pts3d, const float* feat_k1, in
 // ------------------------------------------------------------------------------------------------
 // spatial memory: spann3r/model.py:145-183 (read), :80-95 (append), :97-118 (similarity gate)
 // ------------------------------------------------------------------------------------------------
-int s3r_engine_memory_read(s3r_engine* e, const s3r_bank* bank, const float* feat, float thresh, float* out,
-                           void* stream) {
-  return s3r_engine_memory_read_train(e, bank, feat, thresh, 0.f, 0ull, out, stream);
-}
+// Every memory stage runs per slot (batch item b of the engine: its own region of the bank buffers) with its own length
+// lens[b]; the single-length entry points below are the same code with one length for every slot.
+static_assert(MEM_MAX_SLOTS == S3R_MAX_SLOTS, "the slot arrays of the kernels hold S3R_MAX_SLOTS entries");
+namespace {
 
-// training-mode read (spann3r/model.py:474 attn_thresh = 0, :167-168 dropout on the attention weights): same launches, the
-// softmax stage additionally applies the Philox keep-scale of (seed, row * M + column)
-int s3r_engine_memory_read_train(s3r_engine* e, const s3r_bank* bank, const float* feat, float thresh, float drop_p,
-                                 uint64_t seed, float* out, void* stream) {
-  cudaStream_t st = (cudaStream_t)stream;
-  S3R_ENGINE_DEVICE(e, "s3r_engine_memory_read");
-  if (!(drop_p >= 0.f && drop_p < 1.f)) {
-    set_error("s3r_engine_memory_read: dropout probability %g outside [0, 1)", (double)drop_p);
-    return -1;
-  }
-  const int B = e->B, N = e->N, M = bank->len, cap = bank->cap;
-  if (M <= 0 || M > cap || cap % 8 != 0) {
-    set_error("s3r_engine_memory_read: bad bank (len=%d cap=%d; cap must be a multiple of 8)", M, cap);
-    return -1;
-  }
-  if (M > MEM_SOFTMAX_MAX_LEN) {  // before any allocation or launch: the softmax keeps a whole score row in shared memory
-    set_error("s3r_engine_memory_read: bank of %d tokens exceeds the %d-token row buffer of the softmax", M,
-              MEM_SOFTMAX_MAX_LEN);
-    return -1;
+int memory_read_slots(s3r_engine* e, const s3r_bank* bank, const SlotInts& lens, int Mmax, const float* feat, float thresh,
+                      float drop_p, uint64_t seed, float* out, cudaStream_t st) {
+  const int B = e->B, N = e->N, cap = bank->cap;
+  if (Mmax == 0) {   // every slot empty: P is all zero, out = feat
+    return cudaMemcpyAsync(out, feat, (size_t)B * N * 1024 * sizeof(float), cudaMemcpyDeviceToDevice, st) == cudaSuccess ? 0 : -6;
   }
   if (cap > e->mem_cap) {  // (re)size the score / probability scratch for this bank capacity (rare)
     e->release(e->Sm); e->release(e->Pm.hi); e->release(e->Pm.lo);   // the old scratch is dead: no stage is in flight on it
@@ -904,34 +894,31 @@ int s3r_engine_memory_read_train(s3r_engine* e, const s3r_bank* bank, const floa
     e->mem_cap = cap;
     e->pc_memread.clear();
   }
-  // plans bake in (len, cap, bank pointers): a process that keeps creating banks at new addresses must not grow the
-  // cache without bound (one sequence touches <= 16 distinct lengths)
+  // plans bake in (longest length, cap, bank pointers): a process that keeps creating banks at new addresses must not grow
+  // the cache without bound (one sequence touches <= 16 distinct lengths)
   if (e->pc_memread.size() > 256) e->pc_memread.clear();
-  PlanCache& pc = e->pc_memread[std::make_tuple((long long)M, (long long)cap, (const void*)bank->kn_hi, (const void*)bank->kn_lo,
+  PlanCache& pc = e->pc_memread[std::make_tuple((long long)Mmax, (long long)cap, (const void*)bank->kn_hi, (const void*)bank->kn_lo,
                                                 (const void*)bank->vnt_hi, (const void*)bank->vnt_lo)];
   pc.begin();
   const long long R = (long long)B * N;
-  const int Mpad = (M + 7) / 8 * 8;
+  const int Mpad = (Mmax + 7) / 8 * 8;
   int r;
   if ((r = e->ln(feat, e->w.norm_q, 0, 0, 1e-5f, R, 1024, nullptr, 0, e->Qn, 1024, 0, 0, st))) return r;
-  {  // S = LN_q(feat) . LN_k(mem_k)^T, one group per batch item (each sequence has its own bank)
-    Geom g; g.groups = B; g.W = N; g.Kc = 1024; g.N = M; g.b_group_rows = cap; g.b_static = 0;
+  {  // S = LN_q(feat) . LN_k(mem_k)^T, one group per slot (each sequence has its own bank), Mmax columns in every group
+    Geom g; g.groups = B; g.W = N; g.Kc = 1024; g.N = Mmax; g.b_group_rows = cap; g.b_static = 0;
     Epi ep; ep.out = e->Sm; ep.ldo = e->mem_cap;
-    if ((M + 31) / 32 * 32 > cap) {  // the epilogue writes whole 32-column chunks
-      set_error("s3r_engine_memory_read: bank capacity %d must cover len %d rounded up to 32", cap, M);
-      return -1;
-    }
     Planes Kn; Kn.hi = (__nv_bfloat16*)bank->kn_hi; Kn.lo = (__nv_bfloat16*)bank->kn_lo;
     if ((r = e->gemm(pc, e->Qn, Kn, g, ep, st))) return r;
   }
   e->launches += 3;
-  if ((r = launch_mem_softmax(e->Sm, e->mem_cap, R, M, Mpad, 1.0f / 32.0f, thresh, e->Pm.hi, e->Pm.lo, e->mem_cap, st,
-                              drop_p, seed)))
+  if ((r = launch_mem_softmax(e->Sm, e->mem_cap, R, N, lens, Mmax, Mpad, 1.0f / 32.0f, thresh, e->Pm.hi, e->Pm.lo, e->mem_cap,
+                              st, drop_p, seed)))
     return r;
   // the fp32 scores are dead once the softmax has run: Sm doubles as the [B, chunks, mem_cap] partial-sum scratch
-  if ((r = launch_mem_colsum(e->Pm.hi, e->Pm.lo, e->mem_cap, B, N, M, bank->attn, cap, e->Sm, e->mem_cap, st))) return r;
-  {  // out = attn . LN_v(mem_v) + feat
-    Geom g; g.groups = B; g.W = N; g.Kc = M; g.N = 1024; g.lda = e->mem_cap; g.ldb = cap; g.b_group_rows = 1024; g.b_static = 0;
+  if ((r = launch_mem_colsum(e->Pm.hi, e->Pm.lo, e->mem_cap, B, N, lens, Mmax, bank->attn, cap, e->Sm, e->mem_cap, st)))
+    return r;
+  {  // out = attn . LN_v(mem_v) + feat; P is zero past each slot's length, where V_n^T must only be finite
+    Geom g; g.groups = B; g.W = N; g.Kc = Mmax; g.N = 1024; g.lda = e->mem_cap; g.ldb = cap; g.b_group_rows = 1024; g.b_static = 0;
     Epi ep; ep.res1 = feat; ep.ldr1 = 1024; ep.out = out; ep.ldo = 1024;
     Planes Vt; Vt.hi = (__nv_bfloat16*)bank->vnt_hi; Vt.lo = (__nv_bfloat16*)bank->vnt_lo;
     if ((r = e->gemm(pc, e->Pm, Vt, g, ep, st))) return r;
@@ -940,18 +927,33 @@ int s3r_engine_memory_read_train(s3r_engine* e, const s3r_bank* bank, const floa
   return 0;
 }
 
-int s3r_engine_memory_append(s3r_engine* e, const s3r_bank* bank, const float* feat_k, const float* feat_v,
-                             void* stream) {
-  cudaStream_t st = (cudaStream_t)stream;
-  S3R_ENGINE_DEVICE(e, "s3r_engine_memory_append");
-  const int B = e->B, N = e->N, M = bank->len, cap = bank->cap;
-  if (M + N > cap) {
-    set_error("s3r_engine_memory_append: bank full (len=%d + %d > cap=%d)", M, N, cap);
+// Checks shared by the read entry points, before anything is allocated or launched
+int memory_read_check(const char* what, const s3r_bank* bank, int Mmax) {
+  const int cap = bank->cap;
+  if (cap <= 0 || cap % 8 != 0) {
+    set_error("%s: bad bank (cap=%d must be a positive multiple of 8)", what, cap);
     return -1;
   }
-  int r;
+  if (Mmax > MEM_SOFTMAX_MAX_LEN) {  // the softmax keeps a whole score row in shared memory
+    set_error("%s: bank of %d tokens exceeds the %d-token row buffer of the softmax", what, Mmax, MEM_SOFTMAX_MAX_LEN);
+    return -1;
+  }
+  if ((Mmax + 31) / 32 * 32 > cap) {  // the score GEMM's epilogue writes whole 32-column chunks
+    set_error("%s: bank capacity %d must cover len %d rounded up to 32", what, cap, Mmax);
+    return -1;
+  }
+  return 0;
+}
+
+int memory_append_slots(s3r_engine* e, const s3r_bank* bank, const SlotInts& lens, const SlotInts& on, const float* feat_k,
+                        const float* feat_v, cudaStream_t st) {
+  const int B = e->B, N = e->N, cap = bank->cap;
+  int r, Mmax = -1;
   Planes Kn; Kn.hi = (__nv_bfloat16*)bank->kn_hi; Kn.lo = (__nv_bfloat16*)bank->kn_lo;
   for (int b = 0; b < B; ++b) {
+    if (!on[b]) continue;
+    const int M = lens[b];
+    Mmax = M > Mmax ? M : Mmax;
     const size_t src = (size_t)b * N * 1024, dst = ((size_t)b * cap + M) * 1024;
     // normalised keys straight into the bank rows
     Planes kd; kd.hi = Kn.hi + dst; kd.lo = Kn.lo + dst;
@@ -960,19 +962,105 @@ int s3r_engine_memory_append(s3r_engine* e, const s3r_bank* bank, const float* f
     cudaMemcpyAsync(bank->k_raw + dst, feat_k + src, (size_t)N * 1024 * sizeof(float), cudaMemcpyDeviceToDevice, st);
     cudaMemcpyAsync(bank->v_raw + dst, feat_v + src, (size_t)N * 1024 * sizeof(float), cudaMemcpyDeviceToDevice, st);
   }
-  // normalised values -> transposed planes [B, 1024, cap] at columns [M, M+N)
+  if (Mmax < 0) return 0;   // no slot appends
+  // normalised values -> transposed planes [B, 1024, cap] at columns [lens[b], lens[b] + N)
   if ((r = e->ln(feat_v, e->w.norm_v, 0, 0, 1e-5f, (long long)B * N, 1024, e->ln_tmp, 1024, Planes(), 0, 0, 0, st))) return r;
   e->launches += 2;
   if ((r = launch_split_transpose(e->ln_tmp, B, N, 1024, (__nv_bfloat16*)bank->vnt_hi, (__nv_bfloat16*)bank->vnt_lo, cap,
-                                  (long long)1024 * cap, M, st)))
+                                  (long long)1024 * cap, lens, on, st)))
     return r;
-  dim3 grid((M + N + 255) / 256, B);
-  bank_bump_kernel<<<grid, 256, 0, st>>>(bank->count, bank->attn, cap, M, N);
+  dim3 grid((Mmax + N + 255) / 256, B);
+  bank_bump_kernel<<<grid, 256, 0, st>>>(bank->count, bank->attn, cap, lens, on, N);
   return cudaGetLastError() == cudaSuccess ? 0 : -6;
 }
 
+// host arrays of a _slots call -> SlotInts, with the slot count checked
+int read_slots_arg(const char* what, const s3r_engine* e, const int* a, SlotInts& s) {
+  if (e->B > MEM_MAX_SLOTS) {
+    set_error("%s: engine batch %d exceeds the %d slots of a per-slot call", what, e->B, MEM_MAX_SLOTS);
+    return -1;
+  }
+  if (!a) {
+    set_error("%s: NULL slot array", what);
+    return -1;
+  }
+  s = SlotInts{};
+  s.n = e->B;
+  for (int b = 0; b < e->B; ++b) s.v[b] = a[b];
+  return 0;
+}
+
+}  // namespace
+
+int s3r_engine_memory_read(s3r_engine* e, const s3r_bank* bank, const float* feat, float thresh, float* out,
+                           void* stream) {
+  return s3r_engine_memory_read_train(e, bank, feat, thresh, 0.f, 0ull, out, stream);
+}
+
+// training-mode read (spann3r/model.py:474 attn_thresh = 0, :167-168 dropout on the attention weights): same launches, the
+// softmax stage additionally applies the Philox keep-scale of (seed, row * M + column)
+int s3r_engine_memory_read_train(s3r_engine* e, const s3r_bank* bank, const float* feat, float thresh, float drop_p,
+                                 uint64_t seed, float* out, void* stream) {
+  S3R_ENGINE_DEVICE(e, "s3r_engine_memory_read");
+  if (!(drop_p >= 0.f && drop_p < 1.f)) {
+    set_error("s3r_engine_memory_read: dropout probability %g outside [0, 1)", (double)drop_p);
+    return -1;
+  }
+  const int M = bank->len, cap = bank->cap;
+  if (M <= 0 || M > cap || cap % 8 != 0) {
+    set_error("s3r_engine_memory_read: bad bank (len=%d cap=%d; cap must be a multiple of 8)", M, cap);
+    return -1;
+  }
+  if (int r = memory_read_check("s3r_engine_memory_read", bank, M)) return r;
+  return memory_read_slots(e, bank, slot_uniform(M), M, feat, thresh, drop_p, seed, out, (cudaStream_t)stream);
+}
+
+int s3r_engine_memory_read_slots(s3r_engine* e, const s3r_bank* bank, const int* lens, const float* feat, float thresh,
+                                 float* out, void* stream) {
+  const char* what = "s3r_engine_memory_read_slots";
+  S3R_ENGINE_DEVICE(e, what);
+  SlotInts L;
+  if (int r = read_slots_arg(what, e, lens, L)) return r;
+  int Mmax = 0;
+  for (int b = 0; b < e->B; ++b) {
+    if (L.v[b] < 0 || L.v[b] > bank->cap) {
+      set_error("%s: slot %d length %d outside [0, cap=%d]", what, b, L.v[b], bank->cap);
+      return -1;
+    }
+    Mmax = L.v[b] > Mmax ? L.v[b] : Mmax;
+  }
+  if (int r = memory_read_check(what, bank, Mmax)) return r;
+  return memory_read_slots(e, bank, L, Mmax, feat, thresh, 0.f, 0ull, out, (cudaStream_t)stream);
+}
+
+int s3r_engine_memory_append(s3r_engine* e, const s3r_bank* bank, const float* feat_k, const float* feat_v,
+                             void* stream) {
+  S3R_ENGINE_DEVICE(e, "s3r_engine_memory_append");
+  const int N = e->N, M = bank->len, cap = bank->cap;
+  if (M + N > cap) {
+    set_error("s3r_engine_memory_append: bank full (len=%d + %d > cap=%d)", M, N, cap);
+    return -1;
+  }
+  return memory_append_slots(e, bank, slot_uniform(M), slot_uniform(1), feat_k, feat_v, (cudaStream_t)stream);
+}
+
+int s3r_engine_memory_append_slots(s3r_engine* e, const s3r_bank* bank, const int* lens, const int* append,
+                                   const float* feat_k, const float* feat_v, void* stream) {
+  const char* what = "s3r_engine_memory_append_slots";
+  S3R_ENGINE_DEVICE(e, what);
+  SlotInts L, A;
+  if (int r = read_slots_arg(what, e, lens, L)) return r;
+  if (int r = read_slots_arg(what, e, append, A)) return r;
+  for (int b = 0; b < e->B; ++b) {
+    if (L.v[b] < 0 || L.v[b] + (A.v[b] ? e->N : 0) > bank->cap) {
+      set_error("%s: slot %d of length %d cannot take %d tokens (cap=%d)", what, b, L.v[b], A.v[b] ? e->N : 0, bank->cap);
+      return -1;
+    }
+  }
+  return memory_append_slots(e, bank, L, A, feat_k, feat_v, (cudaStream_t)stream);
+}
+
 int s3r_engine_check_sim(s3r_engine* e, const s3r_bank* bank, const float* feat_k, int wm, float* out, void* stream) {
-  cudaStream_t st = (cudaStream_t)stream;
   S3R_ENGINE_DEVICE(e, "s3r_engine_check_sim");
   const int B = e->B, N = e->N;
   if (wm <= 0 || wm > 8 || wm * N > bank->len) {
@@ -980,8 +1068,30 @@ int s3r_engine_check_sim(s3r_engine* e, const s3r_bank* bank, const float* feat_
     return -1;
   }
   e->launches += 2;
-  const float* wmem = bank->k_raw + (size_t)(bank->len - wm * N) * 1024;  // last wm*N tokens (spann3r/model.py:102-105)
-  return launch_check_sim(feat_k, wmem, (long long)bank->cap * 1024, B, wm, N, 1024, e->sim_scratch, out, st);
+  // last wm*N tokens (spann3r/model.py:102-105)
+  return launch_check_sim(feat_k, bank->k_raw, (long long)bank->cap * 1024, B, slot_uniform(bank->len - wm * N),
+                          slot_uniform(wm), N, 1024, e->sim_scratch, out, wm, (cudaStream_t)stream);
+}
+
+int s3r_engine_check_sim_slots(s3r_engine* e, const s3r_bank* bank, const int* lens, const int* wm, const float* feat_k,
+                               float* out, void* stream) {
+  const char* what = "s3r_engine_check_sim_slots";
+  S3R_ENGINE_DEVICE(e, what);
+  const int B = e->B, N = e->N;
+  SlotInts L, W;
+  if (int r = read_slots_arg(what, e, lens, L)) return r;
+  if (int r = read_slots_arg(what, e, wm, W)) return r;
+  SlotInts start = L;
+  for (int b = 0; b < B; ++b) {
+    if (L.v[b] < 0 || L.v[b] > bank->cap || W.v[b] < 0 || W.v[b] > 8 || W.v[b] * N > L.v[b]) {
+      set_error("%s: slot %d: wm=%d invalid for length %d (cap=%d)", what, b, W.v[b], L.v[b], bank->cap);
+      return -1;
+    }
+    start.v[b] = L.v[b] - W.v[b] * N;
+  }
+  e->launches += 2;
+  return launch_check_sim(feat_k, bank->k_raw, (long long)bank->cap * 1024, B, start, W, N, 1024, e->sim_scratch, out, 8,
+                          (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -53,18 +53,31 @@ int attn_launch(const AttnPlan& plan, __nv_bfloat16* o_hi, __nv_bfloat16* o_lo, 
 // spatial memory (memory.cu)
 // longest bank the softmax takes: one fp32 score row in shared memory, up to 200 KB of it
 constexpr int MEM_SOFTMAX_MAX_LEN = 200 * 1024 / 4;
-int launch_mem_softmax(const float* S, long long ldS, long long rows, int M, int Mpad, float scale, float thresh,
-                       __nv_bfloat16* phi, __nv_bfloat16* plo, long long ldP, cudaStream_t st, float drop_p = 0.f,
-                       unsigned long long seed = 0);
+// One int per batch item ("slot") of a memory stage, passed by value as a launch parameter: n == 1 holds one value for
+// every slot (any batch size), otherwise v[b] is slot b's (b < MEM_MAX_SLOTS == S3R_MAX_SLOTS).
+constexpr int MEM_MAX_SLOTS = 64;
+struct SlotInts {
+  int n;
+  int v[MEM_MAX_SLOTS];
+  __host__ __device__ int operator[](int b) const { return v[n == 1 ? 0 : b]; }
+};
+inline SlotInts slot_uniform(int x) { SlotInts s{}; s.n = 1; s.v[0] = x; return s; }
+// rows = slots * nq; row r belongs to slot r / nq and has lens[r / nq] scores; Mpad (multiple of 8) >= every length
+int launch_mem_softmax(const float* S, long long ldS, long long rows, int nq, const SlotInts& lens, int Mmax, int Mpad,
+                       float scale, float thresh, __nv_bfloat16* phi, __nv_bfloat16* plo, long long ldP, cudaStream_t st,
+                       float drop_p = 0.f, unsigned long long seed = 0);
 // training-mode dropout of the memory read: out[i] = keep-scale (0 or 1 / (1 - p)) of flat element i under `seed`
 int launch_dropout_mask(float* out, long long n, unsigned long long seed, float p, cudaStream_t st);
-// part: scratch of B * ceil(nq/32) rows of ld_part floats (ld_part >= M rounded up to 8)
-int launch_mem_colsum(const __nv_bfloat16* phi, const __nv_bfloat16* plo, long long ldP, int B, int nq, int M,
-                      float* mem_attn, long long ld_attn, float* part, long long ld_part, cudaStream_t st);
+// part: scratch of B * ceil(nq/32) rows of ld_part floats (ld_part >= Mmax rounded up to 8); slot b adds columns < lens[b]
+int launch_mem_colsum(const __nv_bfloat16* phi, const __nv_bfloat16* plo, long long ldP, int B, int nq, const SlotInts& lens,
+                      int Mmax, float* mem_attn, long long ld_attn, float* part, long long ld_part, cudaStream_t st);
+// slot b (on[b] != 0) is written at columns col0[b] + t
 int launch_split_transpose(const float* x, int B, int T, int C, __nv_bfloat16* ohi, __nv_bfloat16* olo, long long ldo,
-                           long long out_batch_stride, int col0, cudaStream_t st);
-int launch_check_sim(const float* feat, const float* wm, long long wm_batch_stride, int B, int T, int P, int C,
-                     float* scratch, float* out, cudaStream_t st);
+                           long long out_batch_stride, const SlotInts& col0, const SlotInts& on, cudaStream_t st);
+// slot b compares with wm[b] frames of P tokens starting at token start[b] of its k rows; out[b * ldo + t], t < ldo,
+// is -inf for t >= wm[b]
+int launch_check_sim(const float* feat, const float* k, long long k_batch_stride, int B, const SlotInts& start,
+                     const SlotInts& wm, int P, int C, float* scratch, float* out, int ldo, cudaStream_t st);
 
 // input adapter (preprocess.cu): Pillow's 8-bit Lanczos resample passes, crops folded in
 int launch_resample_h_u8(const uint8_t* src, long long row_stride, int rows, int out_cols, const int* bounds,

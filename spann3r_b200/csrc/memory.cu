@@ -47,17 +47,28 @@ __global__ void dropout_mask_kernel(float* __restrict__ out, long long n, unsign
     out[i] = dropout_scale(seed, (unsigned long long)i, p, ks);
 }
 
-__global__ void __launch_bounds__(256) mem_softmax_kernel(const float* __restrict__ S, long long ldS, int M, int Mpad,
-                                                          float scale, float thresh, __nv_bfloat16* __restrict__ phi,
-                                                          __nv_bfloat16* __restrict__ plo, long long ldP, float drop_p,
-                                                          float keep_scale, unsigned long long seed) {
+// Row r belongs to slot r / nq and reads that slot's length M = lens[r / nq] (its bank); a slot of length 0 gets an
+// all-zero row, so that P V adds nothing to its queries.
+__global__ void __launch_bounds__(256) mem_softmax_kernel(const float* __restrict__ S, long long ldS, int nq,
+                                                          const SlotInts lens, int Mpad, float scale, float thresh,
+                                                          __nv_bfloat16* __restrict__ phi, __nv_bfloat16* __restrict__ plo,
+                                                          long long ldP, float drop_p, float keep_scale,
+                                                          unsigned long long seed) {
   pdl_launch_dependents();
   pdl_wait();
   extern __shared__ float row[];
   __shared__ float red[8];
   const long long r = blockIdx.x;
-  const float* s = S + r * ldS;
+  const int M = lens[(int)(r / nq)];
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  if (M == 0) {
+    for (int i = tid; i < (Mpad >> 2); i += 256) {
+      *reinterpret_cast<uint2*>(phi + r * ldP + 4 * i) = make_uint2(0u, 0u);
+      *reinterpret_cast<uint2*>(plo + r * ldP + 4 * i) = make_uint2(0u, 0u);
+    }
+    return;
+  }
+  const float* s = S + r * ldS;
   auto block_reduce = [&](float v, bool is_max) -> float {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
@@ -164,13 +175,13 @@ int launch_dropout_mask(float* out, long long n, unsigned long long seed, float 
   return cudaGetLastError() == cudaSuccess ? 0 : -6;
 }
 
-int launch_mem_softmax(const float* S, long long ldS, long long rows, int M, int Mpad, float scale, float thresh,
-                       __nv_bfloat16* phi, __nv_bfloat16* plo, long long ldP, cudaStream_t st, float drop_p,
-                       unsigned long long seed) {
-  if (rows == 0 || M == 0) return 0;
-  const size_t smem = (size_t)M * sizeof(float);
-  if (M > MEM_SOFTMAX_MAX_LEN) {
-    set_error("mem_softmax: bank of %d tokens exceeds the %d-token row buffer", M, MEM_SOFTMAX_MAX_LEN);
+int launch_mem_softmax(const float* S, long long ldS, long long rows, int nq, const SlotInts& lens, int Mmax, int Mpad,
+                       float scale, float thresh, __nv_bfloat16* phi, __nv_bfloat16* plo, long long ldP, cudaStream_t st,
+                       float drop_p, unsigned long long seed) {
+  if (rows == 0 || Mmax == 0) return 0;
+  const size_t smem = (size_t)Mmax * sizeof(float);
+  if (Mmax > MEM_SOFTMAX_MAX_LEN) {
+    set_error("mem_softmax: bank of %d tokens exceeds the %d-token row buffer", Mmax, MEM_SOFTMAX_MAX_LEN);
     return -1;
   }
   // Opt in to the large row buffer on first use, whatever this call's size: the kernel's static shared memory counts
@@ -180,11 +191,11 @@ int launch_mem_softmax(const float* S, long long ldS, long long rows, int M, int
     cudaFuncSetAttribute(mem_softmax_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, MEM_SOFTMAX_MAX_LEN * 4);
     once.cur() = true;
   }
-  launch_pdl(mem_softmax_kernel, dim3((unsigned)rows), dim3(256), smem, st, S, ldS, M, Mpad, scale, thresh, phi, plo, ldP,
-             drop_p, (float)(1.0 / (1.0 - (double)drop_p)), seed);
+  launch_pdl(mem_softmax_kernel, dim3((unsigned)rows), dim3(256), smem, st, S, ldS, nq, lens, Mpad, scale, thresh, phi, plo,
+             ldP, drop_p, (float)(1.0 / (1.0 - (double)drop_p)), seed);
   const cudaError_t err = cudaGetLastError();
   if (err != cudaSuccess) {
-    set_error("mem_softmax: launch of %d rows x %d tokens failed: %s", (int)rows, M, cudaGetErrorString(err));
+    set_error("mem_softmax: launch of %d rows x %d tokens failed: %s", (int)rows, Mmax, cudaGetErrorString(err));
     return -6;
   }
   return 0;
@@ -235,23 +246,24 @@ __global__ void __launch_bounds__(256) mem_colsum_partial_kernel(const __nv_bflo
   }
 }
 __global__ void __launch_bounds__(256) mem_colsum_final_kernel(const float* __restrict__ part, long long ld_part,
-                                                               int chunks, int M, float* __restrict__ mem_attn,
+                                                               int chunks, const SlotInts lens, float* __restrict__ mem_attn,
                                                                long long ld_attn) {
   pdl_launch_dependents();
   pdl_wait();
   const int m = blockIdx.x * 256 + threadIdx.x, b = blockIdx.y;
-  if (m >= M) return;
+  if (m >= lens[b]) return;
   const float* p = part + (long long)b * chunks * ld_part + m;
   float s = 0.f;
   for (int c = 0; c < chunks; ++c) s += p[c * ld_part];
   mem_attn[b * ld_attn + m] += s;
 }
 
-// P planes are zero beyond M up to Mpad (mem_softmax_kernel) and ldP, Mpad are multiples of 8 (16-byte loads).
-int launch_mem_colsum(const __nv_bfloat16* phi, const __nv_bfloat16* plo, long long ldP, int B, int nq, int M,
-                      float* mem_attn, long long ld_attn, float* part, long long ld_part, cudaStream_t st) {
-  if (M == 0) return 0;
-  const int Mpad = (M + 7) / 8 * 8;
+// P planes are zero beyond each slot's length up to Mpad (mem_softmax_kernel) and ldP, Mpad are multiples of 8 (16-byte
+// loads).
+int launch_mem_colsum(const __nv_bfloat16* phi, const __nv_bfloat16* plo, long long ldP, int B, int nq, const SlotInts& lens,
+                      int Mmax, float* mem_attn, long long ld_attn, float* part, long long ld_part, cudaStream_t st) {
+  if (Mmax == 0) return 0;
+  const int Mpad = (Mmax + 7) / 8 * 8;
   const int chunks = (nq + CS_ROWS - 1) / CS_ROWS;
   if (ldP % 8 != 0 || ld_part < Mpad) {
     set_error("mem_colsum: ldP=%lld must be a multiple of 8 and ld_part=%lld >= %d", ldP, ld_part, Mpad);
@@ -259,23 +271,25 @@ int launch_mem_colsum(const __nv_bfloat16* phi, const __nv_bfloat16* plo, long l
   }
   launch_pdl(mem_colsum_partial_kernel, dim3((Mpad + 255) / 256, chunks, B), dim3(256), 0, st, phi, plo, ldP, nq, Mpad,
              part, ld_part);
-  launch_pdl(mem_colsum_final_kernel, dim3((M + 255) / 256, B), dim3(256), 0, st, (const float*)part, ld_part, chunks, M,
+  launch_pdl(mem_colsum_final_kernel, dim3((Mmax + 255) / 256, B), dim3(256), 0, st, (const float*)part, ld_part, chunks, lens,
              mem_attn, ld_attn);
   return cudaGetLastError() == cudaSuccess ? 0 : -6;
 }
 int mem_colsum_chunks(int nq) { return (nq + CS_ROWS - 1) / CS_ROWS; }
 
 // ------------------------------------------------------------------------------------------------
-// fp32 x[b, t, c] (t < T, c < C)  ->  split-bf16 planes out[b, c, col0 + t] (row stride ldo): the
-// transposed write that appends normalised values to the V_n^T bank.  32x32 smem tile transpose.
+// fp32 x[b, t, c] (t < T, c < C)  ->  split-bf16 planes out[b, c, col0[b] + t] (row stride ldo) for the slots b with
+// on[b] != 0: the transposed write that appends normalised values to the V_n^T bank.  32x32 smem tile transpose.
 // ------------------------------------------------------------------------------------------------
 __global__ void split_transpose_kernel(const float* __restrict__ x, int T, int C, __nv_bfloat16* __restrict__ ohi,
                                        __nv_bfloat16* __restrict__ olo, long long ldo, long long out_batch_stride,
-                                       int col0) {
+                                       const SlotInts col0s, const SlotInts on) {
   pdl_launch_dependents();
   pdl_wait();
   __shared__ float tile[32][33];
   const int b = blockIdx.z;
+  if (!on[b]) return;
+  const int col0 = col0s[b];
   const int t0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
   const float* xb = x + (long long)b * T * C;
   for (int i = threadIdx.y; i < 32; i += blockDim.y) {
@@ -296,20 +310,22 @@ __global__ void split_transpose_kernel(const float* __restrict__ x, int T, int C
 }
 
 int launch_split_transpose(const float* x, int B, int T, int C, __nv_bfloat16* ohi, __nv_bfloat16* olo, long long ldo,
-                           long long out_batch_stride, int col0, cudaStream_t st) {
+                           long long out_batch_stride, const SlotInts& col0, const SlotInts& on, cudaStream_t st) {
   if (B * T * C == 0) return 0;
   dim3 grid((T + 31) / 32, (C + 31) / 32, B), block(32, 8);
-  launch_pdl(split_transpose_kernel, dim3(grid), dim3(block), 0, st, x, T, C, ohi, olo, ldo, out_batch_stride, col0);
+  launch_pdl(split_transpose_kernel, dim3(grid), dim3(block), 0, st, x, T, C, ohi, olo, ldo, out_batch_stride, col0, on);
   return cudaGetLastError() == cudaSuccess ? 0 : -6;
 }
 
 // ------------------------------------------------------------------------------------------------
 // Similarity gate (spann3r/model.py:97-118): out[b, t] = mean_p cos(feat_k[b,p,:], wm[b,t,p,:]) for the
 // last `wm` frames of the raw key bank.  One warp per (b, t, p); per-(b,t) sums are reduced in a fixed
-// order by a second tiny kernel so the > 0.95 decision is reproducible.
+// order by a second tiny kernel so the > 0.95 decision is reproducible.  Each slot b has its own window: wm[b] frames
+// from token start[b] of its rows; T = max wm[b], and warps / outputs past a slot's wm[b] are idle / -inf.
 // ------------------------------------------------------------------------------------------------
-__global__ void cos_rows_kernel(const float* __restrict__ feat, const float* __restrict__ wm, long long wm_batch_stride,
-                                int B, int T, int P, int C, float* __restrict__ cosv) {
+__global__ void cos_rows_kernel(const float* __restrict__ feat, const float* __restrict__ kraw, long long k_batch_stride,
+                                int B, int T, const SlotInts start, const SlotInts wm, int P, int C,
+                                float* __restrict__ cosv) {
   pdl_launch_dependents();
   pdl_wait();
   const long long w = blockIdx.x * (long long)(blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -319,8 +335,10 @@ __global__ void cos_rows_kernel(const float* __restrict__ feat, const float* __r
   const int p = (int)(w % P);
   const int t = (int)((w / P) % T);
   const int b = (int)(w / ((long long)P * T));
+  if (t >= wm[b]) return;
   const float4* a = reinterpret_cast<const float4*>(feat + ((long long)b * P + p) * C);
-  const float4* k = reinterpret_cast<const float4*>(wm + (long long)b * wm_batch_stride + ((long long)t * P + p) * C);
+  const float4* k = reinterpret_cast<const float4*>(kraw + (long long)b * k_batch_stride +
+                                                    ((long long)start[b] + (long long)t * P + p) * C);
   float dot = 0.f, na = 0.f, nk = 0.f;
   for (int i = lane; i < C / 4; i += 32) {
     const float4 x = a[i], y = k[i];
@@ -337,11 +355,18 @@ __global__ void cos_rows_kernel(const float* __restrict__ feat, const float* __r
   if (lane == 0) cosv[w] = dot / (fmaxf(sqrtf(na), 1e-12f) * fmaxf(sqrtf(nk), 1e-12f));  // F.normalize eps
 }
 
-__global__ void mean_rows_kernel(const float* __restrict__ cosv, int P, float* __restrict__ out) {
+// one block per output (b, t < ldo); cosv holds T frames per slot
+__global__ void mean_rows_kernel(const float* __restrict__ cosv, int T, const SlotInts wm, int P, float* __restrict__ out,
+                                 int ldo) {
   pdl_launch_dependents();
   pdl_wait();
   __shared__ float red[256];
-  const float* c = cosv + (long long)blockIdx.x * P;
+  const int b = blockIdx.x / ldo, t = blockIdx.x % ldo;
+  if (t >= wm[b]) {
+    if (threadIdx.x == 0) out[blockIdx.x] = -INFINITY;
+    return;
+  }
+  const float* c = cosv + ((long long)b * T + t) * P;
   float s = 0.f;
   for (int i = threadIdx.x; i < P; i += 256) s += c[i];
   red[threadIdx.x] = s;
@@ -353,13 +378,17 @@ __global__ void mean_rows_kernel(const float* __restrict__ cosv, int P, float* _
   if (threadIdx.x == 0) out[blockIdx.x] = red[0] / (float)P;
 }
 
-int launch_check_sim(const float* feat, const float* wm, long long wm_batch_stride, int B, int T, int P, int C,
-                     float* scratch, float* out, cudaStream_t st) {
-  if (B * T * P == 0) return 0;
+int launch_check_sim(const float* feat, const float* k, long long k_batch_stride, int B, const SlotInts& start,
+                     const SlotInts& wm, int P, int C, float* scratch, float* out, int ldo, cudaStream_t st) {
+  if (B * ldo * P == 0) return 0;
   if (C % 4) { set_error("check_sim: C %% 4 != 0"); return -1; }
+  int T = 0;
+  for (int b = 0; b < (wm.n == 1 ? 1 : B); ++b) T = wm[b] > T ? wm[b] : T;
   const long long total = (long long)B * T * P;
-  launch_pdl(cos_rows_kernel, dim3((unsigned)((total + 7) / 8)), dim3(256), 0, st, feat, wm, wm_batch_stride, B, T, P, C, scratch);
-  launch_pdl(mean_rows_kernel, dim3(B * T), dim3(256), 0, st, scratch, P, out);
+  if (total > 0)
+    launch_pdl(cos_rows_kernel, dim3((unsigned)((total + 7) / 8)), dim3(256), 0, st, feat, k, k_batch_stride, B, T, start,
+               wm, P, C, scratch);
+  launch_pdl(mean_rows_kernel, dim3(B * ldo), dim3(256), 0, st, (const float*)scratch, T, wm, P, out, ldo);
   return cudaGetLastError() == cudaSuccess ? 0 : -6;
 }
 

@@ -81,6 +81,9 @@ _lib.register_protos({
     "s3r_engine_memory_read_train": (_i, [_vp, C.POINTER(Bank), _vp, _f, _f, C.c_uint64, _vp, _vp]),
     "s3r_engine_memory_append": (_i, [_vp, C.POINTER(Bank), _vp, _vp, _vp]),
     "s3r_engine_check_sim": (_i, [_vp, C.POINTER(Bank), _vp, _i, _vp, _vp]),
+    "s3r_engine_memory_read_slots": (_i, [_vp, C.POINTER(Bank), C.POINTER(_i), _vp, _f, _vp, _vp]),
+    "s3r_engine_memory_append_slots": (_i, [_vp, C.POINTER(Bank), C.POINTER(_i), C.POINTER(_i), _vp, _vp, _vp]),
+    "s3r_engine_check_sim_slots": (_i, [_vp, C.POINTER(Bank), C.POINTER(_i), C.POINTER(_i), _vp, _vp, _vp]),
     "s3r_engine_take_flops": (C.c_double, [_vp]),
     "s3r_engine_take_launches": (C.c_longlong, [_vp]),
     "s3r_engine_profile": (None, [_vp, _i]),
@@ -89,6 +92,7 @@ _lib.register_protos({
 })
 
 ROPE_MAXPOS = 64
+MAX_SLOTS = 64      # include/spann3r_b200.h: S3R_MAX_SLOTS, the batch limit of the per-slot memory stages
 VALUE_PTS_TRANSPOSED, VALUE_ROPE, VALUE_DEC_TOKENS = 1, 2, 4   # include/spann3r_b200.h: flags of s3r_engine_value
 
 
@@ -390,6 +394,31 @@ class MemoryBank:
             t[:, :k] = torch.gather(t[:, : self.len], 1, idx)
         self.len = k
 
+    # -- per-slot use (model.SlotMemory): slot b is batch item b with its own length -------------------------------
+    def zero_slot_tail(self, b: int, start: int, end: int):
+        """Zero rows / columns [start, end) of slot b, so that the region past the slot's length stays finite (the
+        tail contract of the per-slot read, include/spann3r_b200.h)."""
+        if end > start:
+            for name in ("kn_hi", "kn_lo", "k_raw", "v_raw", "attn", "count"):
+                getattr(self, name)[b, start:end] = 0
+            for name in ("vnt_hi", "vnt_lo"):
+                getattr(self, name)[b, :, start:end] = 0
+
+    def gather_slot(self, b: int, idx: torch.Tensor, n: int):
+        """Keep rows idx [k] of slot b (length n), in that order, and zero the tail [k, n) they leave behind."""
+        k = idx.shape[0]
+        ie = idx[:, None].expand(-1, 1024)
+        for name in ("kn_hi", "kn_lo", "k_raw", "v_raw"):
+            t = getattr(self, name)
+            t[b, :k] = torch.gather(t[b, :n], 0, ie)
+        for name in ("vnt_hi", "vnt_lo"):
+            t = getattr(self, name)
+            t[b, :, :k] = torch.gather(t[b, :, :n], 1, idx[None].expand(1024, -1))
+        for name in ("attn", "count"):
+            t = getattr(self, name)
+            t[b, :k] = torch.gather(t[b, :n], 0, idx)
+        self.zero_slot_tail(b, k, n)
+
 
 PRECISIONS = {"fp32": 0, "bf16": 1}   # Spann3R(precision=...) -> s3r_engine_create_ex's GEMM precision
 
@@ -501,6 +530,35 @@ class Engine:
         out = self._new(self.B, wm)
         bs = bank.struct()
         self._call("s3r_engine_check_sim", "check_sim", C.byref(bs), _lib.ptr(feat_k), wm, _lib.ptr(out))
+        return out
+
+    # -- per-slot memory stages (independent sequences, one per batch item) ------------------------------------
+    def _slot_ints(self, vals):
+        vals = [int(v) for v in vals]
+        if len(vals) != self.B:
+            raise ValueError(f"expected {self.B} per-slot values, got {len(vals)}")
+        return (_i * self.B)(*vals)
+
+    def memory_read_slots(self, bank: MemoryBank, lens, feat, thresh: float):
+        """memory_read with slot b reading its first lens[b] tokens; a slot of length 0 returns its feat row unchanged."""
+        self._chk(feat, (self.B, self.N, 1024))
+        out = self._new(self.B, self.N, 1024)
+        self._call("s3r_engine_memory_read_slots", "memory_read_slots", C.byref(bank.struct()), self._slot_ints(lens),
+                   _lib.ptr(feat), float(thresh), _lib.ptr(out))
+        return out
+
+    def memory_append_slots(self, bank: MemoryBank, lens, append, feat_k, feat_v):
+        """Slot b with append[b] takes its N tokens at offset lens[b]; the caller tracks the lengths."""
+        self._chk(feat_k, (self.B, self.N, 1024)); self._chk(feat_v, (self.B, self.N, 1024))
+        self._call("s3r_engine_memory_append_slots", "memory_append_slots", C.byref(bank.struct()), self._slot_ints(lens),
+                   self._slot_ints(append), _lib.ptr(feat_k), _lib.ptr(feat_v))
+
+    def check_sim_slots(self, bank: MemoryBank, lens, wm, feat_k) -> torch.Tensor:
+        """[B, 8]: slot b's gate values against its last wm[b] frames ending at lens[b]; -inf past wm[b]."""
+        self._chk(feat_k, (self.B, self.N, 1024))
+        out = self._new(self.B, 8)
+        self._call("s3r_engine_check_sim_slots", "check_sim_slots", C.byref(bank.struct()), self._slot_ints(lens),
+                   self._slot_ints(wm), _lib.ptr(feat_k), _lib.ptr(out))
         return out
 
     def take_flops(self) -> float:

@@ -31,7 +31,7 @@ import torch.nn as nn
 
 from . import synth
 from ._lib import conf_score as _conf_score
-from .engine import PRECISIONS, Engine, MemoryBank, PackedWeights
+from .engine import MAX_SLOTS, PRECISIONS, Engine, MemoryBank, PackedWeights
 
 
 # ------------------------------------------------------------------------------------------------
@@ -264,6 +264,106 @@ class SpatialMemory:
         print("Memory pruned:", n, "->", self.bank.len)
 
 
+class SlotMemory:
+    """One SpatialMemory per batch item ("slot") of an engine, for independent sequences run as one batch
+    (`Spann3R.forward_sequences`).  Each slot applies the reference's add_mem_check / memory_prune
+    (spann3r/model.py:120-143,185-210) exactly as a batch-1 run would: its own length, similarity gate, `wm`, `lm` and
+    prune.  The slots share one MemoryBank (slot b = batch item b) and the per-slot engine stages, so a step costs one
+    launch sequence and one host synchronisation for all gates, as SpatialMemory's lockstep batch does."""
+
+    def __init__(self, long_mem_size=4000, work_mem_size=5, attn_thresh=5e-4, sim_thresh=0.95, *, engine: Engine):
+        if engine.B > MAX_SLOTS:
+            raise ValueError(f"at most {MAX_SLOTS} slots, the engine has a batch of {engine.B}")
+        self.engine = engine
+        self.attn_thresh = attn_thresh
+        self.long_mem_size = long_mem_size
+        self.work_mem_size = work_mem_size
+        self.top_k = long_mem_size
+        self.sim_thresh = sim_thresh
+        self.num_patches = P = engine.N
+        B = engine.B
+        self.bank = MemoryBank(B, long_mem_size + (work_mem_size + 3) * P, engine.device)
+        self.len, self.wm, self.lm = [0] * B, [0] * B, [0] * B
+        self.tags = [None] * B            # what the caller runs in each slot (forward_sequences: the sequence index)
+        self._sim_host = None
+
+    def start(self, b, tag=None):
+        """Empty slot b for a new sequence (init_mem of spann3r/model.py:66-78)."""
+        self.finish(b)
+        self.tags[b] = tag
+
+    def finish(self, b):
+        """Slot b's sequence has ended: zero its bank region (the tail contract) and its counters."""
+        self.bank.zero_slot_tail(b, 0, self.len[b])
+        self.len[b] = self.wm[b] = self.lm[b] = 0
+        self.tags[b] = None
+
+    def memory_read(self, feat):
+        """Slot b reads its own bank; an empty slot returns feat[b] itself."""
+        return self.engine.memory_read_slots(self.bank, self.len, feat, self.attn_thresh)
+
+    def check_sim_async(self, feat_k):
+        """Every slot's gate value (max over its window of mean_p cos) copied to pinned host memory; None when no slot has
+        a window.  The window is the last wm frames, or the whole bank after a prune left fewer (spann3r/model.py:102-105)."""
+        P = self.num_patches
+        wm = [min(w, n // P) for w, n in zip(self.wm, self.len)]
+        if max(wm) == 0 or self.sim_thresh == 1.0:
+            return None
+        vals = self.engine.check_sim_slots(self.bank, self.len, wm, feat_k)
+        if self._sim_host is None:
+            self._sim_host = torch.empty(self.engine.B, dtype=torch.float32, pin_memory=True)
+        self._sim_host.copy_(vals.amax(1), non_blocking=True)
+        ev = torch.cuda.Event()
+        ev.record(torch.cuda.current_stream(vals.device))
+        return ev
+
+    def check_sim_finish(self, pending):
+        """Per slot: True where the gate fired (the write is skipped)."""
+        if pending is None:
+            return [False] * self.engine.B
+        pending.synchronize()
+        out = []
+        for b, mx in enumerate(self._sim_host.tolist()):
+            out.append(mx > self.sim_thresh)
+            if out[-1]:
+                print(f"Similarity detected (slot {b}):", mx)
+        return out
+
+    def add_mem_check(self, feat_k, feat_v, active, sim_pending):
+        """add_mem_check of spann3r/model.py:120-143 for every slot with active[b]; returns the per-slot skip decisions."""
+        skip = self.check_sim_finish(sim_pending)
+        append = [bool(a) and not s for a, s in zip(active, skip)]
+        if any(append):
+            self.engine.memory_append_slots(self.bank, self.len, append, feat_k, feat_v)
+        P = self.num_patches
+        for b, a in enumerate(append):
+            if not a:
+                continue
+            self.len[b] += P
+            self.wm[b] += 1
+            if self.wm[b] > self.work_mem_size:
+                self.wm[b] -= 1
+                if self.long_mem_size == 0:
+                    n = self.len[b]
+                    self.bank.gather_slot(b, torch.arange(P, n, device=self.engine.device), n)
+                    self.len[b] = n - P
+                else:
+                    self.lm[b] += P
+            if self.lm[b] > self.long_mem_size:
+                self.memory_prune(b)
+                self.lm[b] = self.top_k - self.wm[b] * P
+        return skip
+
+    def memory_prune(self, b):  # :185-210 on slot b alone, selection by torch.topk on its [1, n] weights
+        n = self.len[b]
+        weights = self.bank.attn[b:b + 1, :n] / self.bank.count[b:b + 1, :n]
+        weights[self.bank.count[b:b + 1, :n] < self.work_mem_size + 5] = 1e8
+        _, idx = torch.topk(weights, self.top_k, dim=1)
+        self.bank.gather_slot(b, idx[0], n)
+        self.len[b] = self.top_k
+        print(f"Memory pruned (slot {b}):", n, "->", self.top_k)
+
+
 # ------------------------------------------------------------------------------------------------
 # Spann3R
 # ------------------------------------------------------------------------------------------------
@@ -485,6 +585,104 @@ class Spann3R(ParamModule):
         if self.use_feat:
             return eng.value(None, feat_k1, rope=self.mem_pos_enc, tokens=True)
         return eng.value(pts1, feat_k1, transposed=portrait, rope=self.mem_pos_enc)
+
+    # -- independent sequences in one batch ------------------------------------------------------------------
+    def forward_sequences(self, sequences, max_batch: int = 8):
+        """Reconstruct many sequences, batched, each exactly as `forward(sequence)` would at batch 1: its own similarity
+        gate, working / long-term counters, prune and bank length (`SlotMemory`).  `forward` with B > 1 instead couples
+        the batch (one gate, shared counters: the reference's semantics); this does not.
+
+        sequences: list of sequences, each a list of >= 2 view dicts {'img': [1, 3, H, W]}; they may differ in length and
+        resolution.  Sequences of one resolution run on one engine with up to `max_batch` slots; a slot whose sequence
+        ends takes the next waiting one, and slots left without a sequence run on zero features with no memory writes.
+        Returns one (preds, preds_all) per sequence, in input order, with the keys and shapes of `forward`.  Eval only."""
+        if self.training:
+            raise NotImplementedError("forward_sequences is an inference path; call .eval() first")
+        if not 1 <= max_batch <= MAX_SLOTS:
+            raise ValueError(f"max_batch must be in [1, {MAX_SLOTS}], got {max_batch}")
+        groups = {}
+        for s, seq in enumerate(sequences):
+            if len(seq) < 2:
+                raise ValueError(f"sequence {s} has {len(seq)} frame(s); the frame loop needs at least 2")
+            img0 = seq[0]["img"]
+            if img0.dim() != 4 or img0.shape[0] != 1:
+                raise ValueError(f"sequence {s}: frames must be single views [1, 3, H, W], got {tuple(img0.shape)}")
+            H, W = img0.shape[-2:]
+            self._check_true_shape(seq, H, W)
+            groups.setdefault((int(H), int(W)), []).append(s)
+        results = [None] * len(sequences)
+        with torch.no_grad():
+            for (H, W), ids in groups.items():
+                self._run_slots([sequences[s] for s in ids], ids, H, W, min(max_batch, len(ids)), results)
+        return results
+
+    def _run_slots(self, seqs, ids, H, W, B, results):
+        """The frame loop of `_frame_loop` over B slots, each advancing its own sequence; refills in input order."""
+        portrait = H > W
+        eng = self._engine_for(B, H, W, n_frames=max(len(q) for q in seqs))
+        N = eng.N
+        mem = SlotMemory(engine=eng)
+        waiting = list(range(len(seqs)))          # positions in seqs, taken in order
+        slot = [None] * B                          # per slot: dict of the running sequence, or None when idle
+        zeros = torch.zeros(1, N, 1024, dtype=torch.float32, device=eng.device)
+
+        def fill(free):
+            """Start the next waiting sequences in the free slots; their frames are encoded in batched calls."""
+            new = []
+            for b in free:
+                if not waiting:
+                    break
+                j = waiting.pop(0)
+                mem.start(b, ids[j])
+                slot[b] = {"j": j, "i": 0, "feats": [], "preds": None, "preds_all": []}
+                new.append(b)
+            imgs = [(b, self._dev(f["img"])) for b in new for f in seqs[slot[b]["j"]]]
+            for s in range(0, len(imgs), eng.max_images):
+                part = imgs[s: s + eng.max_images]
+                out = eng.encode(torch.cat([im for _, im in part], dim=0))
+                for (b, _), f in zip(part, out.view(len(part), 1, N, 1024).unbind(0)):
+                    slot[b]["feats"].append(f)
+
+        fill(range(B))
+        feat_k2 = None
+        while any(st is not None for st in slot):
+            active = [st is not None for st in slot]
+            f1 = torch.cat([st["feats"][st["i"]] if st else zeros for st in slot]).contiguous()
+            f2 = torch.cat([st["feats"][st["i"] + 1] if st else zeros for st in slot]).contiguous()
+            # a slot's first step reads nothing (feat_fuse = feat1, spann3r/model.py:495-500): its bank is empty, and the
+            # read of an empty slot returns its query, here feat1
+            q = f1 if feat_k2 is None else torch.stack(
+                [f1[b] if (st is None or st["i"] == 0) else feat_k2[b] for b, st in enumerate(slot)]).contiguous()
+            feat_fuse = mem.memory_read(q) if max(mem.len) > 0 else q
+            eng.decode(feat_fuse, f2)
+            feat_k1, feat_k2 = eng.keyheads(f1, f2)
+            sim = mem.check_sim_async(feat_k1)
+            pts, conf = eng.heads()
+            mem_v = self._value(eng, pts[0], feat_k1, portrait)
+            mem.add_mem_check(feat_k1, mem_v, active, sim)
+            done = []
+            for b, st in enumerate(slot):
+                if st is None:
+                    continue
+                res1 = {"pts3d": _to_landscape(pts[0, b:b + 1], H, W), "conf": _to_landscape(conf[0, b:b + 1], H, W)}
+                res2 = {"pts3d": _to_landscape(pts[1, b:b + 1], H, W), "conf": _to_landscape(conf[1, b:b + 1], H, W)}
+                res2["pts3d_in_other_view"] = res2.pop("pts3d")
+                if st["preds"] is None:
+                    st["preds"] = [res1]
+                    st["preds_all"] = [(res1, res2)]
+                else:
+                    res1["pts3d_in_other_view"] = res1.pop("pts3d")
+                    st["preds"].append(res1)
+                    st["preds_all"].append((res1, res2))
+                st["i"] += 1
+                if st["i"] == len(seqs[st["j"]]) - 1:
+                    st["preds"].append(res2)
+                    results[ids[st["j"]]] = (st["preds"], st["preds_all"])
+                    mem.finish(b)
+                    slot[b] = None
+                    done.append(b)
+            if done:
+                fill(done)
 
     # -- offline mode (SURVEY.md §8f rank 2) ------------------------------------------------------------
     def find_initial_pair(self, graph, n_frames):

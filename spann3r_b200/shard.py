@@ -32,12 +32,17 @@ def gather_objects(obj):
     return out
 
 
-def run_sharded(forward, sequences, per_gpu_batch: int = 1, rank: int | None = None, world_size: int | None = None):
+def run_sharded(forward, sequences, per_gpu_batch: int = 1, rank: int | None = None, world_size: int | None = None,
+                independent: bool = False):
     """BASELINE config[2] as a function: `sequences` (a list of equal-length lists of view dicts {'img': [1, 3, H, W]},
     the SAME list on every rank) are dealt round-robin to the ranks (`shard_indices`); each rank advances up to
     `per_gpu_batch` of its sequences in lockstep as one batched call of `forward` (= `Spann3R.forward`; sequences in a
     batch must share frame count and resolution) and returns {sequence index: preds of that sequence} for ITS sequences.
-    No collective on the data path; use `gather_objects` for small per-rank summaries."""
+    No collective on the data path; use `gather_objects` for small per-rank summaries.
+
+    independent=True: `forward` is `Spann3R.forward_sequences`, called once with all of the rank's sequences and
+    max_batch = per_gpu_batch; each sequence then runs with its own memory, as at batch 1, and sequences may differ in
+    length and resolution."""
     import torch
     import torch.distributed as dist
     if world_size is None:
@@ -47,6 +52,9 @@ def run_sharded(forward, sequences, per_gpu_batch: int = 1, rank: int | None = N
     if per_gpu_batch < 1:
         raise ValueError("per_gpu_batch must be >= 1")
     mine = shard_indices(len(sequences), world_size, rank)
+    if independent:
+        res = forward([sequences[i] for i in mine], per_gpu_batch)
+        return {i: r[0] for i, r in zip(mine, res)}
     out = {}
     for s0 in range(0, len(mine), per_gpu_batch):
         ids = mine[s0: s0 + per_gpu_batch]
