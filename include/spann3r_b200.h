@@ -252,6 +252,24 @@ int s3r_pcl_stats(const double* x, int64_t n, double threshold, void* workspace,
 /* out[i] = |a[i] . b[idx[i]]| for a [n, 3], b [*, 3] fp64, idx [n] int64 (eval_recon.py's normal consistency). */
 int s3r_pcl_abs_dot(const double* a, const double* b, const int64_t* idx, int64_t n, double* out, void* stream);
 
+/* ---- headless point rendering: spann3r/tools/vis.py:render_frames (an Open3D window, point_size 1) ---------------------
+ * A z-buffer of width * height uint64 keys in caller-owned device memory, 8-byte aligned:
+ * s3r_render_workspace_bytes(width, height) bytes (0 = size out of range; width, height >= 1, width * height < 2^31).
+ * s3r_render_clear empties it.  s3r_render_splat projects n fp32 points [n, 3] with global indices id0 .. id0 + n - 1
+ * (id0 + n < 2^32), skipping those whose uint8 mask entry is 0 (mask NULL = keep all):
+ *   camera (HOST, 16 doubles): [R | t] 3x4 row-major (world -> camera), fx, fy, cx, cy, all finite;
+ *   q = R p + t in fp64 as ((R0 x + R1 y) + R2 z) + t, kept if finite and q.z > z_near (finite, >= 0);
+ *   u = fx (qx / qz) + cx, v = fy (qy / qz) + cy; pixel (floor(u + 0.5), floor(v + 0.5)) if inside the image;
+ *   key = bits(fp32(qz)) << 32 | index, atomicMin into the pixel: the nearest fp32 depth wins, ties -> smaller index.
+ * s3r_render_resolve writes rgb [height, width, 3] uint8: black where empty, else floor(min(1, max(0, c)) * 255 + 0.5)
+ * of colors[index] (fp32 [*, 3], indexed by the global point index).  Deterministic: the result does not depend on the
+ * order of splat calls between two clears. */
+size_t s3r_render_workspace_bytes(int width, int height);
+int s3r_render_clear(void* keys, int width, int height, void* stream);
+int s3r_render_splat(const float* pts, const uint8_t* mask, int64_t n, int64_t id0, const double* camera, double z_near,
+                     int width, int height, void* keys, void* stream);
+int s3r_render_resolve(const void* keys, const float* colors, int width, int height, uint8_t* rgb, void* stream);
+
 /* ---- training / test criteria: spann3r/loss.py:129-369 (Regr3D_t, its ShiftInv / ScaleInv / ScaleShiftInv variants,
  * ConfLoss_t) with L21 (dust3r/losses.py:52-59), forward and backward --------------------------------------------------
  * F >= 2 views of B sequences of H x W pixels.  Pred slot k < F-1 is preds_all[k][0] (frame k: 'pts3d' for k = 0, else

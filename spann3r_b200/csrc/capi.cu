@@ -283,6 +283,18 @@ int s3r_pcl_abs_dot(const double* a, const double* b, const int64_t* idx, int64_
   return launch_pcl_abs_dot(a, b, reinterpret_cast<const long long*>(idx), n, out, S(stream));
 }
 
+size_t s3r_render_workspace_bytes(int width, int height) { return render_workspace_bytes(width, height); }
+int s3r_render_clear(void* keys, int width, int height, void* stream) {
+  return launch_render_clear(keys, width, height, S(stream));
+}
+int s3r_render_splat(const float* pts, const uint8_t* mask, int64_t n, int64_t id0, const double* camera, double z_near,
+                     int width, int height, void* keys, void* stream) {
+  return launch_render_splat(pts, mask, n, id0, camera, z_near, width, height, keys, S(stream));
+}
+int s3r_render_resolve(const void* keys, const float* colors, int width, int height, uint8_t* rgb, void* stream) {
+  return launch_render_resolve(keys, colors, width, height, rgb, S(stream));
+}
+
 size_t s3r_loss_workspace_bytes(const s3r_loss_desc* d) { return loss_workspace_bytes(d); }
 int s3r_loss_forward(const s3r_loss_desc* d, void* workspace, size_t workspace_bytes, float* gt_out, float* pred_out,
                      uint8_t* valid_out, double* results, void* stream) {

@@ -115,6 +115,13 @@ size_t pcl_stats_workspace_bytes();
 int launch_pcl_stats(const double* v, long long n, double threshold, void* workspace, double* out, cudaStream_t st);
 int launch_pcl_abs_dot(const double* a, const double* b, const long long* idx, long long n, double* out, cudaStream_t st);
 
+// headless point rendering (render.cu): z-buffer of w * h uint64 keys, clear / splat one frame / resolve to RGB
+size_t render_workspace_bytes(int w, int h);
+int launch_render_clear(void* keys, int w, int h, cudaStream_t st);
+int launch_render_splat(const float* pts, const uint8_t* mask, long long n, long long id0, const double* camera,
+                        double z_near, int w, int h, void* keys, cudaStream_t st);
+int launch_render_resolve(const void* keys, const float* colors, int w, int h, uint8_t* out, cudaStream_t st);
+
 // conv backward (conv_wgrad.cu): weight gradient over pixels (split-bf16 wgmma, split contraction + fixed-order reduce)
 // and the col2im of the 3x3 stride-2 conv; both validate their arguments before any CUDA call
 size_t conv_wgrad_workspace_bytes(int NB, int H, int W, int N, int Kc, int taps);

@@ -11,7 +11,7 @@ Semantics that differ from the reference's libraries (INTEGRATION.md, "Reconstru
     TransformationEstimationPointToPoint and the default ICPConvergenceCriteria; estimate_normals with
     KDTreeSearchParamKNN(30)); Open3D itself was not run against this module.  Normals use a mean-centred covariance
     and keep the solver's sign; eval.py only reads |n . n|;
-  * no `.ply` files are written.
+  * the `-mask.ply` / `-gt.ply` files are not written here: `spann3r_b200.vis.write_point_cloud` writes them.
 """
 from __future__ import annotations
 
