@@ -172,6 +172,10 @@ int s3r_attention(const float* q, const float* k, const float* vt, int bh, int h
 /* Offline-mode view score: out[0] = mean((conf-1)/conf) over n values (spann3r/model.py:346-352, 372-381);
  * scratch256 = 256 floats of device scratch.  Deterministic. */
 int s3r_conf_score(const float* conf, int64_t n, float* scratch256, float* out, void* stream);
+/* The same score for every image of the engine's confidence output conf [2, batch, H, W] (hw = H * W):
+ * out[i] = s3r_conf_score of image i (i = head * batch + b), bitwise, in one launch pair.
+ * scratch = 2 * batch * 256 floats of device scratch.  1 <= batch <= 32767, hw >= 1, non-null pointers. */
+int s3r_conf_score_batched(const float* conf, int batch, int64_t hw, float* scratch, float* out, void* stream);
 
 /* ---- input adapter (SURVEY.md section 8f rank 3): the reference's CPU preprocessing in front of the path -----------
  * spann3r/datasets/demo.py:57-86 -> dust3r/datasets/base/base_stereo_view_dataset.py:143-194 (centre crop, Lanczos

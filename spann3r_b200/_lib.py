@@ -83,6 +83,7 @@ _PROTOS = {
     "s3r_gemm_tile_n": (_i, [C.POINTER(GemmDesc)]),
     "s3r_attention": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i64, _vp]),
     "s3r_conf_score": (_i, [_vp, _i64, _vp, _vp, _vp]),
+    "s3r_conf_score_batched": (_i, [_vp, _i, _i64, _vp, _vp, _vp]),
     "s3r_dropout_mask": (_i, [_vp, _i64, C.c_uint64, _f, _vp]),
     "s3r_set_option": (_i, [C.c_char_p, _i]),
     "s3r_focal_weiszfeld": (_i, [_vp, _i, _i, _i, _f, _f, _i, _f, _f, _vp, _vp, _vp]),
@@ -290,6 +291,18 @@ def conf_score(conf: torch.Tensor) -> torch.Tensor:
     out = torch.empty(1, dtype=torch.float32, device=conf.device)
     with on_device(conf):
         check(lib().s3r_conf_score(ptr(conf), conf.numel(), ptr(scratch), ptr(out), stream_ptr(conf.device)), "s3r_conf_score")
+    return out
+
+
+def conf_score_batched(conf: torch.Tensor) -> torch.Tensor:
+    """conf [2, B, H, W] (the engine's heads output) -> [2, B]: `conf_score` of every image, bitwise, in one launch pair."""
+    assert conf.is_cuda and conf.dtype == torch.float32 and conf.is_contiguous() and conf.dim() == 4 and conf.shape[0] == 2
+    B, hw = conf.shape[1], conf.shape[2] * conf.shape[3]
+    scratch = torch.empty(2 * B * 256, dtype=torch.float32, device=conf.device)
+    out = torch.empty(2, B, dtype=torch.float32, device=conf.device)
+    with on_device(conf):
+        check(lib().s3r_conf_score_batched(ptr(conf), B, hw, ptr(scratch), ptr(out), stream_ptr(conf.device)),
+              "s3r_conf_score_batched")
     return out
 
 

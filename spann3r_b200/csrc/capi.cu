@@ -317,6 +317,9 @@ int s3r_attn_train_backward(const s3r_attn_train_desc* d, const float* o, const 
 int s3r_conf_score(const float* conf, int64_t n, float* scratch256, float* out, void* stream) {
   return launch_conf_score(conf, n, scratch256, out, S(stream));
 }
+int s3r_conf_score_batched(const float* conf, int batch, int64_t hw, float* scratch, float* out, void* stream) {
+  return launch_conf_score_batched(conf, batch, hw, scratch, out, S(stream));
+}
 
 int s3r_set_option(const char* name, int value) {
   s3r::Options& o = s3r::options();

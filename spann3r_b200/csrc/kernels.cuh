@@ -100,6 +100,7 @@ int launch_focal_median(const float* pts3d, int B, int H, int W, float ppx, floa
                         float* focal, cudaStream_t st);
 
 int launch_conf_score(const float* conf, long long n, float* scratch256, float* out, cudaStream_t st);
+int launch_conf_score_batched(const float* conf, int batch, long long hw, float* scratch, float* out, cudaStream_t st);
 
 // reconstruction metrics (pointcloud.cu): spatial index, 1-NN, k-NN normals, point-to-point ICP, vector statistics
 size_t pcl_index_bytes(long long n);

@@ -395,10 +395,14 @@ int launch_check_sim(const float* feat, const float* k, long long k_batch_stride
 // ------------------------------------------------------------------------------------------------
 // Confidence score of the offline mode (spann3r/model.py:346-352, 372-381): mean over all pixels of
 // (conf - 1) / conf.  Two fixed-shape passes (256 partial sums, then one block): deterministic.
+// The batched score runs the same two kernels with one grid row (partials) / one block (final) per image: image y
+// reads conf + y * n and owns part[y * 256 .. + 256), so each image's value is bitwise the single-image one.
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) conf_partial_kernel(const float* __restrict__ conf, long long n, float* __restrict__ part) {
   pdl_launch_dependents();
   pdl_wait();
+  conf += blockIdx.y * n;
+  part += blockIdx.y * 256LL;
   __shared__ float red[256];
   float s = 0.f;
   for (long long i = blockIdx.x * 256LL + threadIdx.x; i < n; i += 256LL * gridDim.x) {
@@ -416,6 +420,7 @@ __global__ void __launch_bounds__(256) conf_partial_kernel(const float* __restri
 __global__ void __launch_bounds__(256) conf_final_kernel(const float* __restrict__ part, int nparts, long long n, float* __restrict__ out) {
   pdl_launch_dependents();
   pdl_wait();
+  part += blockIdx.x * 256LL;
   __shared__ float red[256];
   red[threadIdx.x] = threadIdx.x < nparts ? part[threadIdx.x] : 0.f;
   __syncthreads();
@@ -423,13 +428,23 @@ __global__ void __launch_bounds__(256) conf_final_kernel(const float* __restrict
     if (threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
     __syncthreads();
   }
-  if (threadIdx.x == 0) out[0] = red[0] / (float)n;
+  if (threadIdx.x == 0) out[blockIdx.x] = red[0] / (float)n;
 }
 
 int launch_conf_score(const float* conf, long long n, float* scratch256, float* out, cudaStream_t st) {
   if (n <= 0) { set_error("conf_score: empty input"); return -1; }
   launch_pdl(conf_partial_kernel, dim3(256), dim3(256), 0, st, conf, n, scratch256);
   launch_pdl(conf_final_kernel, dim3(1), dim3(256), 0, st, (const float*)scratch256, 256, n, out);
+  return cudaGetLastError() == cudaSuccess ? 0 : -6;
+}
+
+int launch_conf_score_batched(const float* conf, int batch, long long hw, float* scratch, float* out, cudaStream_t st) {
+  if (batch < 1 || batch > 32767) { set_error("conf_score_batched: batch %d outside [1, 32767]", batch); return -1; }
+  if (hw < 1) { set_error("conf_score_batched: H*W = %lld must be >= 1", hw); return -1; }
+  if (!conf || !scratch || !out) { set_error("conf_score_batched: null pointer"); return -1; }
+  const unsigned images = 2u * (unsigned)batch;
+  launch_pdl(conf_partial_kernel, dim3(256, images), dim3(256), 0, st, conf, hw, scratch);
+  launch_pdl(conf_final_kernel, dim3(images), dim3(256), 0, st, (const float*)scratch, 256, hw, out);
   return cudaGetLastError() == cudaSuccess ? 0 : -6;
 }
 

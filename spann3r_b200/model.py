@@ -29,7 +29,7 @@ import os
 import torch
 import torch.nn as nn
 
-from . import synth
+from . import offline, synth
 from ._lib import conf_score as _conf_score
 from .engine import MAX_SLOTS, PRECISIONS, Engine, MemoryBank, PackedWeights
 
@@ -536,18 +536,23 @@ class Spann3R(ParamModule):
         self._check_true_shape(frames, H, W)
         eng = self._engine_for(B, H, W, n_frames=F_)
         sp_mem = SpatialMemory(engine=eng)
-        N = eng.N
 
         # The encoder has no dependence on the memory loop: encode every frame up front in large batches
         # (SURVEY.md §3.1); per-image results are identical to the reference's pair / single-frame calls.
-        imgs = [self._dev(f["img"]) for f in frames]
+        feats = self._encode_frames(eng, [self._dev(f["img"]) for f in frames])
+        return self._frame_loop(F_, H, W, eng, sp_mem, lambda i: feats[i], return_memory)
+
+    @staticmethod
+    def _encode_frames(eng, imgs):
+        """Encode the frames imgs ([B, 3, H, W] each) in calls of up to eng.max_images images -> one [B, N, 1024] each."""
+        B = imgs[0].shape[0]
         feats = []
         chunk = max(1, eng.max_images // B)
-        for s in range(0, F_, chunk):
+        for s in range(0, len(imgs), chunk):
             part = imgs[s: s + chunk]
             out = eng.encode(torch.cat(part, dim=0) if len(part) > 1 else part[0])
-            feats += list(out.view(len(part), B, N, 1024).unbind(0))
-        return self._frame_loop(F_, H, W, eng, sp_mem, lambda i: feats[i], return_memory)
+            feats += list(out.view(len(part), B, eng.N, 1024).unbind(0))
+        return feats
 
     def _frame_loop(self, F_, H, W, eng, sp_mem, feat_of, return_memory):
         """The frame loop of spann3r/model.py:484-533 over the already encoded frames."""
@@ -703,30 +708,42 @@ class Spann3R(ParamModule):
         return pair_idx
 
     @torch.no_grad()
-    def offline_reconstruction(self, frames, graph):
+    def offline_reconstruction(self, frames, graph=None, *, scene_graph="complete", prefilter=None, max_batch=None):
         """spann3r/model.py:394-471 + find_next_best_view :359-392 (eval mode).  Every frame is encoded once up front
-        (the reference re-encodes each candidate on every iteration; the features are identical)."""
+        (the reference re-encodes each candidate on every iteration; the features are identical).
+
+        graph: the output of the reference's `inference(make_pairs(...), model.dust3r)` (or `offline.inference`).  With
+        graph=None the initial pair comes from `offline.pair_scores` over `scene_graph` / `prefilter` (single views only),
+        and no pairwise maps are materialised.
+        max_batch: next-best-view candidates decoded per engine call (default 8 without a graph, 1 with one).  Above 1,
+        each step scores its candidates in batches with one host read; the winner is then decoded again at batch 1, so
+        the outputs for a chosen frame do not depend on max_batch -- only a near-tie between candidates can.  Frames of
+        batch B > 1 (the reference's lockstep batch, scored by a mean over the batch) always take the serial loop."""
         if self.training:
             raise NotImplementedError("spann3r_b200 implements the inference path; call .eval() first")
+        if max_batch is None:
+            max_batch = 8 if graph is None else 1
+        if max_batch < 1:
+            raise ValueError(f"max_batch must be >= 1, got {max_batch}")
         n_frames = len(frames)
         idx_todo = list(range(n_frames))
         B, _, H, W = frames[0]["img"].shape
         self._check_true_shape(frames, H, W)
+        if graph is None and B != 1:
+            raise ValueError(f"offline_reconstruction without a graph needs single views [1, 3, H, W], got batch {B}")
         portrait = H > W
         eng = self._engine_for(B, H, W, n_frames=n_frames)
-        N = eng.N
         sp_mem = SpatialMemory(engine=eng)
-        p0, p1 = self.find_initial_pair(graph, n_frames)
+        if graph is not None:
+            p0, p1 = self.find_initial_pair(graph, n_frames)
+        feats = self._encode_frames(eng, [self._dev(f["img"]) for f in frames])
+        if graph is None:
+            p0, p1 = offline.initial_pair(self, feats, H, W, scene_graph, prefilter, max_batch)
         idx_used = [p0, p1]
         idx_todo.remove(p0)
         idx_todo.remove(p1)
-        imgs = [self._dev(f["img"]) for f in frames]
-        feats = []
-        chunk = max(1, eng.max_images // B)
-        for s in range(0, n_frames, chunk):
-            part = imgs[s: s + chunk]
-            out = eng.encode(torch.cat(part, dim=0) if len(part) > 1 else part[0])
-            feats += list(out.view(len(part), B, N, 1024).unbind(0))
+        # the candidate engine: batch K, its own workspace, so the main engine's state is only touched by the winner
+        cand_eng = self._engine_for(min(max_batch, n_frames - 2), H, W) if max_batch > 1 and B == 1 and idx_todo else None
 
         def decode_heads(f_fuse, f2):
             eng.decode(f_fuse, f2)
@@ -742,12 +759,15 @@ class Spann3R(ParamModule):
             if feat_k2 is not None:
                 feat1 = feat2
                 feat_fuse = sp_mem.memory_read(feat_k2, res=True)
-                best_conf, best_id = 0.0, None
-                for i in idx_todo:                                   # find_next_best_view
-                    r1, r2 = decode_heads(feat_fuse, feats[i])
-                    total = float(_conf_score(r1["conf"].contiguous())) + float(_conf_score(r2["conf"].contiguous()))
-                    if total > best_conf:
-                        best_conf, best_id = total, i
+                if cand_eng is not None:
+                    best_id, best_conf = offline.next_best_view(cand_eng, feat_fuse, feats, idx_todo)
+                else:
+                    best_conf, best_id = 0.0, None
+                    for i in idx_todo:                               # find_next_best_view
+                        r1, r2 = decode_heads(feat_fuse, feats[i])
+                        total = float(_conf_score(r1["conf"].contiguous())) + float(_conf_score(r2["conf"].contiguous()))
+                        if total > best_conf:
+                            best_conf, best_id = total, i
                 idx_todo.remove(best_id)
                 idx_used.append(best_id)
                 print(f"next best view: {best_id}, conf: {best_conf}")
