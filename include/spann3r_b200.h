@@ -158,8 +158,11 @@ typedef struct s3r_gemm_desc {
   int precision;
 } s3r_gemm_desc;
 int s3r_gemm(const s3r_gemm_desc* d, void* stream);
-/* tile width the planner would pick (64/128), for tests */
+/* tile width the planner would pick (64/96/128), for tests */
 int s3r_gemm_tile_n(const s3r_gemm_desc* d);
+/* the planner's rule alone, without a descriptor or a device: the tile width for m_tiles 128-row tiles x n columns on
+ * sms SMs, never straddling column col_align (a_swap's swap_col0; 0 = none); force_bn as in s3r_gemm_desc.  -1 = rejected. */
+int s3r_gemm_plan_bn(int64_t m_tiles, int n, int sms, int col_align, int force_bn);
 
 /* Fused multi-head attention core, head dim 64: O = softmax(Q K^T) V per (batch*head) on tf32 wgmma.
  *   q [bh, nq, 64], k [bh, nk, 64] (already RoPE'd / scaled by the QKV epilogue), vt [bh, 64, nk_pad];

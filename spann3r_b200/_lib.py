@@ -81,6 +81,7 @@ _PROTOS = {
     "s3r_col2im_3x3s2": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp]),
     "s3r_gemm": (_i, [C.POINTER(GemmDesc), _vp]),
     "s3r_gemm_tile_n": (_i, [C.POINTER(GemmDesc)]),
+    "s3r_gemm_plan_bn": (_i, [_i64, _i, _i, _i, _i]),
     "s3r_attention": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i64, _vp]),
     "s3r_conf_score": (_i, [_vp, _i64, _vp, _vp, _vp]),
     "s3r_conf_score_batched": (_i, [_vp, _i, _i64, _vp, _vp, _vp]),

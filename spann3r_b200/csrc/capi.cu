@@ -179,7 +179,7 @@ static int fill_plan(const s3r_gemm_desc* d, GemmPlan* plan) {
   if (r) return r;
   const int force_bn = d->epi == S3R_EPI_HEADTAIL ? (d->force_bn == 128 ? 128 : 1128) : d->force_bn;
   r = gemm_plan_init(plan, B(d->a_hi), B(d->a_lo), B(d->b_hi), B(d->b_lo), d->groups, d->nb, d->h, d->w, d->kc,
-                     d->taps, d->n, force_bn, 0, 0, 0, d->precision);
+                     d->taps, d->n, force_bn, 0, 0, 0, d->precision, d->a_swap ? d->swap_col0 : 0);
   if (r) return r;
   GemmArgs& a = plan->args;
   a.epi = d->epi; a.act = d->act; a.plane_relu = d->plane_relu;
@@ -224,6 +224,15 @@ int s3r_gemm_tile_n(const s3r_gemm_desc* d) {
   int r = fill_plan(d, &plan);
   if (r) return r;
   return plan.bn;
+}
+
+int s3r_gemm_plan_bn(int64_t m_tiles, int n, int sms, int col_align, int force_bn) {
+  if (m_tiles < 1 || n < 1 || sms < 1 || col_align < 0) {
+    set_error("s3r_gemm_plan_bn: m_tiles=%lld n=%d sms=%d col_align=%d (positive; col_align >= 0)", (long long)m_tiles,
+              n, sms, col_align);
+    return -1;
+  }
+  return gemm_choose_bn(m_tiles, n, sms, col_align, force_bn);
 }
 
 int s3r_resample_h_u8(const uint8_t* src, int64_t row_stride, int rows, int out_cols, const int32_t* bounds,

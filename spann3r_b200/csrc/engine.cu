@@ -158,7 +158,8 @@ struct s3r_engine {
     if (pc.building) {
       pc.gemms.emplace_back();
       int r = gemm_plan_init(&pc.gemms.back(), A.hi, A.lo, Bw.hi, Bw.lo, g.groups, g.NB, g.H, g.W, g.Kc, g.taps, g.N,
-                             e.epi == EPI_HEADTAIL ? 1128 : g.force_bn, g.lda, g.ldb, g.b_group_rows, pc.precision);
+                             e.epi == EPI_HEADTAIL ? 1128 : g.force_bn, g.lda, g.ldb, g.b_group_rows, pc.precision,
+                             e.a_swap ? e.swap_col0 : 0);
       if (r) return r;
       pc.gemms.back().b_static = (g.b_static && options().prefetch_b) ? 1 : 0;   // decided when the plan is built
     }

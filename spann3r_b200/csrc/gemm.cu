@@ -10,7 +10,7 @@
 // Structure: persistent, warp-specialised, one CTA per SM, 128 x BN output tiles.
 //   warpgroup 0   TMA producer (one warp; registers handed to the consumers with setmaxnreg): per k-block four
 //                 SWIZZLE_64B boxes (A_hi, A_lo: 128 pixels x 32 ch; B_hi, B_lo: BN x 32) into a STAGES-deep smem
-//                 ring (5 stages at BN = 128, 7 at BN = 64); a 3x3 conv is 9 taps whose A box is the same 4-D tensor
+//                 ring (5 / 6 / 7 stages at BN = 128 / 96 / 64); a 3x3 conv is 9 taps whose A box is the same 4-D tensor
 //                 map at (w+dx, h+dy) -- out-of-bounds pixels are zero-filled by TMA, which is exactly the conv's zero
 //                 padding.
 //   warpgroups 1, 2  consumers: each owns 64 rows of the tile and issues per k-block 2 K-steps x 3 wgmma (hi*lo,
@@ -59,8 +59,10 @@ struct GemmCfg {
   static constexpr int STAGES = (kSmemMax - FIXED) / STAGE;
   static constexpr int SMEM = STAGES * STAGE + FIXED;
   static_assert(NP == 3 || NP == 1, "split (3 products) or bf16 (1 product)");
-  // split: 32 KB / 24 KB stages; one product: 16 KB / 12 KB stages, the same 32-channel k-blocks (DESIGN.md §4)
-  static_assert(STAGES == (NP == 3 ? (BN == 128 ? 5 : 7) : (BN == 128 ? 11 : 15)), "ring depth (DESIGN.md §4)");
+  // split: 32 / 28 / 24 KB stages at BN = 128 / 96 / 64; one product: 16 / 14 / 12 KB, the same 32-channel k-blocks
+  // (DESIGN.md §4)
+  static_assert(STAGES == (NP == 3 ? (BN == 128 ? 5 : BN == 96 ? 6 : 7) : (BN == 128 ? 11 : BN == 96 ? 13 : 15)),
+                "ring depth (DESIGN.md §4)");
   static_assert(2 * STAGES * 8 <= 256, "full + empty barriers fit their 256-byte slot");
   static_assert(Stg<32>::WARP_BYTES == 32 * kAccLD * 4, "a warp's staging tile is its own rows of the accumulator chunk");
 };
@@ -68,6 +70,7 @@ struct GemmCfg {
 template <int BN>
 __device__ __forceinline__ void wgmma_bf16(float (&d)[BN / 2], uint64_t da, uint64_t db, int scale_d) {
   if constexpr (BN == 64) wgmma_bf16_n64(d, da, db, scale_d);
+  else if constexpr (BN == 96) wgmma_bf16_n96(d, da, db, scale_d);
   else wgmma_bf16_n128(d, da, db, scale_d);
 }
 
@@ -87,8 +90,9 @@ __global__ void __launch_bounds__(kNumThreads, 1) gemm_bf16x3_kernel(const __gri
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  unsigned long long* const trace = (blockIdx.x == 0) ? args.trace : nullptr;
-  if (trace && threadIdx.x == 0) trace[0] = globaltimer_ns();
+  // CTA 0's timeline: the pointer is read from the parameters at each stamp, not held in registers through the kernel
+  const bool trace = blockIdx.x == 0 && args.trace != nullptr;
+  if (trace && threadIdx.x == 0) args.trace[0] = globaltimer_ns();
 
   const int n_tiles = (args.N + BN - 1) / BN;
   const int m_tiles = args.tiles_w * args.tiles_h * args.NB;
@@ -111,7 +115,7 @@ __global__ void __launch_bounds__(kNumThreads, 1) gemm_bf16x3_kernel(const __gri
   }
   __syncthreads();
   pdl_launch_dependents();
-  if (trace && threadIdx.x == 0) trace[1] = globaltimer_ns();
+  if (trace && threadIdx.x == 0) args.trace[1] = globaltimer_ns();
   // Weights do not depend on the previous kernel: the producer stages the B tiles of the first ring pass of this CTA's first
   // tile BEFORE the dependency wait (their HBM / L2 latency overlaps the previous kernel's tail); the A tiles of those
   // stages follow after the wait, on the same full barrier (expect_tx covers the whole stage).
@@ -134,7 +138,7 @@ __global__ void __launch_bounds__(kNumThreads, 1) gemm_bf16x3_kernel(const __gri
     __syncwarp();
   }
   pdl_wait();  // everything above overlapped the previous kernel's tail; activations are touched only below
-  if (trace && threadIdx.x == 0) trace[2] = globaltimer_ns();
+  if (trace && threadIdx.x == 0) args.trace[2] = globaltimer_ns();
 
   if (warp < 4) {
     // ------------------------------------------------------------------ TMA producer (warp 0; warps 1..3 idle)
@@ -196,7 +200,11 @@ __global__ void __launch_bounds__(kNumThreads, 1) gemm_bf16x3_kernel(const __gri
     const int wq = cw & 3;              //      and this warp rows 16 wq + (lane / 4) (+8) of them
     const int quad = cw & 3;            // epilogue: thread = tile row quad * 32 + lane ...
     const int half = cw >> 2;           // ... of column half `half`
-    constexpr int CH = BN / 64;         // 32-column chunks per half
+    // The tile's NCH 32-column chunks go to the two column halves, CH rounds of one chunk per half: half h takes chunks
+    // [h CH, h CH + CH).  At BN = 96 that is chunks 0, 1 for half 0 and chunk 2 for half 1, which sits out the second
+    // round (and still joins every barrier).
+    constexpr int NCH = BN / 32;
+    constexpr int CH = (NCH + 1) / 2;
     const uint32_t smem_u = __shfl_sync(0xffffffffu, smem_u32(smem), 0);
     int stage = 0;
     uint32_t phase = 0;
@@ -232,7 +240,7 @@ __global__ void __launch_bounds__(kNumThreads, 1) gemm_bf16x3_kernel(const __gri
       int prev = -1;
       for (int kb = 0; kb < num_kb; ++kb) {
         mbar_wait(&full_bar[stage], phase);
-        if (trace && kb == 0 && it == 0 && threadIdx.x == 128) trace[3] = globaltimer_ns();
+        if (trace && kb == 0 && it == 0 && threadIdx.x == 128) args.trace[3] = globaltimer_ns();
         const uint32_t sa = smem_u + stage * Cfg::STAGE;
         const uint64_t da_hi = wgmma_desc_sw64_kmajor(sa + wg * (64 * BK * 2));
         const uint64_t db_hi = wgmma_desc_sw64_kmajor(sa + Cfg::B_OFF);
@@ -271,15 +279,16 @@ __global__ void __launch_bounds__(kNumThreads, 1) gemm_bf16x3_kernel(const __gri
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty_bar[prev]);
       }
-      if (trace && it == 0 && threadIdx.x == 128) trace[4] = globaltimer_ns();
+      if (trace && it == 0 && threadIdx.x == 128) args.trace[4] = globaltimer_ns();
 
       float ht_acc[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
       for (int cc = 0; cc < CH; ++cc) {
         if (cc > 0) asm volatile("bar.sync 1, %0;" ::"n"(32 * kEpiWarps) : "memory");   // previous chunk consumed
-        // accumulator fragment -> staging rows: chunk cc of each column half
+        // accumulator fragment -> staging rows: round cc's chunk of each column half
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
+          if (h * CH + cc >= NCH) continue;
           float* dst = sacc + h * (BM * kAccLD);
 #pragma unroll
           for (int ii = 0; ii < 4; ++ii) {
@@ -304,8 +313,8 @@ __global__ void __launch_bounds__(kNumThreads, 1) gemm_bf16x3_kernel(const __gri
         __syncwarp();
         const int c = half * CH + cc;
         const int col0 = nt * BN + c * 32;
-        if (col0 < args.N) {   // warp-uniform
-          const int res_next = (cc + 1 < CH && col0 + 32 < args.N) ? col0 + 32 : -1;
+        if (col0 < args.N && (NCH % 2 == 0 || c < NCH)) {   // warp-uniform
+          const int res_next = (cc + 1 < CH && (NCH % 2 == 0 || c + 1 < NCH) && col0 + 32 < args.N) ? col0 + 32 : -1;
           epi_chunk<EPI, 32>(args, v, sb + c * 32, scs + c * 32, myrows, tg, er, tr, res, col0, res_next, lane, ht_acc);
         }
       }
@@ -323,9 +332,9 @@ __global__ void __launch_bounds__(kNumThreads, 1) gemm_bf16x3_kernel(const __gri
         }
       }
     }
-    if (trace && threadIdx.x == 128) trace[5] = globaltimer_ns();   // epilogue of this CTA's last tile done
+    if (trace && threadIdx.x == 128) args.trace[5] = globaltimer_ns();   // epilogue of this CTA's last tile done
   }
-  if (trace && threadIdx.x == 128) trace[6] = globaltimer_ns();     // exit (the producer warpgroup has no work left)
+  if (trace && threadIdx.x == 128) args.trace[6] = globaltimer_ns();     // exit (the producer warpgroup has no work left)
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -411,9 +420,51 @@ int num_sms() {
   return n;
 }
 
+// Tile shape: 128 x 64, 128 x 96 or 128 x 128, the cheapest under makespan = waves x (bytes staged per k-block), with
+// waves = ceil(tiles / SMs) for the persistent static schedule and 24 / 28 / 32 KB staged per k-block at BN = 64 / 96 / 128
+// (split planes; the one-product ring halves every figure, which keeps the ranking).  Ties go to the wider tile.  A
+// 64-row warpgroup holds a 64 x BN fp32 accumulator in registers next to the epilogue's working set, so 128 is the widest
+// tile; wider requests (force_bn 256, and 2064 / 2128 / 2256, the tile widths of CTA-pair kernels on other architectures)
+// run at the nearest width the kernel has.  col_align (0 = none) is a column no tile may straddle: a_swap's swap_col0,
+// since the producer and the epilogue pick the swapped A group once per tile; a width that does not divide it is never
+// chosen, and rejected when forced.
+int gemm_choose_bn(long long m_tiles, int N, int sms, int col_align, int force_bn) {
+  auto fits = [&](int bn) { return col_align == 0 || col_align % bn == 0; };
+  auto cost = [&](int bn, double kb) {
+    const long long tiles = m_tiles * ((N + bn - 1) / bn);
+    return (double)((tiles + sms - 1) / sms) * kb;
+  };
+  const int fb = force_bn >= 2000 ? force_bn - 2000 : force_bn == 1128 ? 128 : force_bn;
+  if (fb > 0) {
+    if (fb != 64 && fb != 128 && fb != 256 && !(fb == 96 && force_bn == 96)) {
+      set_error("gemm_plan_init: force_bn %d (64, 96, 128, 256, 1128, 2064, 2128, 2256 or 0)", force_bn);
+      return -1;
+    }
+    const int bn = fb > 128 ? 128 : fb;
+    if (!fits(bn)) {
+      set_error("gemm_plan_init: force_bn %d: a %d-wide tile would straddle swap_col0 = %d", force_bn, bn, col_align);
+      return -1;
+    }
+    return bn;
+  }
+  if (col_align % 64 != 0) {
+    set_error("gemm_plan_init: swap_col0 = %d is not a multiple of 64 (no tile width fits it)", col_align);
+    return -1;
+  }
+  int bn = 64;
+  double best = cost(64, 24.0);
+  if (fits(96) && cost(96, 28.0) <= best) {
+    bn = 96;
+    best = cost(96, 28.0);
+  }
+  if (N > 64 && fits(128) && cost(128, 32.0) <= best) bn = 128;
+  return bn;
+}
+
 int gemm_plan_init(GemmPlan* plan, const __nv_bfloat16* a_hi, const __nv_bfloat16* a_lo,
                    const __nv_bfloat16* b_hi, const __nv_bfloat16* b_lo, int groups, int NB, int H, int W, int Kc,
-                   int taps, int N, int force_bn, long long lda, long long ldb, long long b_group_rows, int precision) {
+                   int taps, int N, int force_bn, long long lda, long long ldb, long long b_group_rows, int precision,
+                   int col_align) {
   memset(plan, 0, sizeof(*plan));
   if (precision != GEMM_SPLIT && precision != GEMM_BF16) {
     set_error("gemm_plan_init: precision %d (0 = split bf16, 1 = one bf16 product)", precision);
@@ -437,26 +488,9 @@ int gemm_plan_init(GemmPlan* plan, const __nv_bfloat16* a_hi, const __nv_bfloat1
   a.tiles_w = (W + a.bw - 1) / a.bw;
   a.tiles_h = (H + a.bh - 1) / a.bh;
   a.out_group_rows = (long long)NB * H * W;
-  // Tile shape: 128 x 64 or 128 x 128, the cheaper under makespan = waves x (bytes staged per k-block), with waves =
-  // ceil(tiles / SMs) for the persistent static schedule and 24 KB (128 x 64) / 32 KB (128 x 128) staged per k-block.
-  // A 64-row warpgroup holds a 64 x BN fp32 accumulator in registers next to the epilogue's working set, so 128 is the
-  // widest tile; wider requests (force_bn 256, and 2064 / 2128 / 2256, the tile widths of CTA-pair kernels on other
-  // architectures) run at the nearest width the kernel has.
   const long long m_tiles = (long long)a.tiles_w * a.tiles_h * NB * groups;
-  const int sms = num_sms();
-  auto waves = [](long long tiles, long long slots) { return (double)((tiles + slots - 1) / slots); };
-  const long long nt64 = (N + 63) / 64, nt128 = (N + 127) / 128;
-  const double c64 = waves(m_tiles * nt64, sms) * 24.0;
-  const double c128 = (N > 64) ? waves(m_tiles * nt128, sms) * 32.0 : 1e30;
-  int bn = (c128 <= c64) ? 128 : 64;
-  int fb = force_bn >= 2000 ? force_bn - 2000 : force_bn == 1128 ? 128 : force_bn;
-  if (fb > 0) {
-    if (fb != 64 && fb != 128 && fb != 256) {
-      set_error("gemm_plan_init: force_bn %d (64, 128, 256, 1128, 2064, 2128, 2256 or 0)", force_bn);
-      return -1;
-    }
-    bn = fb > 128 ? 128 : fb;
-  }
+  const int bn = gemm_choose_bn(m_tiles, N, num_sms(), col_align, force_bn);
+  if (bn < 0) return -1;
   plan->bn = bn;
 
   const uint64_t esz = 2;
@@ -518,8 +552,9 @@ static int launch_epi(const GemmPlan& plan, cudaStream_t stream) {
     case EPI_PIXSHUF: return launch_bn<BN, EPI_PIXSHUF, NP>(plan, stream);
     case EPI_QKV: return launch_bn<BN, EPI_QKV, NP>(plan, stream);
     case EPI_HEADTAIL:
-      // the DPT head tail runs in heads(), which is always split; not instantiated at one product (it would spill)
-      if constexpr (NP == 3) return launch_bn<BN, EPI_HEADTAIL, NP>(plan, stream);
+      // the DPT head tail runs in heads(), which is always split; not instantiated at one product (it would spill), nor
+      // at BN = 96 (its hand-over pairs the two column halves; the planner pins it to 128)
+      if constexpr (NP == 3 && BN != 96) return launch_bn<BN, EPI_HEADTAIL, NP>(plan, stream);
       break;
   }
   set_error("gemm_launch: bad epilogue mode %d", plan.args.epi);
@@ -530,6 +565,7 @@ template <int NP>
 static int launch_np(const GemmPlan& plan, cudaStream_t stream) {
   switch (plan.bn) {
     case 64: return launch_epi<64, NP>(plan, stream);
+    case 96: return launch_epi<96, NP>(plan, stream);
     case 128: return launch_epi<128, NP>(plan, stream);
   }
   set_error("gemm_launch: bad bn %d", plan.bn);

@@ -75,7 +75,7 @@ struct GemmArgs {
 struct GemmPlan {
   GemmArgs args;
   dim3 grid;
-  int bn;          // 64 / 128
+  int bn;          // 64 / 96 / 128
   int precision;   // GemmPrecision
   int b_static;    // engine: B is a packed weight and the prefetch option was on when the plan was built
   double flops;    // algorithmic 2*M*N*K (all groups), for roofline accounting
@@ -85,13 +85,18 @@ struct GemmPlan {
 // shape.  Returns 0 or a negative error.
 // lda / ldb: row strides (elements) of A pixels / B rows (0 = dense: Kc resp. taps*Kc);
 // b_group_rows: rows between consecutive groups of B (0 = N).
-// force_bn: 0 = planner's choice; 64 / 128 = that tile width; 256, 1128, 2064, 2128, 2256 = the nearest width the kernel has
-// (128, 128, 64, 128, 128).
+// force_bn: 0 = planner's choice; 64 / 96 / 128 = that tile width; 256, 1128, 2064, 2128, 2256 = the nearest width the
+// kernel has (128, 128, 64, 128, 128).
+// col_align: a_swap's swap_col0 when only the columns from there on are swapped (0 = none): no tile may straddle it.
 int gemm_plan_init(GemmPlan* plan,
                    const __nv_bfloat16* a_hi, const __nv_bfloat16* a_lo,   // [G*NB, H, W, Kc]
                    const __nv_bfloat16* b_hi, const __nv_bfloat16* b_lo,   // [G*N, taps, Kc]
                    int groups, int NB, int H, int W, int Kc, int taps, int N, int force_bn = 0,
-                   long long lda = 0, long long ldb = 0, long long b_group_rows = 0, int precision = GEMM_SPLIT);
+                   long long lda = 0, long long ldb = 0, long long b_group_rows = 0, int precision = GEMM_SPLIT,
+                   int col_align = 0);
+// The planner's tile width for m_tiles 128-row tiles x N columns on `sms` SMs (pure host function; gemm.cu explains the
+// rule).  Returns 64, 96 or 128, or -1 with last_error() set.
+int gemm_choose_bn(long long m_tiles, int N, int sms, int col_align, int force_bn);
 int gemm_launch(const GemmPlan& plan, cudaStream_t stream);
 
 // Tuning knobs of the tile planner / producers (s3r_set_option): read when a plan is BUILT, so two engines of one

@@ -92,7 +92,8 @@ struct EpiRow {
 };
 // Transposed-domain state: lane serves rows rr = it * RPI + lane / LPR, it < NIT (NIT <= 8), four columns each.
 struct EpiTRows {
-  long long key[8];   // PLAIN: global output row; QKV: (gb * heads * ntok + t) * 64; PIXSHUF: h << 32 | w; -1 = no pixel
+  long long key[8];   // PLAIN: global output row; QKV: (gb * heads * ntok + t) * 64; PIXSHUF: global output row of the
+                      // pixel's sub-pixel (0, 0); -1 = no pixel
 };
 
 // Everything that does not need the accumulator; called before the accumulator wait so that its global loads overlap
@@ -164,8 +165,9 @@ __device__ __forceinline__ void epi_tile_pre(const GemmArgs& args, const TileGeo
           const int t = (int)(pix2 - (long long)bidx * args.q_ntok);
           const long long gb = (long long)tg.g * args.q_nb + bidx;
           key = (gb * (args.q_C >> 6) * args.q_ntok + t) * 64;
-        } else {
-          key = ((long long)h2 << 32) | (unsigned int)w2;
+        } else {   // the output row of sub-pixel (0, 0); epi_chunk adds the chunk's (i, j) offset
+          const int s = args.ps_s;
+          key = (long long)tg.g * args.out_group_rows + ((long long)tg.nb * (args.H * s) + h2 * s) * (args.W * s) + w2 * s;
         }
       }
       tr.key[it] = key;
@@ -325,12 +327,7 @@ __device__ __forceinline__ void epi_chunk(const GemmArgs& args, float (&v)[32], 
       } else {
         long long orow = key;
         if constexpr (EPI == EPI_PIXSHUF) {
-          if (key >= 0) {
-            const int s = args.ps_s;
-            const int h = (int)(key >> 32), w = (int)(key & 0xffffffffLL);
-            orow = (long long)tg.g * args.out_group_rows +
-                   ((long long)tg.nb * (args.H * s) + (h * s + ps_i)) * (args.W * s) + (w * s + ps_j);
-          }
+          if (key >= 0) orow = key + (long long)ps_i * (args.W * args.ps_s) + ps_j;
         }
         const bool ok = key >= 0;
         if (ok) {
