@@ -493,6 +493,54 @@ int s3r_engine_profile_read(s3r_engine* e, double* out);
 /* number of kernel launches since the last call; resets the counter */
 long long s3r_engine_take_launches(s3r_engine* e);
 
+/* ---- dataset views (spann3r_b200/views.py): the tail of BaseStereoViewDataset.__getitem__ on the device -----------
+ * dust3r/datasets/base/base_stereo_view_dataset.py:63-194 (crop on the principal point, Lanczos image / nearest depth
+ * rescale, centred crop, ImgNorm, depthmap_to_absolute_camera_coordinates, valid_mask, transpose_to_landscape) for a
+ * sequence of views, one launch per pass.  The host plans every view (crops, index and coefficient tables, final
+ * intrinsics); the descriptor arrays below live in DEVICE memory, one entry per view.
+ *
+ * s3r_views_depth: out pixel (x, y) of the w x h cropped view reads depth[row_src[y] * depth_stride + col_src[x]]
+ * (crop 1, cv2 INTER_NEAREST resize and crop 2 folded into the two index tables) and writes depthmap, pts3d (world,
+ * fp32, [.., 3]) and valid (uint8 0 / 1) at y * w + x, or at x * h + y when `transpose` is set (a portrait view stored
+ * landscape).  intr = (fu, fv, cu, cv), pose = 3x4 row-major [R | t] (NaN for a view without pose).  A non-finite depth
+ * value read sets *nonfinite = 1 (the reference asserts on it).  max_pixels >= every w * h, 1 <= n <= 65535.
+ *
+ * s3r_views_resample_h / s3r_views_resample_v_norm: s3r_resample_h_u8 / s3r_resample_v_u8_norm of every view in one
+ * launch each, bit for bit; img [3, out_rows, cols] fp32, or [3, cols, out_rows] when `transpose` is set.
+ * max_rows / max_out_rows / max_cols bound every view's rows / out_rows / cols, max_span every view's span (see
+ * s3r_resample_h_u8). */
+typedef struct s3r_view_depth_desc {
+  const float* depth;
+  const int32_t* col_src;
+  const int32_t* row_src;
+  float* depthmap;
+  float* pts3d;
+  uint8_t* valid;
+  int32_t* nonfinite;
+  int64_t depth_stride;
+  int32_t w, h, transpose;
+  float intr[4];
+  float pose[12];
+} s3r_view_depth_desc;
+
+typedef struct s3r_view_image_desc {
+  const uint8_t* src;
+  const int32_t* bh;
+  const int32_t* kh;
+  const int32_t* bv;
+  const int32_t* kv;
+  uint8_t* tmp;
+  float* img;
+  int64_t row_stride;
+  int32_t rows, cols, out_rows, ksh, ksv, transpose;
+} s3r_view_image_desc;
+
+/* sizeof the two descriptors (which = 0: depth, 1: image), for the bindings to check their mirrors */
+int s3r_views_abi_sizeof(int which);
+int s3r_views_depth(const s3r_view_depth_desc* descs, int n, int64_t max_pixels, void* stream);
+int s3r_views_resample_h(const s3r_view_image_desc* descs, int n, int max_rows, int max_cols, int max_span, void* stream);
+int s3r_views_resample_v_norm(const s3r_view_image_desc* descs, int n, int max_out_rows, int max_cols, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -113,7 +113,31 @@ _PROTOS = {
     "s3r_attn_train_backward": (_i, [C.POINTER(AttnTrainDesc), _vp, _vp, _vp, _vp, C.c_size_t, _vp, _vp, _vp, _vp]),
     "s3r_resample_h_u8": (_i, [_vp, _i64, _i, _i, _vp, _vp, _i, _i, _vp, _vp]),
     "s3r_resample_v_u8_norm": (_i, [_vp, _i, _i, _vp, _vp, _i, _vp, _vp]),
+    "s3r_views_abi_sizeof": (_i, [_i]),
+    "s3r_views_depth": (_i, [_vp, _i, _i64, _vp]),
+    "s3r_views_resample_h": (_i, [_vp, _i, _i, _i, _i, _vp]),
+    "s3r_views_resample_v_norm": (_i, [_vp, _i, _i, _i, _vp]),
 }
+
+
+class ViewDepthDesc(C.Structure):
+    """Mirror of s3r_view_depth_desc."""
+    _fields_ = [
+        ("depth", _vp), ("col_src", _vp), ("row_src", _vp),
+        ("depthmap", _vp), ("pts3d", _vp), ("valid", _vp), ("nonfinite", _vp),
+        ("depth_stride", _i64), ("w", C.c_int32), ("h", C.c_int32), ("transpose", C.c_int32),
+        ("intr", _f * 4), ("pose", _f * 12),
+    ]
+
+
+class ViewImageDesc(C.Structure):
+    """Mirror of s3r_view_image_desc."""
+    _fields_ = [
+        ("src", _vp), ("bh", _vp), ("kh", _vp), ("bv", _vp), ("kv", _vp), ("tmp", _vp), ("img", _vp),
+        ("row_stride", _i64),
+        ("rows", C.c_int32), ("cols", C.c_int32), ("out_rows", C.c_int32), ("ksh", C.c_int32), ("ksv", C.c_int32),
+        ("transpose", C.c_int32),
+    ]
 
 _lib = None
 

@@ -11,18 +11,11 @@
 #include "kernels.cuh"
 
 #include "common.cuh"
+#include "resample_u8.cuh"
 
 namespace s3r {
 
-constexpr int kPrec = 32 - 8 - 2;   // PRECISION_BITS of Resample.c
-
-__device__ __forceinline__ int clip8(int v) {   // clip8(): (in >> PRECISION_BITS) clamped to [0, 255]
-  v >>= kPrec;
-  return v < 0 ? 0 : (v > 255 ? 255 : v);
-}
-
-// Horizontal pass.  Block = one source row x 128 output columns; the source span those columns need is staged in
-// shared memory with coalesced byte loads, then thread t computes output column x0 + t (3 channels).
+// Horizontal pass.  Block = one source row x 128 output columns (resample_u8.cuh).
 // src: RGB rows of `row_stride` bytes, first needed row / column already applied by the caller through the pointer and
 // the bounds; bounds[x] = (first source column, tap count), kk[x][ksize] fixed-point taps.
 __global__ void __launch_bounds__(128) resample_h_u8_kernel(const uint8_t* __restrict__ src, long long row_stride,
@@ -33,35 +26,12 @@ __global__ void __launch_bounds__(128) resample_h_u8_kernel(const uint8_t* __res
   pdl_wait();
   extern __shared__ uint8_t span[];
   const int row = blockIdx.y;
-  const int x0 = blockIdx.x * 128;
-  const int xl = min(x0 + 127, out_cols - 1);
-  const int s0 = bounds[2 * x0];                                  // first source column of the block's span
-  const int s1 = bounds[2 * xl] + bounds[2 * xl + 1];             // one past the last
-  const uint8_t* srow = src + (long long)row * row_stride + 3LL * s0;
-  const int nbytes = 3 * (s1 - s0);
-  for (int i = threadIdx.x; i < nbytes; i += 128) span[i] = srow[i];
-  __syncthreads();
-  const int x = x0 + threadIdx.x;
-  if (x >= out_cols) return;
-  const int b0 = bounds[2 * x] - s0, n = bounds[2 * x + 1];
-  const int* k = kk + (long long)x * ksize;
-  int a0 = 1 << (kPrec - 1), a1 = a0, a2 = a0;
-  for (int i = 0; i < n; ++i) {
-    const int c = __ldg(k + i);
-    const uint8_t* p = span + 3 * (b0 + i);
-    a0 += p[0] * c;
-    a1 += p[1] * c;
-    a2 += p[2] * c;
-  }
-  uint8_t* o = dst + ((long long)row * out_cols + x) * 3;
-  o[0] = (uint8_t)clip8(a0);
-  o[1] = (uint8_t)clip8(a1);
-  o[2] = (uint8_t)clip8(a2);
+  resample_h_u8_block(src + (long long)row * row_stride, out_cols, blockIdx.x * 128, bounds, kk, ksize, span,
+                      dst + (long long)row * out_cols * 3);
 }
 
 // Vertical pass + ToTensor + Normalize: thread = one byte column of the intermediate (x * 3 + c, coalesced across the
-// warp), loops over the output rows of its block.  dst [3, out_rows, cols] fp32 = ((v / 255) - 0.5) / 0.5 in fp32, the
-// operation order of torchvision's ToTensor / Normalize.
+// warp), block row = one output row.  dst [3, out_rows, cols] fp32.
 __global__ void __launch_bounds__(256) resample_v_u8_norm_kernel(const uint8_t* __restrict__ tmp, int cols,
                                                                  int out_rows, const int* __restrict__ bounds,
                                                                  const int* __restrict__ kk, int ksize,
@@ -72,13 +42,7 @@ __global__ void __launch_bounds__(256) resample_v_u8_norm_kernel(const uint8_t* 
   if (j >= cols * 3) return;
   const int x = j / 3, c = j - 3 * x;
   const int y = blockIdx.y;
-  const int y0 = bounds[2 * y], n = bounds[2 * y + 1];
-  const int* k = kk + (long long)y * ksize;
-  const uint8_t* p = tmp + (long long)y0 * cols * 3 + j;
-  int a = 1 << (kPrec - 1);
-  for (int i = 0; i < n; ++i) a += (int)p[(long long)i * cols * 3] * __ldg(k + i);
-  const float v = (float)clip8(a) / 255.0f;
-  dst[((long long)c * out_rows + y) * cols + x] = (v - 0.5f) / 0.5f;
+  dst[((long long)c * out_rows + y) * cols + x] = resample_v_u8_norm_value(tmp, cols, j, y, bounds, kk, ksize);
 }
 
 int launch_resample_h_u8(const uint8_t* src, long long row_stride, int rows, int out_cols, const int* bounds,

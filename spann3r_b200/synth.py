@@ -29,6 +29,7 @@ import os
 import re
 import zlib
 
+import numpy as np
 import torch
 
 _SPEC_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "state_dict_spec.json")
@@ -361,3 +362,118 @@ LOSS_CASES = {
     "even_pts": {"criterion": "Regr3D_t_ScaleShiftInv(L21, gt_scale=False)", "call": "pts",
                  "data": {"batch": 2, "frames": 3, "height": 32, "width": 48, "invalid": 0.0, "seed": 8}},
 }
+
+
+# ---- dataset views (spann3r_b200/views.py): golden cases of tests/golden/views.json (tools/make_golden_views.py),
+# regenerated from their parameters by the tests, and a 7Scenes-layout scene on disk for the loader tests / benchmark
+
+_SEVEN_K = (525.0, 525.0, 320.0, 240.0)
+
+VIEW_CASES = [  # name, h, w, (fx, fy, cx, cy), views, resolution, aug_crop, item seed, depth kind, pose kind
+    dict(name="7scenes_224", h=480, w=640, K=_SEVEN_K, views=3, res=(224, 224), aug=0, seed=1, depth="std", pose="random"),
+    dict(name="7scenes_512", h=480, w=640, K=_SEVEN_K, views=2, res=(512, 384), aug=0, seed=2, depth="std", pose="random"),
+    dict(name="dtu_512", h=1200, w=1600, K=(2892.33, 2883.18, 823.205, 619.071), views=1, res=(512, 384), aug=0, seed=3,
+         depth="std", pose="random"),
+    dict(name="offcentre_224", h=480, w=640, K=(530.5, 529.25, 301.5, 254.5), views=2, res=(224, 224), aug=0, seed=4,
+         depth="std", pose="random"),
+    dict(name="portrait_512", h=640, w=480, K=(500.0, 500.0, 240.0, 320.0), views=2, res=(512, 384), aug=0, seed=5,
+         depth="std", pose="random"),
+    dict(name="portrait_224", h=640, w=480, K=(500.0, 500.0, 241.0, 318.0), views=1, res=(224, 224), aug=0, seed=6,
+         depth="std", pose="random"),
+    dict(name="square_512", h=600, w=600, K=(600.0, 600.0, 300.0, 300.0), views=4, res=(512, 384), aug=0, seed=14,
+         depth="std", pose="random"),
+    dict(name="aug16_a", h=480, w=640, K=_SEVEN_K, views=2, res=(224, 224), aug=16, seed=8, depth="std", pose="random"),
+    dict(name="aug16_b", h=480, w=640, K=_SEVEN_K, views=2, res=(224, 224), aug=16, seed=9, depth="std", pose="random"),
+    dict(name="aug16_c", h=480, w=640, K=_SEVEN_K, views=2, res=(512, 384), aug=16, seed=10, depth="std", pose="random"),
+    dict(name="extreme_depth", h=480, w=640, K=(150.0, 150.0, 320.0, 240.0), views=1, res=(224, 224), aug=0, seed=11,
+         depth="extreme", pose="identity"),
+    dict(name="no_pose", h=480, w=640, K=_SEVEN_K, views=1, res=(224, 224), aug=0, seed=12, depth="std", pose="none"),
+]
+
+
+def _random_rotation(g) -> np.ndarray:
+    q = g.standard_normal(4)
+    a, b, c, d = q / np.linalg.norm(q)
+    return np.array([[a * a + b * b - c * c - d * d, 2 * (b * c - a * d), 2 * (b * d + a * c)],
+                     [2 * (b * c + a * d), a * a - b * b + c * c - d * d, 2 * (c * d - a * b)],
+                     [2 * (b * d - a * c), 2 * (c * d + a * b), a * a - b * b - c * c + d * d]])
+
+
+def make_view_case(case) -> list:
+    """Deterministic [(rgb uint8, depth float32, K float32, pose float32 4x4 or None)] of a VIEW_CASES entry."""
+    g = np.random.default_rng(1000 + case["seed"])
+    fx, fy, cx, cy = case["K"]
+    K = np.array([[fx, 0, cx], [0, fy, cy], [0, 0, 1]], dtype=np.float32)
+    h, w = case["h"], case["w"]
+    out = []
+    for _ in range(case["views"]):
+        rgb = g.integers(0, 256, (h, w, 3), dtype=np.uint8)
+        depth = g.uniform(0.3, 6.0, (h, w)).astype(np.float32)
+        depth[g.random((h, w)) < 0.1] = 0.0
+        if case["depth"] == "extreme":
+            depth[g.random((h, w)) < 0.2] = np.float32(3.0e38)
+        if case["pose"] == "random":
+            pose = np.eye(4)
+            pose[:3, :3] = _random_rotation(g)
+            pose[:3, 3] = g.uniform(-2.0, 2.0, 3)
+            pose = pose.astype(np.float32)
+        elif case["pose"] == "identity":
+            pose = np.eye(4, dtype=np.float32)
+        else:
+            pose = None
+        out.append((rgb, depth, K, pose))
+    return out
+
+
+def write_7scenes_sequence(root: str, frames: int = 6, seed: int = 0):
+    """A 7Scenes-layout sequence in `root`: frame-XXXXXX.color.png (RGB 640x480, part gradient, part noise),
+    .depth.proj.png (uint16 mm, 65535 = missing) and .pose.txt (cam-to-world 4x4).  PNG decodes identically across
+    library versions."""
+    import cv2
+    g = np.random.default_rng(seed)
+    os.makedirs(root, exist_ok=True)
+    yy, xx = np.mgrid[0:480, 0:640]
+    for i in range(frames):
+        rgb = np.stack([(xx * (i + 1) // 7) % 256, (yy * 3 + 40 * i) % 256, g.integers(0, 256, (480, 640))], -1)
+        cv2.imwrite(os.path.join(root, f"frame-{i:06d}.color.png"), rgb.astype(np.uint8)[..., ::-1])
+        depth = g.integers(300, 6000, (480, 640)).astype(np.uint16)
+        depth[g.random((480, 640)) < 0.05] = 65535
+        depth[g.random((480, 640)) < 0.05] = 0
+        cv2.imwrite(os.path.join(root, f"frame-{i:06d}.depth.proj.png"), depth)
+        pose = np.eye(4)
+        pose[:3, :3] = _random_rotation(g)
+        pose[:3, 3] = g.uniform(-1, 1, 3)
+        np.savetxt(os.path.join(root, f"frame-{i:06d}.pose.txt"), pose)
+
+
+class SevenScenesLike:
+    """Duck-typed stand-in for the reference's SevenScenes(full_video=True, kf_every=...) over a sequence written by
+    write_7scenes_sequence: the same decoding and depth clean-up (spann3r/datasets/seven_scenes.py:87-143), then
+    `_crop_resize_if_necessary` per frame, with ImgNorm as transform."""
+
+    def __init__(self, root: str, resolution=224, kf_every: int = 2, seed: int = 7, aug_crop=0):
+        import torchvision.transforms as tvf
+        self.ROOT, self.kf_every, self.seed, self.aug_crop = root, kf_every, seed, aug_crop
+        self._resolutions = [(resolution, resolution) if isinstance(resolution, int) else tuple(resolution)]
+        self.transform = tvf.Compose([tvf.ToTensor(), tvf.Normalize((0.5, 0.5, 0.5), (0.5, 0.5, 0.5))])
+
+    def __len__(self):
+        return 1
+
+    def _get_views(self, idx, resolution, rng):
+        import cv2
+        n = len([f for f in os.listdir(self.ROOT) if "color" in f])
+        K = np.array([[525, 0, 320], [0, 525, 240], [0, 0, 1]], dtype=np.float32)
+        views = []
+        for im_idx in [f"{i:06d}" for i in range(n)][::self.kf_every]:
+            rgb = cv2.cvtColor(cv2.imread(os.path.join(self.ROOT, f"frame-{im_idx}.color.png")), cv2.COLOR_BGR2RGB)
+            depth = cv2.imread(os.path.join(self.ROOT, f"frame-{im_idx}.depth.proj.png"), cv2.IMREAD_UNCHANGED)
+            depth[depth == 65535] = 0
+            depth = np.nan_to_num(depth.astype(np.float32), 0.0) / 1000.0
+            depth[depth > 10] = 0
+            depth[depth < 1e-3] = 0
+            pose = np.loadtxt(os.path.join(self.ROOT, f"frame-{im_idx}.pose.txt")).astype(np.float32)
+            rgb, depth, Kf = self._crop_resize_if_necessary(rgb, depth, K, resolution, rng=rng, info=im_idx)
+            views.append(dict(img=rgb, depthmap=depth, camera_pose=pose, camera_intrinsics=Kf, dataset="7scenes",
+                              label=im_idx, instance=im_idx))
+        return views
