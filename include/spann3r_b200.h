@@ -535,11 +535,36 @@ typedef struct s3r_view_image_desc {
   int32_t rows, cols, out_rows, ksh, ksv, transpose;
 } s3r_view_image_desc;
 
-/* sizeof the two descriptors (which = 0: depth, 1: image), for the bindings to check their mirrors */
+/* sizeof the view descriptors (which = 0: depth, 1: image, 2: s3r_view_jitter_desc below), for the bindings to check
+ * their mirrors */
 int s3r_views_abi_sizeof(int which);
 int s3r_views_depth(const s3r_view_depth_desc* descs, int n, int64_t max_pixels, void* stream);
 int s3r_views_resample_h(const s3r_view_image_desc* descs, int n, int max_rows, int max_cols, int max_span, void* stream);
 int s3r_views_resample_v_norm(const s3r_view_image_desc* descs, int n, int max_out_rows, int max_cols, void* stream);
+
+/* ---- training views: torchvision's ColorJitter (PIL path) before ImgNorm, bit for bit (spann3r_b200/train_views.py) --
+ * s3r_views_resample_v_u8: the vertical pass of s3r_views_resample_v_norm without ImgNorm: view v's uint8 image
+ * [out_rows, cols, 3] (before any transpose) goes to jit[v].u8.  descs / jit: device arrays of n entries each.
+ *
+ * s3r_views_color_jitter: one CTA per view.  Applies the view's ops in `order` (0 brightness, 1 contrast, 2 saturation,
+ * 3 hue; bit k of `skip` set: op k's factor was None and it is not applied) to u8 [rows, cols, 3], with Pillow's rules
+ * (csrc/jitter_math.cuh): brightness / contrast / saturation are Image.blend toward black / the image's mean L / each
+ * pixel's L with the fp32 factor, hue adds `hue_shift` (= (int32) trunc(hue_factor * 255)) to the uint8 HSV hue mod 256.
+ * Then ImgNorm, writing img [3, rows, cols] fp32, or [3, cols, rows] when `transpose` is set.  The contrast mean is an
+ * exact integer reduction.  max_pixels >= every rows * cols.  u8 is only read. */
+typedef struct s3r_view_jitter_desc {
+  uint8_t* u8;
+  float* img;
+  int32_t rows, cols, transpose;
+  int32_t order[4];
+  int32_t skip;
+  float brightness, contrast, saturation;
+  int32_t hue_shift;
+} s3r_view_jitter_desc;
+
+int s3r_views_resample_v_u8(const s3r_view_image_desc* descs, const s3r_view_jitter_desc* jit, int n, int max_out_rows,
+                            int max_cols, void* stream);
+int s3r_views_color_jitter(const s3r_view_jitter_desc* jit, int n, int64_t max_pixels, void* stream);
 
 #ifdef __cplusplus
 }

@@ -117,6 +117,8 @@ _PROTOS = {
     "s3r_views_depth": (_i, [_vp, _i, _i64, _vp]),
     "s3r_views_resample_h": (_i, [_vp, _i, _i, _i, _i, _vp]),
     "s3r_views_resample_v_norm": (_i, [_vp, _i, _i, _i, _vp]),
+    "s3r_views_resample_v_u8": (_i, [_vp, _vp, _i, _i, _i, _vp]),
+    "s3r_views_color_jitter": (_i, [_vp, _i, _i64, _vp]),
 }
 
 
@@ -137,6 +139,15 @@ class ViewImageDesc(C.Structure):
         ("row_stride", _i64),
         ("rows", C.c_int32), ("cols", C.c_int32), ("out_rows", C.c_int32), ("ksh", C.c_int32), ("ksv", C.c_int32),
         ("transpose", C.c_int32),
+    ]
+
+
+class ViewJitterDesc(C.Structure):
+    """Mirror of s3r_view_jitter_desc."""
+    _fields_ = [
+        ("u8", _vp), ("img", _vp),
+        ("rows", C.c_int32), ("cols", C.c_int32), ("transpose", C.c_int32), ("order", C.c_int32 * 4),
+        ("skip", C.c_int32), ("brightness", _f), ("contrast", _f), ("saturation", _f), ("hue_shift", C.c_int32),
     ]
 
 _lib = None

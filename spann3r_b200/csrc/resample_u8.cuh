@@ -45,18 +45,30 @@ __device__ __forceinline__ void resample_h_u8_block(const uint8_t* __restrict__ 
   o[2] = (uint8_t)clip8(a2);
 }
 
-// Vertical pass + ToTensor + Normalize of one byte column j (= x * 3 + c) of output row y of the uint8 intermediate
-// tmp [*, cols, 3]: ((v / 255) - 0.5) / 0.5 in fp32, the operation order of torchvision's ToTensor / Normalize.
-__device__ __forceinline__ float resample_v_u8_norm_value(const uint8_t* __restrict__ tmp, int cols, int j, int y,
-                                                          const int* __restrict__ bounds, const int* __restrict__ kk,
-                                                          int ksize) {
+// Vertical pass of one byte column j (= x * 3 + c) of output row y of the uint8 intermediate tmp [*, cols, 3]: the
+// uint8 value of the resized image.
+__device__ __forceinline__ int resample_v_u8_value(const uint8_t* __restrict__ tmp, int cols, int j, int y,
+                                                   const int* __restrict__ bounds, const int* __restrict__ kk, int ksize) {
   const int y0 = bounds[2 * y], n = bounds[2 * y + 1];
   const int* k = kk + (long long)y * ksize;
   const uint8_t* p = tmp + (long long)y0 * cols * 3 + j;
   int a = 1 << (kPrec - 1);
   for (int i = 0; i < n; ++i) a += (int)p[(long long)i * cols * 3] * __ldg(k + i);
-  const float v = (float)clip8(a) / 255.0f;
-  return (v - 0.5f) / 0.5f;
+  return clip8(a);
+}
+
+// ImgNorm (ToTensor + Normalize((0.5,) * 3, (0.5,) * 3)) of one uint8 value: ((v / 255) - 0.5) / 0.5 in fp32, the
+// operation order of torchvision's ToTensor / Normalize.
+__device__ __forceinline__ float img_norm_u8(int v) {
+  const float f = (float)v / 255.0f;
+  return (f - 0.5f) / 0.5f;
+}
+
+// Vertical pass + ImgNorm of one byte column j of output row y.
+__device__ __forceinline__ float resample_v_u8_norm_value(const uint8_t* __restrict__ tmp, int cols, int j, int y,
+                                                          const int* __restrict__ bounds, const int* __restrict__ kk,
+                                                          int ksize) {
+  return img_norm_u8(resample_v_u8_value(tmp, cols, j, y, bounds, kk, ksize));
 }
 
 }  // namespace s3r

@@ -80,6 +80,7 @@ int s3r_views_abi_sizeof(int which) {
   switch (which) {
     case 0: return (int)sizeof(s3r_view_depth_desc);
     case 1: return (int)sizeof(s3r_view_image_desc);
+    case 2: return (int)sizeof(s3r_view_jitter_desc);
   }
   return -1;
 }

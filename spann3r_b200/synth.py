@@ -477,3 +477,350 @@ class SevenScenesLike:
             views.append(dict(img=rgb, depthmap=depth, camera_pose=pose, camera_intrinsics=Kf, dataset="7scenes",
                               label=im_idx, instance=im_idx))
         return views
+
+
+def write_co3d_tree(root: str, frames: int = 10, width: int = 320, height: int = 240, seed: int = 0,
+                    zero_frames=(3,), category: str = "apple", instance: str = "110_13051_23361"):
+    """A tree in the layout of the reference's preprocessed Co3d (spann3r/datasets/co3d.py): selected_seqs_train.json,
+    <cat>/<inst>/images/frameNNNNNN.jpg (+ .npz with camera_pose, camera_intrinsics, maximum_depth),
+    depths/frameNNNNNN.jpg.geometric.png (uint16, depth / maximum_depth * 65535) and masks/frameNNNNNN.png (uint8).
+    Frames in `zero_frames` have an all-zero depth map, so the dataset's invalidate / retry path fires on them.
+    Principal points wander around the centre; some frames are portrait crops."""
+    import cv2
+    g = np.random.default_rng(seed)
+    base = os.path.join(root, category, instance)
+    for sub in ("images", "depths", "masks"):
+        os.makedirs(os.path.join(base, sub), exist_ok=True)
+    yy, xx = np.mgrid[0:height, 0:width]
+    ids = list(range(1, frames + 1))
+    for k, fid in enumerate(ids):
+        rgb = np.stack([(xx * (k + 2) // 5 + yy) % 256, (yy * 3 + 25 * k) % 256, g.integers(0, 256, (height, width))], -1)
+        name = f"frame{fid:06d}"
+        cv2.imwrite(os.path.join(base, "images", name + ".jpg"), rgb.astype(np.uint8)[..., ::-1])
+        maxd = np.float32(g.uniform(4.0, 6.0))
+        depth = g.integers(2000, 65535, (height, width)).astype(np.uint16)
+        depth[g.random((height, width)) < 0.1] = 0
+        if k in zero_frames:
+            depth[:] = 0
+        cv2.imwrite(os.path.join(base, "depths", name + ".jpg.geometric.png"), depth)
+        mask = np.where(g.random((height, width)) < 0.8, 255, g.integers(0, 40, (height, width))).astype(np.uint8)
+        cv2.imwrite(os.path.join(base, "masks", name + ".png"), mask)
+        f = g.uniform(0.8, 1.2) * width
+        cx, cy = width / 2 + g.uniform(-8, 8), height / 2 + g.uniform(-8, 8)
+        if k % 4 == 1:                      # a portrait crop: the principal point near a side
+            cx = width * 0.3
+        K = np.array([[f, 0, cx], [0, f, cy], [0, 0, 1]], dtype=np.float32)
+        pose = np.eye(4, dtype=np.float32)
+        pose[:3, :3] = _random_rotation(g)
+        pose[:3, 3] = g.uniform(-1, 1, 3)
+        np.savez(os.path.join(base, "images", name + ".npz"), camera_pose=pose, camera_intrinsics=K, maximum_depth=maxd)
+    with open(os.path.join(root, "selected_seqs_train.json"), "w") as fh:
+        json.dump({category: {instance: ids}, "empty": {}}, fh)
+
+
+def _imread_rgb(path, flags=None):
+    import cv2
+    img = cv2.imread(path, cv2.IMREAD_COLOR if flags is None else flags)
+    if img is None:
+        raise IOError(f"could not load image {path}")
+    return cv2.cvtColor(img, cv2.COLOR_BGR2RGB) if img.ndim == 3 else img
+
+
+class _ManyViewLike:
+    """What the duck-typed training sets below share with the reference's BaseManyViewDataset: the base options, the
+    transform (ImgNorm or the reference's Compose([ColorJitter(0.5, 0.5, 0.5, 0.1), ImgNorm])) and sample_frames.
+    `_crop_resize_if_necessary` comes from whoever builds the views (TrainViews, or the oracle)."""
+
+    def __init__(self, ROOT, resolution, num_frames, jitter, seed, min_thresh, max_thresh, num_seq, aug_crop, split):
+        import torchvision.transforms as tvf
+        self.ROOT, self.split, self.num_frames, self.seed = ROOT, split, num_frames, seed
+        self.min_thresh, self.max_thresh, self.num_seq, self.aug_crop = min_thresh, max_thresh, num_seq, aug_crop
+        self.train_ratio = 0.5
+        self._resolutions = [(resolution, resolution) if isinstance(resolution, int) else tuple(resolution)]
+        norm = tvf.Compose([tvf.ToTensor(), tvf.Normalize((0.5, 0.5, 0.5), (0.5, 0.5, 0.5))])
+        self.transform = tvf.Compose([tvf.ColorJitter(0.5, 0.5, 0.5, 0.1), norm]) if jitter else norm
+
+    def __len__(self):
+        return len(self.scene_list) * self.num_seq
+
+    def sample_frames(self, img_idxs, rng):
+        n = self.num_frames
+        thresh = int(self.min_thresh + self.train_ratio * (self.max_thresh - self.min_thresh))
+        pool = list(range(len(img_idxs)))
+        first_span = max(len(pool) // n, len(pool) - thresh * (n - 1))
+        cur = rng.choice(pool[:first_span])
+        chosen = [cur]
+        while len(chosen) < n:
+            hi = min(cur + thresh, len(pool) - (n - len(chosen)))
+            cand = [i for i in range(cur + 1, hi + 1) if i not in chosen]
+            if not cand:
+                break
+            cur = rng.choice(cand)
+            chosen.append(cur)
+        if len(chosen) < n:
+            return self.sample_frames(img_idxs, rng)
+        out = [img_idxs[i] for i in chosen]
+        if rng.choice([True, False]):
+            out.reverse()
+        return out
+
+
+class Co3dLike(_ManyViewLike):
+    """Duck-typed stand-in for the reference's training Co3d(use_comb=False, ...) (spann3r/datasets/co3d.py with
+    BaseManyViewDataset.sample_frames) over a tree written by write_co3d_tree, for tests that cannot import the
+    reference: the same frame sampling, background masking, invalidate / retry loop and depth-range resampling, with
+    the same numpy RNG draws."""
+
+    def __init__(self, ROOT, resolution=224, num_frames=3, mask_bg="rand", jitter=True, seed=None, min_thresh=2,
+                 max_thresh=5, num_seq=20, aug_crop=0, split="train"):
+        super().__init__(ROOT, resolution, num_frames, jitter, seed, min_thresh, max_thresh, num_seq, aug_crop, split)
+        self.mask_bg = mask_bg
+        with open(os.path.join(ROOT, f"selected_seqs_{split}.json")) as fh:
+            seqs = json.load(fh)
+        self.scenes = {(c, i): v for c, insts in seqs.items() if len(insts) > 0 for i, v in insts.items()}
+        self.scene_list = list(self.scenes)
+        self.invalidate = {s: {} for s in self.scene_list}
+
+    def _get_views(self, idx, resolution, rng):
+        import cv2
+        from collections import deque
+        obj, inst = self.scene_list[idx // self.num_seq]
+        pool = self.scenes[obj, inst]
+        order = self.sample_frames(range(0, len(pool)), rng)
+        bad = self.invalidate[obj, inst].setdefault(resolution, [False] * len(pool))
+        mask_bg = (self.mask_bg is True) or (self.mask_bg == "rand" and rng.choice(2))
+        queue = deque(order)
+        dmin, dmax, dfirst = 1e8, 0.0, None
+        views = []
+        while queue:
+            im = queue.popleft()
+            if bad[im]:
+                step = 2 * rng.choice(2) - 1
+                for off in range(1, len(pool)):
+                    alt = (im + step * off) % len(pool)
+                    if not bad[alt]:
+                        im = alt
+                        break
+            path = os.path.join(self.ROOT, obj, inst, "images", f"frame{pool[im]:06d}.jpg")
+            meta = np.load(path.replace("jpg", "npz"))
+            pose = meta["camera_pose"].astype(np.float32)
+            K = meta["camera_intrinsics"].astype(np.float32)
+            rgb = _imread_rgb(path)
+            depth = _imread_rgb(path.replace("images", "depths") + ".geometric.png", cv2.IMREAD_UNCHANGED)
+            depth = (depth.astype(np.float32) / 65535) * np.nan_to_num(meta["maximum_depth"])
+            if mask_bg:
+                m = _imread_rgb(os.path.join(self.ROOT, obj, inst, "masks", f"frame{pool[im]:06d}.png"),
+                                cv2.IMREAD_UNCHANGED).astype(np.float32)
+                depth *= (m / 255.0) > 0.1
+            rgb, depth, K = self._crop_resize_if_necessary(rgb, depth, K, resolution, rng=rng, info=path)
+            if (depth > 0.0).sum() == 0:
+                bad[im] = True
+                queue.appendleft(im)
+                continue
+            md = meta["maximum_depth"]
+            if md > dmax:
+                dmax = md
+            if md < dmin:
+                dmin = md
+            if dfirst is None:
+                dfirst = md
+            views.append(dict(img=rgb, depthmap=depth, camera_pose=pose, camera_intrinsics=K, dataset="Co3d_v2",
+                              label=os.path.join(obj, inst), instance=os.path.split(path)[1]))
+        if dmax / dmin > 100.0 or dmax / dfirst > 10.0:
+            return self._get_views(rng.integers(0, len(self) - 1), resolution, rng)
+        return views
+
+
+def _scene_frames(g, k, width, height, zero):
+    """One synthetic frame: RGB (part gradient, part noise), depth in metres (10 % holes; all zero when `zero`)."""
+    yy, xx = np.mgrid[0:height, 0:width]
+    rgb = np.stack([(xx * (k + 3) // 4 + 2 * yy) % 256, (yy * 5 + 31 * k) % 256, g.integers(0, 256, (height, width))], -1)
+    depth = g.uniform(0.5, 4.0, (height, width)).astype(np.float32)
+    depth[g.random((height, width)) < 0.1] = 0
+    if zero:
+        depth[:] = 0
+    return rgb.astype(np.uint8), depth
+
+
+def write_scannetpp_tree(root: str, frames: int = 10, width: int = 320, height: int = 240, seed: int = 0,
+                         zero_frames=(3,), scene: str = "0a5c013435"):
+    """A tree in the layout of the reference's preprocessed ScanNet++ (spann3r/datasets/scannetpp.py):
+    splits/nvs_sem_train.txt, data/<scene>/dslr/nerfstudio/transforms_undistorted.json (fl_x, fl_y, cx, cy and a
+    cam-to-world OpenGL `transform_matrix` per frame), dslr/train_test_lists.json, dslr/undistorted_images/*.JPG and
+    dslr/undistorted_depths/*.png (uint16 mm).  Frames in `zero_frames` have an all-zero depth map, so the dataset's
+    recursive retry fires on them."""
+    import cv2
+    g = np.random.default_rng(seed)
+    base = os.path.join(root, "data", scene, "dslr")
+    for sub in ("nerfstudio", "undistorted_images", "undistorted_depths"):
+        os.makedirs(os.path.join(base, sub), exist_ok=True)
+    os.makedirs(os.path.join(root, "splits"), exist_ok=True)
+    names, metas = [], []
+    for k in range(frames):
+        name = f"DSC{k + 1:05d}.JPG"
+        rgb, depth = _scene_frames(g, k, width, height, k in zero_frames)
+        cv2.imwrite(os.path.join(base, "undistorted_images", name), rgb[..., ::-1])
+        cv2.imwrite(os.path.join(base, "undistorted_depths", name.replace(".JPG", ".png")),
+                    np.round(depth * 1000).astype(np.uint16))
+        pose = np.eye(4)
+        pose[:3, :3] = _random_rotation(g)
+        pose[:3, 3] = g.uniform(-1, 1, 3)
+        names.append(name)
+        metas.append({"file_path": name, "transform_matrix": pose.tolist()})
+    f = float(g.uniform(0.8, 1.2) * width)
+    cams = {"fl_x": f, "fl_y": f * 1.01, "cx": width / 2 + 3.3, "cy": height / 2 - 2.6, "frames": metas[::-1]}
+    with open(os.path.join(base, "nerfstudio", "transforms_undistorted.json"), "w") as fh:
+        json.dump(cams, fh)
+    with open(os.path.join(base, "train_test_lists.json"), "w") as fh:
+        json.dump({"train": names[::-1], "test": []}, fh)
+    with open(os.path.join(root, "splits", "nvs_sem_train.txt"), "w") as fh:
+        fh.write(scene + "\n")
+
+
+class ScannetppLike(_ManyViewLike):
+    """Duck-typed stand-in for the reference's training Scannetpp (spann3r/datasets/scannetpp.py) over a tree written
+    by write_scannetpp_tree: the same frame sampling and the same recursive retry (`attempts`) on a frame without valid
+    depth, with the same numpy RNG draws."""
+
+    def __init__(self, ROOT, resolution=224, num_frames=3, jitter=True, seed=None, min_thresh=2, max_thresh=5,
+                 num_seq=20, aug_crop=0, split="train"):
+        super().__init__(ROOT, resolution, num_frames, jitter, seed, min_thresh, max_thresh, num_seq, aug_crop, split)
+        with open(os.path.join(ROOT, "splits", f"nvs_sem_{split}.txt")) as fh:
+            self.scene_list = fh.read().splitlines()
+
+    def _get_views(self, idx, resolution, rng, attempts=0):
+        import cv2
+        scene = self.scene_list[idx // self.num_seq]
+        base = os.path.join(self.ROOT, "data", scene, "dslr")
+        with open(os.path.join(base, "nerfstudio", "transforms_undistorted.json")) as fh:
+            cams = json.load(fh)
+        with open(os.path.join(base, "train_test_lists.json")) as fh:
+            order = self.sample_frames(sorted(json.load(fh)["train"]), rng)
+        by_path = {fr["file_path"]: i for i, fr in enumerate(cams["frames"])}
+        K = np.array([[cams["fl_x"], 0, cams["cx"]], [0, cams["fl_y"], cams["cy"]], [0, 0, 1]], dtype=np.float32)
+        views = []
+        for name in order:
+            path = os.path.join(base, "undistorted_images", name)
+            rgb = _imread_rgb(path)
+            depth = _imread_rgb(os.path.join(base, "undistorted_depths", name.replace(".JPG", ".png")),
+                                cv2.IMREAD_UNCHANGED)
+            depth = np.nan_to_num(depth.astype(np.float32), 0.0) / 1000.0
+            pose = np.array(cams["frames"][by_path[name]]["transform_matrix"], dtype=np.float32)
+            pose[:, 1:3] *= -1.0
+            rgb, depth, Kf = self._crop_resize_if_necessary(rgb, depth, K, resolution, rng=rng, info=path)
+            if (depth > 0.0).sum() == 0 or not np.isfinite(pose).all():
+                if attempts >= 5:
+                    return self._get_views(rng.integers(0, len(self) - 1), resolution, rng)
+                return self._get_views(idx, resolution, rng, attempts + 1)
+            views.append(dict(img=rgb, depthmap=depth, camera_pose=pose, camera_intrinsics=Kf, dataset="scannetpp",
+                              label=os.path.join(scene, name), instance=os.path.split(path)[1]))
+        return views
+
+
+def write_blendmvs_tree(root: str, frames: int = 10, width: int = 320, height: int = 256, seed: int = 0,
+                        zero_frames=(3,), scene: str = "5a3ca9cb270f0e3f14d0eddb"):
+    """A tree in the layout of the reference's BlendedMVS (spann3r/datasets/blendedmvs.py): train_list.txt,
+    <scene>/blended_images/NNNNNNNN.jpg, rendered_depth_maps/NNNNNNNN.pfm (float32), cams/NNNNNNNN_cam.txt (MVSNet
+    text: world-to-cam extrinsic, intrinsic) and cams/pair.txt (MVSNet view clusters).  Frames in `zero_frames` have an
+    all-zero depth map, so the dataset's recursive retry fires on them."""
+    import cv2
+    g = np.random.default_rng(seed)
+    base = os.path.join(root, scene)
+    for sub in ("blended_images", "rendered_depth_maps", "cams"):
+        os.makedirs(os.path.join(base, sub), exist_ok=True)
+    for k in range(frames):
+        rgb, depth = _scene_frames(g, k, width, height, k in zero_frames)
+        cv2.imwrite(os.path.join(base, "blended_images", f"{k:08d}.jpg"), rgb[..., ::-1])
+        cv2.imwrite(os.path.join(base, "rendered_depth_maps", f"{k:08d}.pfm"), depth)
+        c2w = np.eye(4)
+        c2w[:3, :3] = _random_rotation(g)
+        c2w[:3, 3] = g.uniform(-1, 1, 3)
+        w2c = np.linalg.inv(c2w)
+        f = g.uniform(0.8, 1.2) * width
+        K = np.array([[f, 0, width / 2 + g.uniform(-6, 6)], [0, f, height / 2 + g.uniform(-6, 6)], [0, 0, 1]])
+        with open(os.path.join(base, "cams", f"{k:08d}_cam.txt"), "w") as fh:
+            fh.write("extrinsic\n" + "\n".join(" ".join(f"{v:.9g}" for v in row) for row in w2c) + "\n\n")
+            fh.write("intrinsic\n" + "\n".join(" ".join(f"{v:.9g}" for v in row) for row in K) + "\n\n")
+            fh.write("425.0 2.5\n")
+    with open(os.path.join(base, "cams", "pair.txt"), "w") as fh:
+        fh.write(f"{frames}\n")
+        for k in range(frames):
+            others = [j for j in range(frames) if j != k][: frames - 2]
+            fh.write(f"{k}\n{len(others)} " + " ".join(f"{j} {100.0 - j:.1f}" for j in others) + "\n")
+    with open(os.path.join(root, "train_list.txt"), "w") as fh:
+        fh.write(scene + "\n")
+
+
+class BlendMVSLike(_ManyViewLike):
+    """Duck-typed stand-in for the reference's BlendMVS (spann3r/datasets/blendedmvs.py) over a tree written by
+    write_blendmvs_tree: the same pair sampling, the margin check, `depthmap.max()` of every cropped depth map for the
+    depth-range check, and the same recursive retry (`attempts`) on a frame without valid depth."""
+
+    def __init__(self, ROOT, resolution=224, num_frames=3, jitter=True, seed=None, min_thresh=2, max_thresh=5,
+                 num_seq=20, aug_crop=0, split="train"):
+        super().__init__(ROOT, resolution, num_frames, jitter, seed, min_thresh, max_thresh, num_seq, aug_crop, split)
+        with open(os.path.join(ROOT, f"{split}_list.txt")) as fh:
+            self.scene_list = fh.read().splitlines()
+
+    def sample_pairs(self, pairs_path, rng, max_trials=10):
+        with open(pairs_path) as fh:
+            lines = fh.read().splitlines()
+        for _ in range(max_trials):
+            s = rng.choice(int(lines[0]))
+            ref, cluster = int(lines[2 * s + 1]), lines[2 * s + 2].split()
+            n = int(cluster[0])
+            if n > self.num_frames - 1:
+                names = [f"{ref:08d}.jpg"] + [f"{int(cluster[2 * c + 1]):08d}.jpg"
+                                               for c in rng.choice(n, self.num_frames - 1, replace=False)]
+                if rng.choice([True, False]):
+                    names.reverse()
+                return names
+        return None
+
+    @staticmethod
+    def _read_cam(path):
+        with open(path) as fh:
+            lines = fh.read().splitlines()
+        RT = np.array([row.split() for row in lines[1:5]], dtype=np.float32)
+        K = np.array([row.split() for row in lines[7:10]], dtype=np.float32)
+        return K, RT
+
+    def _get_views(self, idx, resolution, rng, attempts=0):
+        import cv2
+        scene = self.scene_list[idx // self.num_seq]
+        base = os.path.join(self.ROOT, scene)
+        names = self.sample_pairs(os.path.join(base, "cams", "pair.txt"), rng)
+        if names is None:
+            return self._get_views(rng.integers(0, len(self) - 1), resolution, rng)
+        dmin, dmax, dfirst = 1e8, 0.0, None
+        views = []
+        for name in names:
+            path = os.path.join(base, "blended_images", name)
+            rgb = _imread_rgb(path)
+            depth = _imread_rgb(os.path.join(base, "rendered_depth_maps", name.replace(".jpg", ".pfm")),
+                                cv2.IMREAD_UNCHANGED)
+            depth = np.nan_to_num(depth.astype(np.float32), 0.0)
+            K, RT = self._read_cam(os.path.join(base, "cams", name.replace(".jpg", "_cam.txt")))
+            K = K[:3, :3]
+            pose = np.linalg.inv(RT)
+            H, W = rgb.shape[:2]
+            cx, cy = K[:2, 2].round().astype(int)
+            if min(cx, W - cx) <= W / 5 or min(cy, H - cy) <= H / 5:
+                return self._get_views(rng.integers(0, len(self) - 1), resolution, rng)
+            rgb, depth, Kf = self._crop_resize_if_necessary(rgb, depth, K, resolution, rng=rng, info=path)
+            dm = depth.max()
+            if dm > dmax:
+                dmax = dm
+            if dm < dmin:
+                dmin = dm
+            if dfirst is None:
+                dfirst = dm
+            if (depth > 0.0).sum() == 0 or not np.isfinite(pose).all():
+                if attempts >= 5:
+                    return self._get_views(rng.integers(0, len(self) - 1), resolution, rng)
+                return self._get_views(idx, resolution, rng, attempts + 1)
+            views.append(dict(img=rgb, depthmap=depth, camera_pose=pose, camera_intrinsics=Kf, dataset="blendmvs",
+                              label=os.path.join(scene, name), instance=os.path.split(path)[1]))
+        if dmax / dmin > 100.0 or dmax / dfirst > 10.0:
+            return self._get_views(rng.integers(0, len(self) - 1), resolution, rng)
+        return views

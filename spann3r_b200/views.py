@@ -21,6 +21,7 @@ File decoding stays on the CPU.  No CPU fallback: without the library or an H100
 from __future__ import annotations
 
 import ctypes as C
+from collections import OrderedDict
 
 import numpy as np
 import torch
@@ -40,6 +41,16 @@ def nearest_index(src: int, dst: int) -> np.ndarray:
     when dsize is given, as cropping.py:72 gives both."""
     ifx = 1.0 / (dst / src)
     return np.minimum(np.floor(np.arange(dst, dtype=np.int64) * ifx).astype(np.int64), src - 1)
+
+
+def depth_index(plan) -> tuple:
+    """Source column of every output column and source row of every output row of a planned view's depth map (int32):
+    crop 1, cv2 INTER_NEAREST rescale and crop 2 folded into two index tables (what the depth kernel gathers through)."""
+    l, t, r, b = plan["crop1"]
+    W2, H2 = plan["scaled"]
+    l2, t2, r2, b2 = plan["crop2"]
+    return ((l + nearest_index(r - l, W2)[l2:r2]).astype(np.int32),
+            (t + nearest_index(b - t, H2)[t2:b2]).astype(np.int32))
 
 
 def _to_colmap_scaled_shifted(K, scaling, offset):
@@ -111,6 +122,31 @@ def plan_view(h: int, w: int, K, resolution, aug_crop=0, rng=None) -> dict:
                 out=res, K=Kf.astype(np.float32), portrait=res[0] < res[1])
 
 
+JITTER_OPS = ("brightness", "contrast", "saturation", "hue")   # torchvision's fn_idx numbering
+
+
+def jitter_fields(params):
+    """One view's ColorJitter draw (None, or dict(order, brightness, contrast, saturation, hue)) -> the descriptor's
+    (order, skip mask, (b, c, s) fp32 factors, hue shift).  The shift is np.int32(hue * 255), which adjust_hue adds to
+    the uint8 hue (wrapping mod 256)."""
+    if params is None:
+        return (0, 1, 2, 3), 0xF, (1.0, 1.0, 1.0), 0
+    order = tuple(int(k) for k in params["order"])
+    if sorted(order) != [0, 1, 2, 3]:
+        raise ValueError(f"jitter order {order} is not a permutation of 0..3")
+    skip = sum(1 << k for k, name in enumerate(JITTER_OPS) if params.get(name) is None)
+    facs = []
+    for name in JITTER_OPS[:3]:
+        f = params.get(name)
+        if f is not None and float(np.float32(f)) != float(f):
+            raise ValueError(f"{name} factor {f!r} is not an fp32 value (torchvision draws them in fp32)")
+        facs.append(1.0 if f is None else float(f))
+    hue = params.get("hue")
+    if hue is not None and not -0.5 <= hue <= 0.5:
+        raise ValueError(f"hue factor {hue} is not in [-0.5, 0.5]")
+    return order, skip, tuple(facs), 0 if hue is None else int(np.int32(hue * 255))
+
+
 def _as_rgb(rgb) -> np.ndarray:
     if isinstance(rgb, torch.Tensor):
         rgb = rgb.cpu().numpy()
@@ -152,7 +188,11 @@ class ViewBuilder:
     camera_intrinsics [3, 3] f32, camera_pose [4, 4] f32, and true_shape int32 (height, width) before the landscape
     transpose (a host tensor, as the reference's collated batch has it).  (H, W) = (resolution[1], resolution[0]):
     portrait views come out transposed, as transpose_to_landscape leaves them.  Coefficient and index tables are
-    cached on the device per geometry."""
+    cached on the device for the MAX_GEOMETRIES most recently used geometries."""
+
+    # Training sets give nearly every frame its own crop geometry (the crop-1 window follows the principal point), so
+    # the per-geometry device tables (a few tens of KB each) are kept for the most recently used geometries only.
+    MAX_GEOMETRIES = 512
 
     def __init__(self, resolution, aug_crop=0, device="cuda"):
         _lib.require_device()
@@ -164,10 +204,11 @@ class ViewBuilder:
         self.device = torch.device(device)
         if self.device.type != "cuda":
             raise ValueError("ViewBuilder builds views on a CUDA device")
-        self._tables = {}
+        self._tables = OrderedDict()     # least recently used first; at most MAX_GEOMETRIES entries
         L = _lib.lib()
         if (L.s3r_views_abi_sizeof(0) != C.sizeof(_lib.ViewDepthDesc)
-                or L.s3r_views_abi_sizeof(1) != C.sizeof(_lib.ViewImageDesc)):
+                or L.s3r_views_abi_sizeof(1) != C.sizeof(_lib.ViewImageDesc)
+                or L.s3r_views_abi_sizeof(2) != C.sizeof(_lib.ViewJitterDesc)):
             raise _lib.S3RError("libspann3r_b200.so's view descriptors do not match the bindings: rebuild it")
 
     def plan(self, h: int, w: int, K, rng=None) -> dict:
@@ -189,7 +230,9 @@ class ViewBuilder:
         FrameAdapter), and the depth's source column / row of every output column / row."""
         key = (h, w, p["crop1"], p["scaled"], p["crop2"])
         g = self._tables.get(key)
-        if g is None:
+        if g is not None:
+            self._tables.move_to_end(key)
+        else:
             l, t, r, b = p["crop1"]
             W1, H1 = r - l, b - t
             W2, H2 = p["scaled"]
@@ -203,8 +246,7 @@ class ViewBuilder:
             bv[:, 0] -= row0
             n = bh.shape[0]
             span = max(int(bh[min(x0 + 127, n - 1), 0] + bh[min(x0 + 127, n - 1), 1] - bh[x0, 0]) for x0 in range(0, n, 128))
-            col_src = (l + nearest_index(W1, W2)[l2:r2]).astype(np.int32)
-            row_src = (t + nearest_index(H1, H2)[t2:b2]).astype(np.int32)
+            col_src, row_src = depth_index(p)
             parts = [bh, kh, bv, kv, col_src, row_src]
             offs = np.cumsum([0] + [a.size for a in parts])
             flat = np.concatenate([np.ascontiguousarray(a, dtype=np.int32).ravel() for a in parts])
@@ -214,17 +256,29 @@ class ViewBuilder:
             g = dict(tables=dev, bh=ptrs[0], kh=ptrs[1], bv=ptrs[2], kv=ptrs[3], col_src=ptrs[4], row_src=ptrs[5],
                      ksh=ksh, ksv=ksv, span=span, src_row0=t + row0, src_col0=l, rows=rows)
             self._tables[key] = g
+            if len(self._tables) > self.MAX_GEOMETRIES:
+                self._tables.popitem(last=False)   # device memory goes back to the stream-ordered caching allocator
         return g
 
     @torch.no_grad()
-    def build_planned(self, planned) -> list:
+    def build_planned(self, planned, jitter=None) -> list:
         """planned: (rgb, depth, pose, plan) per view, `plan` from plan_view (its K may be replaced by the intrinsics
-        the caller keeps).  One host-to-device copy and three launches for the whole list."""
+        the caller keeps).  One host-to-device copy and three launches for the whole list.
+
+        jitter: None (ImgNorm only), or one entry per view: None or the parameters torchvision's ColorJitter drew for
+        it, dict(order=fn_idx, brightness=, contrast=, saturation=, hue=) with None for an op that does not run (what
+        train_views.draw_jitter returns).  Then the vertical Lanczos pass stops at uint8 and a fourth launch applies
+        ColorJitter and ImgNorm (csrc/jitter.cu)."""
         n = len(planned)
         if n == 0:
             return []
         if n > 65535:
             raise ValueError("at most 65535 views per call")
+        if jitter is not None:
+            jitter = list(jitter)
+            if len(jitter) != n:
+                raise ValueError(f"jitter has {len(jitter)} entries for {n} views")
+            jitter = [jitter_fields(j) for j in jitter]
         Wr, Hr = self.resolution
         dev = self.device
         views = []
@@ -249,13 +303,17 @@ class ViewBuilder:
         dd_off = off
         off = _align(dd_off + n * C.sizeof(_lib.ViewDepthDesc))
         id_off = off
-        total = _align(id_off + n * C.sizeof(_lib.ViewImageDesc))
+        off = _align(id_off + n * C.sizeof(_lib.ViewImageDesc))
+        jd_off = off
+        total = _align(jd_off + n * C.sizeof(_lib.ViewJitterDesc)) if jitter is not None else off
         host = torch.empty(total, dtype=torch.uint8, pin_memory=True)
         hb = host.numpy()
         buf = torch.empty(total, dtype=torch.uint8, device=dev)
         base = buf.data_ptr()
         tmp_rows = [g["rows"] * p["out"][0] * 3 for (_, _, _, p, _, g) in views]
         tmp = torch.empty(max(1, sum(tmp_rows)), dtype=torch.uint8, device=dev)
+        u8_bytes = [_align(p["out"][0] * p["out"][1] * 3) for (_, _, _, p, _, _) in views]
+        u8 = torch.empty(sum(u8_bytes) if jitter is not None else 0, dtype=torch.uint8, device=dev)
         img = torch.empty((n, 3, Hr, Wr), dtype=torch.float32, device=dev)
         depthmap = torch.empty((n, Hr, Wr), dtype=torch.float32, device=dev)
         pts3d = torch.empty((n, Hr, Wr, 3), dtype=torch.float32, device=dev)
@@ -264,7 +322,8 @@ class ViewBuilder:
         kp = hb[kp_off:kp_off + n * 100].view(np.float32).reshape(n, 25)
         dds = (_lib.ViewDepthDesc * n)()
         ids = (_lib.ViewImageDesc * n)()
-        tmp_ptr = tmp.data_ptr()
+        jds = (_lib.ViewJitterDesc * n)()
+        tmp_ptr, u8_ptr = tmp.data_ptr(), u8.data_ptr()
         for i, ((rgb, depth, pose, p, K, g), (ro, do)) in enumerate(zip(views, lay)):
             h, w = rgb.shape[:2]
             hb[ro:ro + rgb.nbytes] = rgb.reshape(-1)
@@ -287,8 +346,16 @@ class ViewBuilder:
             tmp_ptr += tmp_rows[i]
             m.row_stride, m.rows, m.cols, m.out_rows = w * 3, g["rows"], W, H
             m.ksh, m.ksv, m.transpose = g["ksh"], g["ksv"], tr
+            if jitter is not None:
+                j = jds[i]
+                j.u8, j.img = u8_ptr, img[i].data_ptr()
+                u8_ptr += u8_bytes[i]
+                j.rows, j.cols, j.transpose = H, W, tr
+                j.order[:], j.skip, (j.brightness, j.contrast, j.saturation), j.hue_shift = jitter[i]
         hb[dd_off:dd_off + C.sizeof(dds)] = np.frombuffer(bytes(dds), dtype=np.uint8)
         hb[id_off:id_off + C.sizeof(ids)] = np.frombuffer(bytes(ids), dtype=np.uint8)
+        if jitter is not None:
+            hb[jd_off:jd_off + C.sizeof(jds)] = np.frombuffer(bytes(jds), dtype=np.uint8)
         buf.copy_(host, non_blocking=True)
         L = _lib.lib()
         max_pix = max(p["out"][0] * p["out"][1] for (_, _, _, p, _, _) in views)
@@ -300,7 +367,13 @@ class ViewBuilder:
             sp = _lib.stream_ptr(dev)
             _lib.check(L.s3r_views_depth(base + dd_off, n, max_pix, sp), "s3r_views_depth")
             _lib.check(L.s3r_views_resample_h(base + id_off, n, max_rows, max_cols, max_span, sp), "s3r_views_resample_h")
-            _lib.check(L.s3r_views_resample_v_norm(base + id_off, n, max_out_rows, max_cols, sp), "s3r_views_resample_v_norm")
+            if jitter is None:
+                _lib.check(L.s3r_views_resample_v_norm(base + id_off, n, max_out_rows, max_cols, sp),
+                           "s3r_views_resample_v_norm")
+            else:
+                _lib.check(L.s3r_views_resample_v_u8(base + id_off, base + jd_off, n, max_out_rows, max_cols, sp),
+                           "s3r_views_resample_v_u8")
+                _lib.check(L.s3r_views_color_jitter(base + jd_off, n, max_pix, sp), "s3r_views_color_jitter")
         bad = nonfinite.cpu().nonzero().flatten().tolist()     # waits for the launches
         if bad:
             raise ValueError(f"NaN / inf in the cropped depth map of view(s) {bad}")
