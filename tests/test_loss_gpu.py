@@ -15,6 +15,14 @@ pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 
 
+@pytest.fixture(autouse=True)
+def _restore_tf32():
+    """Tests below turn TF32 off for their comparisons: give the tests after them the settings they started with."""
+    old = torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32
+    yield
+    torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32 = old
+
+
 def native(crit_str):
     ns = {}
     exec("from spann3r_b200.loss import *", ns)

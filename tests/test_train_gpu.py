@@ -10,6 +10,14 @@ from conftest import get_state_dict, rel_l2
 pytestmark = pytest.mark.gpu
 
 
+@pytest.fixture(autouse=True)
+def _restore_tf32():
+    """Tests below turn TF32 off for their comparisons: give the tests after them the settings they started with."""
+    old = torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32
+    yield
+    torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32 = old
+
+
 @pytest.fixture(scope="module")
 def model():
     from spann3r_b200 import Spann3R
