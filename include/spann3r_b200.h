@@ -101,10 +101,13 @@ int s3r_col2im_3x3s2(const float* cols, int nb, int h, int w, int c, int ho, int
  *   taps = 1 (linear / 1x1 conv / ConvTranspose with kernel == stride) or 9 (3x3, stride 1, pad 1).
  * Replaces nn.Linear / Conv2d / ConvTranspose2d calls of croco/models/blocks.py:73-79,94-112,149-169,
  * dust3r/model.py:189-190, spann3r/model.py:250-261,310 and croco/models/dpt_block.py (all convs).
- * n is a multiple of 32 (the epilogue stores whole 32-column chunks).  ldr1, ldr2, ldo, ldp and plane_col0 are
+ * n is a multiple of 32 (the epilogue stores whole 32-column chunks), except in an S3R_EPI_PLAIN launch whose only
+ * output is out_f32, without residuals, with ldo >= n rounded up to 32 (the memory read's scores): there columns n ..
+ * of the last chunk are written too, with unspecified values.  ldr1, ldr2, ldo, ldp and plane_col0 are
  * non-negative multiples of 4 below 2^31 (16-byte residual / fp32 accesses, 8-byte plane stores); res1 may be
  * out_f32 with ldr1 == ldo (in-place residual, as the engine's proj / cproj / fc2 launches).  Every rule is
- * checked before the driver is touched: a rejected descriptor returns -1 and names the field in s3r_last_error(). */
+ * checked before the driver is touched: a rejected descriptor returns -1 and names the field in s3r_last_error().
+ * force_bn: 0 = the planner's tile width, or 64, 96 or 128; S3R_EPI_HEADTAIL always runs 128 wide. */
 typedef struct s3r_gemm_desc {
   const void* a_hi; const void* a_lo;
   const void* b_hi; const void* b_lo;
@@ -156,6 +159,12 @@ typedef struct s3r_gemm_desc {
    * accumulation; a_lo and b_lo are not read and may be NULL, and a folded LayerNorm's ln_cs must then be the row sums of
    * the hi plane alone (s3r_lin.cs_hi); S3R_EPI_HEADTAIL is split only.  Any other value is rejected. */
   int precision;
+  /* operand layout: lda / ldb are the row strides (elements) of an A pixel / a B row, non-negative multiples of 8
+   * (0 = dense: kc resp. taps*kc); b_group_rows (>= 0, 0 = n) is the number of B rows between consecutive groups.
+   * b_static = 1: B is never written by the work this launch depends on (packed weights), so the kernel may stage its
+   * first B tiles before the programmatic-dependent-launch wait; 0 = B is loaded after the wait. */
+  int64_t lda, ldb, b_group_rows;
+  int b_static;
 } s3r_gemm_desc;
 int s3r_gemm(const s3r_gemm_desc* d, void* stream);
 /* tile width the planner would pick (64/96/128), for tests */
@@ -450,10 +459,6 @@ int s3r_engine_memory_read(s3r_engine* e, const s3r_bank* bank, const float* fea
  * of (seed, (b * N + row) * len + column): reproducible, regenerated for the backward pass / tests by s3r_dropout_mask */
 int s3r_engine_memory_read_train(s3r_engine* e, const s3r_bank* bank, const float* feat, float thresh, float drop_p,
                                  uint64_t seed, float* out, void* stream);
-/* Tuning knobs of the GEMM planner, read when an engine builds its plans (first pass of a stage): "prefetch_b" (weight
- * tiles staged before the programmatic-dependent-launch wait; default 1).  The call exists so that two engines of one
- * process can be planned differently and timed alternately. */
-int s3r_set_option(const char* name, int value);
 /* out[i] = 0 or 1/(1-p): the keep-scale the training-mode read applies to flat element i = (b * N + row) * len + column */
 int s3r_dropout_mask(float* out, int64_t n, uint64_t seed, float p, void* stream);
 /* spann3r/model.py:80-95 add_mem: append N tokens at bank.len (caller then sets len += N) */

@@ -40,6 +40,7 @@ class GemmDesc(C.Structure):
         ("trace", _vp),
         ("swap_col0", _i), ("k2_out", _vp), ("vt2_out", _vp),
         ("precision", _i),
+        ("lda", _i64), ("ldb", _i64), ("b_group_rows", _i64), ("b_static", _i),
     ]
 
 
@@ -86,7 +87,6 @@ _PROTOS = {
     "s3r_conf_score": (_i, [_vp, _i64, _vp, _vp, _vp]),
     "s3r_conf_score_batched": (_i, [_vp, _i, _i64, _vp, _vp, _vp]),
     "s3r_dropout_mask": (_i, [_vp, _i64, C.c_uint64, _f, _vp]),
-    "s3r_set_option": (_i, [C.c_char_p, _i]),
     "s3r_focal_weiszfeld": (_i, [_vp, _i, _i, _i, _f, _f, _i, _f, _f, _vp, _vp, _vp]),
     "s3r_focal_median": (_i, [_vp, _i, _i, _i, _f, _f, _f, _f, _vp, _vp, _vp]),
     "s3r_pnp_workspace_bytes": (C.c_size_t, [_i, _i]),

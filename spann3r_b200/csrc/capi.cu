@@ -1,8 +1,6 @@
 // extern "C" boundary of libspann3r_b200.so (declared in include/spann3r_b200.h) -- op level.
 #include "../../include/spann3r_b200.h"
 
-#include <cstring>
-
 #include "gemm.cuh"
 #include "kernels.cuh"
 
@@ -85,144 +83,15 @@ int s3r_col2im_3x3s2(const float* cols, int nb, int h, int w, int c, int ho, int
   return launch_col2im_3x3s2(cols, nb, h, w, c, ho, wo, out, S(stream));
 }
 
-// Row strides and column offsets of the epilogue's fp32 (float4) and planes (uint2) accesses: multiples of 4 elements
-// that fit the kernel's int fields.
-static bool bad_ld(int64_t ld) { return ld < 0 || ld > INT32_MAX || ld % 4 != 0; }
-
-// Every descriptor rule the epilogue relies on, checked before anything touches the driver.
-static int check_desc(const s3r_gemm_desc* d) {
-  if (d->precision != GEMM_SPLIT && d->precision != GEMM_BF16) {
-    set_error("s3r_gemm: precision=%d must be 0 (split bf16) or 1 (one bf16 product)", d->precision);
-    return -1;
-  }
-  if (d->precision == GEMM_BF16 && d->epi == S3R_EPI_HEADTAIL) {
-    set_error("s3r_gemm: precision=1 does not support EPI_HEADTAIL (the DPT head tail is split-only)");
-    return -1;
-  }
-  if (d->n <= 0 || d->n % 32 != 0) {
-    set_error("s3r_gemm: n=%d must be a positive multiple of 32 (the epilogue stores whole 32-column chunks)", d->n);
-    return -1;
-  }
-  if (d->epi == S3R_EPI_HEADTAIL && d->n != 128) {
-    set_error("s3r_gemm: EPI_HEADTAIL needs n == 128");
-    return -1;
-  }
-  if (d->epi == S3R_EPI_PIXSHUF && (d->ps_s <= 0 || d->ps_cout % 32 != 0 || d->n != d->ps_s * d->ps_s * d->ps_cout)) {
-    set_error("s3r_gemm: EPI_PIXSHUF needs n == s*s*cout and cout %% 32 == 0");
-    return -1;
-  }
-  const struct { const char* name; bool used; int64_t v; } lds[5] = {
-      {"ldr1", d->res1 != nullptr, d->ldr1}, {"ldr2", d->res2 != nullptr, d->ldr2}, {"ldo", d->out_f32 != nullptr, d->ldo},
-      {"ldp", d->out_hi != nullptr, d->ldp}, {"plane_col0", d->out_hi != nullptr, d->plane_col0}};
-  for (const auto& l : lds)
-    if (l.used && bad_ld(l.v)) {
-      set_error("s3r_gemm: %s=%lld must be a non-negative multiple of 4 below 2^31 (vector accesses)", l.name,
-                (long long)l.v);
-      return -1;
-    }
-  if (d->epi == S3R_EPI_QKV) {
-    if (d->q_c <= 0 || d->q_c % 64 != 0 || d->h != 1 || d->q_ntok <= 0 || d->w != d->q_nb * d->q_ntok) {
-      set_error("s3r_gemm: EPI_QKV needs q_c %% 64 == 0, h == 1, w == q_nb*q_ntok");
-      return -1;
-    }
-    if (d->n % d->q_c != 0) {
-      set_error("s3r_gemm: EPI_QKV n=%d must be a multiple of q_c=%d", d->n, d->q_c);
-      return -1;
-    }
-    if (d->q_role_base < 0 || d->q_role_base + d->n / d->q_c > 5) {
-      set_error("s3r_gemm: EPI_QKV q_role_base=%d + n/q_c=%d must stay within the 5 roles", d->q_role_base,
-                d->n / d->q_c);
-      return -1;
-    }
-    if (d->q_ntok_pad < d->q_ntok || d->q_ntok_pad % 4 != 0) {
-      set_error("s3r_gemm: EPI_QKV q_ntok_pad=%d must be >= q_ntok=%d and a multiple of 4", d->q_ntok_pad, d->q_ntok);
-      return -1;
-    }
-    static const char* const kRoleOut[5] = {"q_out", "k_out", "vt_out", "k2_out", "vt2_out"};
-    for (int role = d->q_role_base; role < d->q_role_base + d->n / d->q_c; ++role) {
-      const void* p = role == 0 ? (const void*)d->q_out : role == 1 ? (const void*)d->k_out : role == 2 ? (const void*)d->vt_out
-                    : role == 3 ? (const void*)d->k2_out : (const void*)d->vt2_out;
-      if (!p) {
-        set_error("s3r_gemm: EPI_QKV role %d is written but %s is NULL", role, kRoleOut[role]);
-        return -1;
-      }
-    }
-    if (d->q_rope && (!d->q_pos || !d->q_cs)) {
-      set_error("s3r_gemm: EPI_QKV with q_rope needs %s", d->q_pos ? "q_cs" : "q_pos");
-      return -1;
-    }
-  }
-  if (d->ln_stats) {
-    if (d->ln_cs == nullptr || d->ln_np * 32 != d->kc || d->taps != 1 || d->epi == S3R_EPI_PIXSHUF) {
-      set_error("s3r_gemm: folded LayerNorm needs ln_cs, ln_np == kc/32, taps == 1 and a non-PIXSHUF epilogue");
-      return -1;
-    }
-    if (d->ln_np < 2 || d->ln_np > 32 || d->ln_np % 2 != 0) {
-      set_error("s3r_gemm: folded LayerNorm needs an even ln_np in [2, 32] (kc %% 64 == 0, kc <= 1024), got ln_np=%d",
-                d->ln_np);
-      return -1;
-    }
-  }
-  if (d->swap_col0 % 256 != 0) {
-    set_error("s3r_gemm: swap_col0 must be a multiple of 256");
-    return -1;
-  }
-  if (d->stats_out && d->epi != S3R_EPI_PLAIN) {
-    set_error("s3r_gemm: stats_out needs EPI_PLAIN");
-    return -1;
-  }
-  return 0;
-}
-
-static int fill_plan(const s3r_gemm_desc* d, GemmPlan* plan) {
-  int r = check_desc(d);
-  if (r) return r;
-  const int force_bn = d->epi == S3R_EPI_HEADTAIL ? (d->force_bn == 128 ? 128 : 1128) : d->force_bn;
-  r = gemm_plan_init(plan, B(d->a_hi), B(d->a_lo), B(d->b_hi), B(d->b_lo), d->groups, d->nb, d->h, d->w, d->kc,
-                     d->taps, d->n, force_bn, 0, 0, 0, d->precision, d->a_swap ? d->swap_col0 : 0);
-  if (r) return r;
-  GemmArgs& a = plan->args;
-  a.epi = d->epi; a.act = d->act; a.plane_relu = d->plane_relu;
-  a.bias = d->bias;
-  a.res1 = d->res1; a.ldr1 = (int)d->ldr1;
-  a.res2 = d->res2; a.ldr2 = (int)d->ldr2;
-  a.out_f32 = d->out_f32; a.ldo = (int)d->ldo;
-  a.out_hi = B(d->out_hi); a.out_lo = B(d->out_lo); a.ldp = (int)d->ldp; a.plane_col0 = d->plane_col0;
-  if (d->epi == S3R_EPI_PIXSHUF) {
-    a.ps_s = d->ps_s; a.ps_cout = d->ps_cout;
-    a.out_group_rows = (long long)d->nb * d->h * d->ps_s * d->w * d->ps_s;
-  }
-  if (d->epi == S3R_EPI_QKV) {
-    a.q_C = d->q_c; a.q_role_base = d->q_role_base; a.q_ntok = d->q_ntok; a.q_ntok_pad = d->q_ntok_pad;
-    a.q_rope = d->q_rope; a.q_nb = d->q_nb; a.q_pos = d->q_pos;
-    a.q_cs = reinterpret_cast<const float2*>(d->q_cs);
-    a.q_out = d->q_out; a.k_out = d->k_out; a.vt_out = d->vt_out; a.q_scale = d->q_scale;
-    a.k2_out = d->k2_out; a.vt2_out = d->vt2_out;
-  }
-  if (d->epi == S3R_EPI_HEADTAIL) {
-    a.ht_w = d->ht_w; a.ht_b = d->ht_b; a.ht_pts = d->ht_pts; a.ht_conf = d->ht_conf;
-  }
-  if (d->ln_stats) {
-    a.ln_stats = reinterpret_cast<const float2*>(d->ln_stats); a.ln_np = d->ln_np; a.ln_eps = d->ln_eps; a.ln_cs = d->ln_cs;
-  }
-  a.a_swap = d->a_swap ? 1 : 0;
-  a.swap_col0 = d->swap_col0;
-  a.stats_out = reinterpret_cast<float2*>(d->stats_out);
-  a.trace = reinterpret_cast<unsigned long long*>(d->trace);
-  return 0;
-}
-
 int s3r_gemm(const s3r_gemm_desc* d, void* stream) {
   GemmPlan plan;
-  int r = fill_plan(d, &plan);
-  if (r) return r;
+  if (int r = gemm_plan(*d, &plan)) return r;
   return gemm_launch(plan, S(stream));
 }
 
 int s3r_gemm_tile_n(const s3r_gemm_desc* d) {
   GemmPlan plan;
-  int r = fill_plan(d, &plan);
-  if (r) return r;
+  if (int r = gemm_plan(*d, &plan)) return r;
   return plan.bn;
 }
 
@@ -328,14 +197,6 @@ int s3r_conf_score(const float* conf, int64_t n, float* scratch256, float* out, 
 }
 int s3r_conf_score_batched(const float* conf, int batch, int64_t hw, float* scratch, float* out, void* stream) {
   return launch_conf_score_batched(conf, batch, hw, scratch, out, S(stream));
-}
-
-int s3r_set_option(const char* name, int value) {
-  s3r::Options& o = s3r::options();
-  if (!name) { set_error("s3r_set_option: null name"); return -1; }
-  if (!strcmp(name, "prefetch_b")) o.prefetch_b = value;
-  else { set_error("s3r_set_option: unknown option '%s' (prefetch_b)", name); return -1; }
-  return 0;
 }
 
 int s3r_dropout_mask(float* out, int64_t n, uint64_t seed, float p, void* stream) {

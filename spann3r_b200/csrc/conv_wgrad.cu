@@ -8,7 +8,7 @@
 // dW [N, taps, Kc] is the engine's packed-weight layout, i.e. PyTorch's weight.permute(0, 2, 3, 1).
 //
 // No transposed copies: both operands are read straight from the NHWC planes by TMA, 64 channels x (bw x bh = 64) pixels
-// per box -- the 4-D box geometry of gemm_plan_init, with the tap offset on X's pixel coordinates and the zero fill of
+// per box -- the 4-D box geometry of gemm_plan, with the tap offset on X's pixel coordinates and the zero fill of
 // out-of-bounds pixels as the conv's zero padding.  A box lands in shared memory as 64 rows (pixels, the contraction) of
 // 128 bytes (channels), SWIZZLE_128B: exactly wgmma's MN-major 128-byte-swizzle canonical layout, so the MMAs read it with
 // the transpose bits set.  The contraction is split over CTAs (the conv's output is at most a few hundred 128 x 128 tiles,

@@ -32,30 +32,16 @@ inline Planes WP(const s3r_planes& p) {
   return r;
 }
 
-struct Geom {
-  int groups = 1, NB = 1, H = 1, W = 1, Kc = 0, taps = 1, N = 0, force_bn = 0;
-  int b_static = 1;   // B = packed weights (everything except the two memory-read GEMMs, whose B is the bank)
-  long long lda = 0, ldb = 0, b_group_rows = 0;
-};
-
-struct Epi {
-  int epi = EPI_PLAIN, act = ACT_NONE, plane_relu = 0;
-  const float* bias = nullptr;
-  const float* res1 = nullptr; int ldr1 = 0;
-  const float* res2 = nullptr; int ldr2 = 0;
-  float* out = nullptr; int ldo = 0;
-  Planes op; int ldp = 0, col0 = 0;
-  int ps_s = 0, ps_cout = 0;
-  int q_C = 0, q_role_base = 0, q_ntok = 0, q_ntok_pad = 0, q_rope = 0, q_nb = 0;
-  const int* q_pos = nullptr; const float2* q_cs = nullptr;
-  float *q_out = nullptr, *k_out = nullptr, *vt_out = nullptr; float q_scale = 1.f;
-  float *k2_out = nullptr, *vt2_out = nullptr; int swap_col0 = 0;
-  const float *ht_w = nullptr, *ht_b = nullptr; float *ht_pts = nullptr, *ht_conf = nullptr;
-  // folded LayerNorm: consumer side (statistics of the A rows + column sums of the gamma-folded weights) ...
-  const float2* ln_stats = nullptr; int ln_np = 0; float ln_eps = 0.f; const float* ln_cs = nullptr; int a_swap = 0;
-  const float* ln_cs_hi = nullptr;   // column sums of the hi plane alone: the ones a GEMM_BF16 launch subtracts
-  float2* stats_out = nullptr;   // ... and producer side (chunk sums of the rows this GEMM writes)
-};
+// A GEMM on planes A (groups x [W, Kc]) and B (groups x [N, Kc]): dense layout, EPI_PLAIN, B a packed weight that the
+// kernel may stage before its dependency wait (b_static: every launch except the memory read's two, whose B is the bank).
+s3r_gemm_desc gemm_desc(Planes A, Planes Bw, int groups, int W, int Kc, int N) {
+  s3r_gemm_desc d = {};
+  d.a_hi = A.hi; d.a_lo = A.lo; d.b_hi = Bw.hi; d.b_lo = Bw.lo;
+  d.groups = groups; d.nb = d.h = d.taps = 1; d.w = W; d.kc = Kc; d.n = N;
+  d.b_static = 1;
+  return d;
+}
+void out_planes(s3r_gemm_desc& d, Planes p, int ldp) { d.out_hi = p.hi; d.out_lo = p.lo; d.ldp = ldp; }
 
 // Plans are created on the first pass through a stage and replayed afterwards (same call order).  `precision` is the
 // GemmPrecision of every GEMM of the stage: the engine's for encode / decode / keyheads / value, split for the rest.
@@ -154,45 +140,29 @@ struct s3r_engine {
     return p;
   }
 
-  int gemm(PlanCache& pc, Planes A, Planes Bw, const Geom& g, const Epi& e, cudaStream_t st) {
+  // Folded LayerNorm (consumer side): the chunk statistics of the A rows, and the column sums of exactly the planes the
+  // tensor core multiplies (hi + lo, or hi alone at GEMM_BF16)
+  static void fold_ln(s3r_gemm_desc& d, const PlanCache& pc, const float2* stats, const s3r_lin& w) {
+    d.ln_stats = (const float*)stats; d.ln_np = d.kc / 32; d.ln_eps = 1e-6f;
+    d.ln_cs = pc.precision == GEMM_BF16 ? w.cs_hi : w.cs;
+  }
+
+  int gemm(PlanCache& pc, s3r_gemm_desc d, cudaStream_t st) {
+    if (d.ln_stats && !d.ln_cs) {
+      set_error("engine: a LayerNorm-folded linear lacks its %s column sums", pc.precision == GEMM_BF16 ? "cs_hi" : "cs");
+      return -1;
+    }
     if (pc.building) {
+      d.precision = pc.precision;
       pc.gemms.emplace_back();
-      int r = gemm_plan_init(&pc.gemms.back(), A.hi, A.lo, Bw.hi, Bw.lo, g.groups, g.NB, g.H, g.W, g.Kc, g.taps, g.N,
-                             e.epi == EPI_HEADTAIL ? 1128 : g.force_bn, g.lda, g.ldb, g.b_group_rows, pc.precision,
-                             e.a_swap ? e.swap_col0 : 0);
-      if (r) return r;
-      pc.gemms.back().b_static = (g.b_static && options().prefetch_b) ? 1 : 0;   // decided when the plan is built
+      if (int r = gemm_plan(d, &pc.gemms.back())) return r;
     }
     if (pc.gc >= pc.gemms.size()) {
       set_error("engine: plan cache out of sync");
       return -8;
     }
     GemmPlan& p = pc.gemms[pc.gc++];
-    GemmArgs& a = p.args;
-    a.epi = e.epi; a.act = e.act; a.plane_relu = e.plane_relu;
-    a.bias = e.bias; a.res1 = e.res1; a.ldr1 = e.ldr1; a.res2 = e.res2; a.ldr2 = e.ldr2;
-    a.out_f32 = e.out; a.ldo = e.ldo; a.out_hi = e.op.hi; a.out_lo = e.op.lo; a.ldp = e.ldp; a.plane_col0 = e.col0;
-    if (e.epi == EPI_PIXSHUF) {
-      a.ps_s = e.ps_s; a.ps_cout = e.ps_cout;
-      a.out_group_rows = (long long)g.NB * g.H * e.ps_s * g.W * e.ps_s;
-    } else if (e.epi == EPI_QKV) {
-      a.q_C = e.q_C; a.q_role_base = e.q_role_base; a.q_ntok = e.q_ntok; a.q_ntok_pad = e.q_ntok_pad;
-      a.q_rope = e.q_rope; a.q_nb = e.q_nb; a.q_pos = e.q_pos; a.q_cs = e.q_cs;
-      a.q_out = e.q_out; a.k_out = e.k_out; a.vt_out = e.vt_out; a.q_scale = e.q_scale;
-      a.k2_out = e.k2_out; a.vt2_out = e.vt2_out;
-    } else if (e.epi == EPI_HEADTAIL) {
-      a.ht_w = e.ht_w; a.ht_b = e.ht_b; a.ht_pts = e.ht_pts; a.ht_conf = e.ht_conf;
-    }
-    // a folded LayerNorm subtracts mean * (column sums of exactly the planes the tensor core multiplies)
-    const float* cs = p.precision == GEMM_BF16 ? e.ln_cs_hi : e.ln_cs;
-    if (e.ln_stats && !cs) {
-      set_error("engine: a LayerNorm-folded linear lacks its %s column sums", p.precision == GEMM_BF16 ? "cs_hi" : "cs");
-      return -1;
-    }
-    a.ln_stats = e.ln_stats; a.ln_np = e.ln_np; a.ln_eps = e.ln_eps; a.ln_cs = cs; a.a_swap = e.a_swap;
-    a.swap_col0 = e.swap_col0;
-    a.stats_out = e.stats_out;
-    a.b_static = p.b_static;
+    gemm_set_epilogue(d, p.args);
     flops += p.flops;
     ++launches;
     if (!profiling) return gemm_launch(p, st);
@@ -249,13 +219,12 @@ struct s3r_engine {
   };
   int vit_qkv(PlanCache& pc, const s3r_block_w& bw, const VitCfg& c, int nimg, bool rope, cudaStream_t st,
               const int* pos_tab) {
-    const int rows = nimg * N;
-    Geom g; g.W = rows; g.Kc = c.D; g.N = 3 * c.Da;
-    Epi e; e.epi = EPI_QKV; e.bias = bw.qkv.b; e.q_C = c.Da; e.q_role_base = 0; e.q_ntok = N; e.q_ntok_pad = Npad;
-    e.q_rope = rope ? 1 : 0; e.q_nb = nimg; e.q_pos = pos_tab; e.q_cs = (const float2*)(c.cs ? c.cs : w.rope_cs);
-    e.q_out = Qb; e.k_out = Kb; e.vt_out = Vtb; e.q_scale = c.q_scale;
-    e.ln_stats = St1; e.ln_np = c.D / 32; e.ln_eps = 1e-6f; e.ln_cs = bw.qkv.cs; e.ln_cs_hi = bw.qkv.cs_hi;   // norm1
-    return gemm(pc, P, WP(bw.qkv.w), g, e, st);
+    s3r_gemm_desc d = gemm_desc(P, WP(bw.qkv.w), 1, nimg * N, c.D, 3 * c.Da);
+    d.epi = EPI_QKV; d.bias = bw.qkv.b; d.q_c = c.Da; d.q_role_base = 0; d.q_ntok = N; d.q_ntok_pad = Npad;
+    d.q_rope = rope ? 1 : 0; d.q_nb = nimg; d.q_pos = pos_tab; d.q_cs = c.cs ? c.cs : w.rope_cs;
+    d.q_out = Qb; d.k_out = Kb; d.vt_out = Vtb; d.q_scale = c.q_scale;
+    fold_ln(d, pc, St1, bw.qkv);   // norm1
+    return gemm(pc, d, st);
   }
   int vit_blocks(PlanCache& pc, const s3r_block_w* blocks, int depth, const VitCfg& c, int nimg, bool rope, float* Xp,
                  cudaStream_t st, const int* pos_tab = nullptr) {
@@ -267,22 +236,22 @@ struct s3r_engine {
       const s3r_block_w& bw = blocks[l];
       if ((r = attention(pc, Qb, Kb, Vtb, nimg * heads, heads, N, N, AO, c.Da, st))) return r;
       {
-        Geom g; g.W = rows; g.Kc = c.Da; g.N = D;
-        Epi e; e.bias = bw.proj.b; e.res1 = Xp; e.ldr1 = D; e.out = Xp; e.ldo = D;
-        e.op = P2; e.ldp = D; e.stats_out = St2;
-        if ((r = gemm(pc, AO, WP(bw.proj.w), g, e, st))) return r;
+        s3r_gemm_desc d = gemm_desc(AO, WP(bw.proj.w), 1, rows, c.Da, D);
+        d.bias = bw.proj.b; d.res1 = Xp; d.ldr1 = D; d.out_f32 = Xp; d.ldo = D;
+        out_planes(d, P2, D); d.stats_out = (float*)St2;
+        if ((r = gemm(pc, d, st))) return r;
       }
       {
-        Geom g; g.W = rows; g.Kc = D; g.N = 4 * D;
-        Epi e; e.bias = bw.fc1.b; e.act = ACT_GELU; e.op = Hb; e.ldp = 4 * D;
-        e.ln_stats = St2; e.ln_np = D / 32; e.ln_eps = 1e-6f; e.ln_cs = bw.fc1.cs; e.ln_cs_hi = bw.fc1.cs_hi;   // norm2
-        if ((r = gemm(pc, P2, WP(bw.fc1.w), g, e, st))) return r;
+        s3r_gemm_desc d = gemm_desc(P2, WP(bw.fc1.w), 1, rows, D, 4 * D);
+        d.bias = bw.fc1.b; d.act = ACT_GELU; out_planes(d, Hb, 4 * D);
+        fold_ln(d, pc, St2, bw.fc1);   // norm2
+        if ((r = gemm(pc, d, st))) return r;
       }
       {
-        Geom g; g.W = rows; g.Kc = 4 * D; g.N = D;
-        Epi e; e.bias = bw.fc2.b; e.res1 = Xp; e.ldr1 = D; e.out = Xp; e.ldo = D;
-        e.op = P; e.ldp = D; e.stats_out = St1;
-        if ((r = gemm(pc, Hb, WP(bw.fc2.w), g, e, st))) return r;
+        s3r_gemm_desc d = gemm_desc(Hb, WP(bw.fc2.w), 1, rows, 4 * D, D);
+        d.bias = bw.fc2.b; d.res1 = Xp; d.ldr1 = D; d.out_f32 = Xp; d.ldo = D;
+        out_planes(d, P, D); d.stats_out = (float*)St1;
+        if ((r = gemm(pc, d, st))) return r;
       }
       if (l + 1 < depth && (r = vit_qkv(pc, blocks[l + 1], c, nimg, rope, st, pos_tab))) return r;
     }
@@ -546,10 +515,10 @@ int s3r_engine_encode(s3r_engine* e, const float* img, int nimg, float* feat, vo
                                  e->Pim.lo, st)))
     return r;
   {
-    Geom g; g.W = rows; g.Kc = 768; g.N = 1024;
-    Epi ep; ep.bias = e->w.patch_embed.b; ep.out = e->X; ep.ldo = 1024;
-    ep.op = e->P; ep.ldp = 1024; ep.stats_out = e->St1;   // block 0's folded norm1 reads these
-    if ((r = e->gemm(pc, e->Pim, WP(e->w.patch_embed.w), g, ep, st))) return r;
+    s3r_gemm_desc d = gemm_desc(e->Pim, WP(e->w.patch_embed.w), 1, rows, 768, 1024);
+    d.bias = e->w.patch_embed.b; d.out_f32 = e->X; d.ldo = 1024;
+    out_planes(d, e->P, 1024); d.stats_out = (float*)e->St1;   // block 0's folded norm1 reads these
+    if ((r = e->gemm(pc, d, st))) return r;
   }
   if ((r = e->vit_blocks(pc, e->w.enc, 24, s3r_engine::VitCfg(), nimg, true, e->X, st))) return r;
   if ((r = e->ln(e->X, e->w.enc_norm, 0, 0, 1e-6f, rows, 1024, feat, 1024, Planes(), 0, 0, 0, st))) return r;
@@ -567,7 +536,6 @@ int s3r_engine_decode(s3r_engine* e, const float* f1, const float* f2, float* de
   pc.begin();
   const int N = e->N, B = e->B;
   const long long R = (long long)B * N;
-  const float2* cs = (const float2*)e->w.rope_cs;
   int r;
   // hook 0 of the DPT heads = the encoder-dim inputs themselves (dust3r/model.py:187); also the A operand of
   // decoder_embed.  Stream 1 -> group 0, stream 2 -> group 1.
@@ -575,10 +543,11 @@ int s3r_engine_decode(s3r_engine* e, const float* f1, const float* f2, float* de
   if ((r = launch_split(f1, 1024, e->E0.hi, e->E0.lo, 1024, 0, R, 1024, 0, st))) return r;
   if ((r = launch_split(f2, 1024, e->E0.hi + R * 1024, e->E0.lo + R * 1024, 1024, 0, R, 1024, 0, st))) return r;
   {
-    Geom g; g.W = (int)(2 * R); g.Kc = 1024; g.N = 768;   // shared weights: one group of 2R rows
-    Epi ep; ep.bias = e->w.decoder_embed.b; ep.out = e->Xd; ep.ldo = 768;
-    ep.op = e->Pa; ep.ldp = 768; ep.stats_out = e->Sa;
-    if ((r = e->gemm(pc, e->E0, WP(e->w.decoder_embed.w), g, ep, st))) return r;
+    // shared weights: one group of 2R rows
+    s3r_gemm_desc d = gemm_desc(e->E0, WP(e->w.decoder_embed.w), 1, (int)(2 * R), 1024, 768);
+    d.bias = e->w.decoder_embed.b; d.out_f32 = e->Xd; d.ldo = 768;
+    out_planes(d, e->Pa, 768); d.stats_out = (float*)e->Sa;
+    if ((r = e->gemm(pc, d, st))) return r;
   }
   // All four LayerNorms of a DecoderBlock are folded into the GEMMs that consume them (s3r_lin.cs).  `xin` = planes
   // of the layer input (both streams), Sa its chunk statistics: read by qkv (norm1) and -- with the groups swapped,
@@ -590,13 +559,13 @@ int s3r_engine_decode(s3r_engine* e, const float* f1, const float* f2, float* de
     // self-attention q, k, v (norm1 folded) and -- same launch, columns >= 2304 reading the OTHER stream's layer
     // input (norm_y folded, group swap) -- the cross-attention k, v
     const s3r_decblock_w& bw = e->w.dec[l];
-    Geom g; g.groups = 2; g.W = (int)R; g.Kc = 768; g.N = 3840;
-    Epi ep; ep.epi = EPI_QKV; ep.bias = bw.qkv.b; ep.q_C = 768; ep.q_role_base = 0; ep.q_ntok = N; ep.q_ntok_pad = e->Npad;
-    ep.q_rope = 1; ep.q_nb = B; ep.q_pos = e->pos; ep.q_cs = cs;
-    ep.q_out = e->Qd; ep.k_out = e->Kd; ep.vt_out = e->Vtd; ep.k2_out = e->Kd2; ep.vt2_out = e->Vtd2; ep.q_scale = 0.125f;
-    ep.ln_stats = e->Sa; ep.ln_np = 24; ep.ln_eps = 1e-6f; ep.ln_cs = bw.qkv.cs; ep.ln_cs_hi = bw.qkv.cs_hi;
-    ep.a_swap = 1; ep.swap_col0 = 2304;
-    return e->gemm(pc, xin, WP(bw.qkv.w), g, ep, st);
+    s3r_gemm_desc d = gemm_desc(xin, WP(bw.qkv.w), 2, (int)R, 768, 3840);
+    d.epi = EPI_QKV; d.bias = bw.qkv.b; d.q_c = 768; d.q_role_base = 0; d.q_ntok = N; d.q_ntok_pad = e->Npad;
+    d.q_rope = 1; d.q_nb = B; d.q_pos = e->pos; d.q_cs = e->w.rope_cs;
+    d.q_out = e->Qd; d.k_out = e->Kd; d.vt_out = e->Vtd; d.k2_out = e->Kd2; d.vt2_out = e->Vtd2; d.q_scale = 0.125f;
+    e->fold_ln(d, pc, e->Sa, bw.qkv);
+    d.a_swap = 1; d.swap_col0 = 2304;
+    return e->gemm(pc, d, st);
   };
   Planes xin = e->Pa;
   if ((r = qkv_launch(0, xin))) return r;
@@ -604,42 +573,42 @@ int s3r_engine_decode(s3r_engine* e, const float* f1, const float* f2, float* de
     const s3r_decblock_w& bw = e->w.dec[l];
     if ((r = e->attention(pc, e->Qd, e->Kd, e->Vtd, 2 * B * 12, 12, N, N, e->AOd, 768, st))) return r;
     {
-      Geom g; g.groups = 2; g.W = (int)R; g.Kc = 768; g.N = 768;
-      Epi ep; ep.bias = bw.proj.b; ep.res1 = e->Xd; ep.ldr1 = 768; ep.out = e->Xd; ep.ldo = 768;
-      ep.op = e->Pb; ep.ldp = 768; ep.stats_out = e->Sb;
-      if ((r = e->gemm(pc, e->AOd, WP(bw.proj.w), g, ep, st))) return r;
+      s3r_gemm_desc d = gemm_desc(e->AOd, WP(bw.proj.w), 2, (int)R, 768, 768);
+      d.bias = bw.proj.b; d.res1 = e->Xd; d.ldr1 = 768; d.out_f32 = e->Xd; d.ldo = 768;
+      out_planes(d, e->Pb, 768); d.stats_out = (float*)e->Sb;
+      if ((r = e->gemm(pc, d, st))) return r;
     }
     // cross attention: q from norm2(x), k/v from norm_y(y), y = the other stream's layer input
     {
-      Geom g; g.groups = 2; g.W = (int)R; g.Kc = 768; g.N = 768;
-      Epi ep; ep.epi = EPI_QKV; ep.bias = bw.q.b; ep.q_C = 768; ep.q_role_base = 0; ep.q_ntok = N; ep.q_ntok_pad = e->Npad;
-      ep.q_rope = 1; ep.q_nb = B; ep.q_pos = e->pos; ep.q_cs = cs;
-      ep.q_out = e->Qd; ep.k_out = e->Kd; ep.vt_out = e->Vtd; ep.q_scale = 0.125f;
-      ep.ln_stats = e->Sb; ep.ln_np = 24; ep.ln_eps = 1e-6f; ep.ln_cs = bw.q.cs; ep.ln_cs_hi = bw.q.cs_hi;     // norm2
-      if ((r = e->gemm(pc, e->Pb, WP(bw.q.w), g, ep, st))) return r;
+      s3r_gemm_desc d = gemm_desc(e->Pb, WP(bw.q.w), 2, (int)R, 768, 768);
+      d.epi = EPI_QKV; d.bias = bw.q.b; d.q_c = 768; d.q_role_base = 0; d.q_ntok = N; d.q_ntok_pad = e->Npad;
+      d.q_rope = 1; d.q_nb = B; d.q_pos = e->pos; d.q_cs = e->w.rope_cs;
+      d.q_out = e->Qd; d.k_out = e->Kd; d.vt_out = e->Vtd; d.q_scale = 0.125f;
+      e->fold_ln(d, pc, e->Sb, bw.q);     // norm2
+      if ((r = e->gemm(pc, d, st))) return r;
     }
     if ((r = e->attention(pc, e->Qd, e->Kd2, e->Vtd2, 2 * B * 12, 12, N, N, e->AOd, 768, st))) return r;
     {
-      Geom g; g.groups = 2; g.W = (int)R; g.Kc = 768; g.N = 768;
-      Epi ep; ep.bias = bw.cproj.b; ep.res1 = e->Xd; ep.ldr1 = 768; ep.out = e->Xd; ep.ldo = 768;
-      ep.op = e->Pc; ep.ldp = 768; ep.stats_out = e->Sc;
-      if ((r = e->gemm(pc, e->AOd, WP(bw.cproj.w), g, ep, st))) return r;
+      s3r_gemm_desc d = gemm_desc(e->AOd, WP(bw.cproj.w), 2, (int)R, 768, 768);
+      d.bias = bw.cproj.b; d.res1 = e->Xd; d.ldr1 = 768; d.out_f32 = e->Xd; d.ldo = 768;
+      out_planes(d, e->Pc, 768); d.stats_out = (float*)e->Sc;
+      if ((r = e->gemm(pc, d, st))) return r;
     }
     // MLP
     {
-      Geom g; g.groups = 2; g.W = (int)R; g.Kc = 768; g.N = 3072;
-      Epi ep; ep.bias = bw.fc1.b; ep.act = ACT_GELU; ep.op = e->Hd; ep.ldp = 3072;
-      ep.ln_stats = e->Sc; ep.ln_np = 24; ep.ln_eps = 1e-6f; ep.ln_cs = bw.fc1.cs; ep.ln_cs_hi = bw.fc1.cs_hi; // norm3
-      if ((r = e->gemm(pc, e->Pc, WP(bw.fc1.w), g, ep, st))) return r;
+      s3r_gemm_desc d = gemm_desc(e->Pc, WP(bw.fc1.w), 2, (int)R, 768, 3072);
+      d.bias = bw.fc1.b; d.act = ACT_GELU; out_planes(d, e->Hd, 3072);
+      e->fold_ln(d, pc, e->Sc, bw.fc1);   // norm3
+      if ((r = e->gemm(pc, d, st))) return r;
     }
     {
       // the planes of the layer output are the next layer's xin; after layers 6 and 9 they are also DPT hooks
       // (dpt_head.py:108), so those layers write them straight into the hook buffers
       Planes xout = (l == 5) ? e->Hk6 : (l == 8) ? e->Hk9 : e->Pa;
-      Geom g; g.groups = 2; g.W = (int)R; g.Kc = 3072; g.N = 768;
-      Epi ep; ep.bias = bw.fc2.b; ep.res1 = e->Xd; ep.ldr1 = 768; ep.out = e->Xd; ep.ldo = 768;
-      ep.op = xout; ep.ldp = 768; ep.stats_out = e->Sa;
-      if ((r = e->gemm(pc, e->Hd, WP(bw.fc2.w), g, ep, st))) return r;
+      s3r_gemm_desc d = gemm_desc(e->Hd, WP(bw.fc2.w), 2, (int)R, 3072, 768);
+      d.bias = bw.fc2.b; d.res1 = e->Xd; d.ldr1 = 768; d.out_f32 = e->Xd; d.ldo = 768;
+      out_planes(d, xout, 768); d.stats_out = (float*)e->Sa;
+      if ((r = e->gemm(pc, d, st))) return r;
       xin = xout;
     }
     if (l < 11 && (r = qkv_launch(l + 1, xin))) return r;
@@ -676,14 +645,14 @@ int s3r_engine_keyheads(s3r_engine* e, const float* feat1, const float* feat2, f
   if ((r = launch_split(feat1, 1024, e->KH.hi, e->KH.lo, 1792, 0, R, 1024, 0, st))) return r;
   if ((r = launch_split(feat2, 1024, e->KH.hi + R * 1792, e->KH.lo + R * 1792, 1792, 0, R, 1024, 0, st))) return r;
   {
-    Geom g; g.groups = 2; g.W = (int)R; g.Kc = 1792; g.N = 1792;
-    Epi ep; ep.bias = e->w.key_fc1.b; ep.act = ACT_GELU; ep.op = e->KHh; ep.ldp = 1792;
-    if ((r = e->gemm(pc, e->KH, WP(e->w.key_fc1.w), g, ep, st))) return r;
+    s3r_gemm_desc d = gemm_desc(e->KH, WP(e->w.key_fc1.w), 2, (int)R, 1792, 1792);
+    d.bias = e->w.key_fc1.b; d.act = ACT_GELU; out_planes(d, e->KHh, 1792);
+    if ((r = e->gemm(pc, d, st))) return r;
   }
   {
-    Geom g; g.groups = 2; g.W = (int)R; g.Kc = 1792; g.N = 1024;
-    Epi ep; ep.bias = e->w.key_fc2.b; ep.out = e->KO; ep.ldo = 1024;
-    if ((r = e->gemm(pc, e->KHh, WP(e->w.key_fc2.w), g, ep, st))) return r;
+    s3r_gemm_desc d = gemm_desc(e->KHh, WP(e->w.key_fc2.w), 2, (int)R, 1792, 1024);
+    d.bias = e->w.key_fc2.b; d.out_f32 = e->KO; d.ldo = 1024;
+    if ((r = e->gemm(pc, d, st))) return r;
   }
   e->launches += 2;
   cudaMemcpyAsync(k1, e->KO, (size_t)R * 1024 * sizeof(float), cudaMemcpyDeviceToDevice, st);
@@ -708,21 +677,19 @@ int s3r_engine_heads(s3r_engine* e, float* pts, float* conf, void* stream) {
   const int h3 = (gh + 1) / 2, w3 = (gw + 1) / 2;
   int r;
   cudaStream_t cur = st;   // stream the next launch goes to
-  auto conv1x1 = [&](Planes A, int H, int W, int Cin, const s3r_lin& w, int Cout, Epi ep) {
-    Geom g; g.groups = 2; g.NB = B; g.H = H; g.W = W; g.Kc = Cin; g.N = Cout;
-    ep.bias = w.b;
-    return e->gemm(pc, A, WP(w.w), g, ep, cur);
+  // a 1x1 (taps 1) or 3x3 (taps 9) conv of both heads as groups; the caller adds the epilogue and runs it on `cur`
+  auto conv = [&](Planes A, int H, int W, int Cin, int taps, const s3r_lin& w, int Cout) {
+    s3r_gemm_desc g = gemm_desc(A, WP(w.w), 2, W, Cin, Cout);
+    g.nb = B; g.h = H; g.taps = taps; g.bias = w.b;
+    return g;
   };
-  auto conv3x3 = [&](Planes A, int H, int W, int Cin, const s3r_lin& w, int Cout, Epi ep) {
-    Geom g; g.groups = 2; g.NB = B; g.H = H; g.W = W; g.Kc = Cin; g.taps = 9; g.N = Cout;
-    ep.bias = w.b;
-    return e->gemm(pc, A, WP(w.w), g, ep, cur);
-  };
+  auto run = [&](const s3r_gemm_desc& g) { return e->gemm(pc, g, cur); };
   const int LH[4] = {4 * gh, 2 * gh, gh, h3}, LW[4] = {4 * gw, 2 * gw, gw, w3}, LC[4] = {96, 192, 384, 768};
   Planes Lin[4] = {e->A1, e->A2, e->A3, e->A4};
   auto layer_rn = [&](int i) {   // layer_rn (3x3, no bias): fp32 (residual) + relu planes (next conv's input)
-    Epi ep; ep.out = e->Lf[i]; ep.ldo = 256; ep.op = e->Lr[i]; ep.ldp = 256; ep.plane_relu = 1;
-    return conv3x3(Lin[i], LH[i], LW[i], LC[i], d.layer_rn[i], 256, ep);
+    s3r_gemm_desc g = conv(Lin[i], LH[i], LW[i], LC[i], 9, d.layer_rn[i], 256);
+    g.out_f32 = e->Lf[i]; g.ldo = 256; out_planes(g, e->Lr[i], 256); g.plane_relu = 1;
+    return run(g);
   };
   // --- act_postprocess (dpt_block.py:356-410) + layer_rn (:33-75): four chains, one per pyramid level, independent
   // until refinenet4.  They are small (2 .. 96 pixel tiles) and latency-bound, so levels 2-4 run on side streams
@@ -734,26 +701,26 @@ int s3r_engine_heads(s3r_engine* e, float* pts, float* conf, void* stream) {
     for (int i = 0; i < 3; ++i) cudaStreamWaitEvent(e->side[i], e->ev_fork, 0);
   }
   // level 1 (4gh x 4gw)
-  { Epi ep; ep.op = e->T1; ep.ldp = 96; if ((r = conv1x1(e->E0, gh, gw, 1024, d.act1_conv, 96, ep))) return r; }
-  { Epi ep; ep.epi = EPI_PIXSHUF; ep.ps_s = 4; ep.ps_cout = 96; ep.op = e->A1; ep.ldp = 96;
-    if ((r = conv1x1(e->T1, gh, gw, 96, d.act1_up, 16 * 96, ep))) return r; }
+  { auto g = conv(e->E0, gh, gw, 1024, 1, d.act1_conv, 96); out_planes(g, e->T1, 96); if ((r = run(g))) return r; }
+  { auto g = conv(e->T1, gh, gw, 96, 1, d.act1_up, 16 * 96); g.epi = EPI_PIXSHUF; g.ps_s = 4; g.ps_cout = 96;
+    out_planes(g, e->A1, 96); if ((r = run(g))) return r; }
   if ((r = layer_rn(0))) return r;
   // level 2 (2gh x 2gw)
   if (par) cur = e->side[0];
-  { Epi ep; ep.op = e->T2; ep.ldp = 192; if ((r = conv1x1(e->Hk6, gh, gw, 768, d.act2_conv, 192, ep))) return r; }
-  { Epi ep; ep.epi = EPI_PIXSHUF; ep.ps_s = 2; ep.ps_cout = 192; ep.op = e->A2; ep.ldp = 192;
-    if ((r = conv1x1(e->T2, gh, gw, 192, d.act2_up, 4 * 192, ep))) return r; }
+  { auto g = conv(e->Hk6, gh, gw, 768, 1, d.act2_conv, 192); out_planes(g, e->T2, 192); if ((r = run(g))) return r; }
+  { auto g = conv(e->T2, gh, gw, 192, 1, d.act2_up, 4 * 192); g.epi = EPI_PIXSHUF; g.ps_s = 2; g.ps_cout = 192;
+    out_planes(g, e->A2, 192); if ((r = run(g))) return r; }
   if ((r = layer_rn(1))) return r;
   // level 3 (gh x gw)
   if (par) cur = e->side[1];
-  { Epi ep; ep.op = e->A3; ep.ldp = 384; if ((r = conv1x1(e->Hk9, gh, gw, 768, d.act3_conv, 384, ep))) return r; }
+  { auto g = conv(e->Hk9, gh, gw, 768, 1, d.act3_conv, 384); out_planes(g, e->A3, 384); if ((r = run(g))) return r; }
   if ((r = layer_rn(2))) return r;
   // level 4 (gh/2 x gw/2): 1x1, then the stride-2 3x3 as im2col + GEMM
   if (par) cur = e->side[2];
-  { Epi ep; ep.op = e->T4; ep.ldp = 768; if ((r = conv1x1(e->Hk12, gh, gw, 768, d.act4_conv, 768, ep))) return r; }
+  { auto g = conv(e->Hk12, gh, gw, 768, 1, d.act4_conv, 768); out_planes(g, e->T4, 768); if ((r = run(g))) return r; }
   ++e->launches;
   if ((r = launch_im2col_3x3s2(e->T4.hi, e->T4.lo, 2 * B, gh, gw, 768, h3, w3, e->T4c.hi, e->T4c.lo, cur))) return r;
-  { Epi ep; ep.op = e->A4; ep.ldp = 768; if ((r = conv1x1(e->T4c, h3, w3, 9 * 768, d.act4_down, 768, ep))) return r; }
+  { auto g = conv(e->T4c, h3, w3, 9 * 768, 1, d.act4_down, 768); out_planes(g, e->A4, 768); if ((r = run(g))) return r; }
   if ((r = layer_rn(3))) return r;
   cur = st;
   if (par) {
@@ -771,18 +738,22 @@ int s3r_engine_heads(s3r_engine* e, float* pts, float* conf, void* stream) {
     Planes xin_r = e->Lr[lvl];       // ... and its relu planes
     if (path) {
       // output = path + resConfUnit1(layer):  conv1(relu(layer)) -> relu -> conv2 + layer + path
-      { Epi ep; ep.act = ACT_RELU; ep.op = e->Ra; ep.ldp = 256; if ((r = conv3x3(e->Lr[lvl], Hh, Ww, 256, f.rcu1.conv1, 256, ep))) return r; }
-      { Epi ep; ep.res1 = e->Lf[lvl]; ep.ldr1 = 256; ep.res2 = path; ep.ldr2 = 256; ep.out = e->Rf; ep.ldo = 256;
-        ep.op = e->Rfr; ep.ldp = 256; ep.plane_relu = 1;
-        if ((r = conv3x3(e->Ra, Hh, Ww, 256, f.rcu1.conv2, 256, ep))) return r; }
+      { auto g = conv(e->Lr[lvl], Hh, Ww, 256, 9, f.rcu1.conv1, 256); g.act = ACT_RELU; out_planes(g, e->Ra, 256);
+        if ((r = run(g))) return r; }
+      { auto g = conv(e->Ra, Hh, Ww, 256, 9, f.rcu1.conv2, 256);
+        g.res1 = e->Lf[lvl]; g.ldr1 = 256; g.res2 = path; g.ldr2 = 256; g.out_f32 = e->Rf; g.ldo = 256;
+        out_planes(g, e->Rfr, 256); g.plane_relu = 1;
+        if ((r = run(g))) return r; }
       xin = e->Rf;
       xin_r = e->Rfr;
     }
     // resConfUnit2
-    { Epi ep; ep.act = ACT_RELU; ep.op = e->Ra; ep.ldp = 256; if ((r = conv3x3(xin_r, Hh, Ww, 256, f.rcu2.conv1, 256, ep))) return r; }
-    { Epi ep; ep.res1 = xin; ep.ldr1 = 256; ep.op = e->Rb; ep.ldp = 256; if ((r = conv3x3(e->Ra, Hh, Ww, 256, f.rcu2.conv2, 256, ep))) return r; }
+    { auto g = conv(xin_r, Hh, Ww, 256, 9, f.rcu2.conv1, 256); g.act = ACT_RELU; out_planes(g, e->Ra, 256);
+      if ((r = run(g))) return r; }
+    { auto g = conv(e->Ra, Hh, Ww, 256, 9, f.rcu2.conv2, 256); g.res1 = xin; g.ldr1 = 256; out_planes(g, e->Rb, 256);
+      if ((r = run(g))) return r; }
     // out_conv at this resolution, then bilinear x2 (align_corners=True)
-    { Epi ep; ep.out = e->Rlow; ep.ldo = 256; if ((r = conv1x1(e->Rb, Hh, Ww, 256, f.out_conv, 256, ep))) return r; }
+    { auto g = conv(e->Rb, Hh, Ww, 256, 1, f.out_conv, 256); g.out_f32 = e->Rlow; g.ldo = 256; if ((r = run(g))) return r; }
     ++e->launches;
     if (lvl > 0) {
       // refinenet4's output is cropped to layers[2]'s size when the patch grid is odd (dpt_head.py:56)
@@ -793,11 +764,12 @@ int s3r_engine_heads(s3r_engine* e, float* pts, float* conf, void* stream) {
     }
   }
   // --- head (dpt_block.py:318-324): conv3x3 256->128, x2 bilinear, conv3x3 128->128, ReLU, conv1x1 128->4, postprocess
-  { Epi ep; ep.out = e->H0; ep.ldo = 128; if ((r = conv3x3(e->P1, 8 * gh, 8 * gw, 256, d.head0, 128, ep))) return r; }
+  { auto g = conv(e->P1, 8 * gh, 8 * gw, 256, 9, d.head0, 128); g.out_f32 = e->H0; g.ldo = 128; if ((r = run(g))) return r; }
   ++e->launches;
   if ((r = launch_upsample2x(e->H0, 2 * B, 8 * gh, 8 * gw, 128, nullptr, e->H0u.hi, e->H0u.lo, st))) return r;
-  { Epi ep; ep.epi = EPI_HEADTAIL; ep.act = ACT_RELU; ep.ht_w = d.head4_w; ep.ht_b = d.head4_b; ep.ht_pts = pts; ep.ht_conf = conf;
-    if ((r = conv3x3(e->H0u, 16 * gh, 16 * gw, 128, d.head2, 128, ep))) return r; }
+  { auto g = conv(e->H0u, 16 * gh, 16 * gw, 128, 9, d.head2, 128);
+    g.epi = EPI_HEADTAIL; g.act = ACT_RELU; g.ht_w = d.head4_w; g.ht_b = d.head4_b; g.ht_pts = pts; g.ht_conf = conf;
+    if ((r = run(g))) return r; }
   pc.end();
   return 0;
 }
@@ -857,17 +829,17 @@ int s3r_engine_value(s3r_engine* e, const float* pts3d, const float* feat_k1, in
     if ((r = launch_im2col_patch16(pts3d, (long long)e->H * e->W * 3, 1, tr ? spx : srow, tr ? srow : spx, B,
                                    tr ? e->gw : e->gh, tr ? e->gh : e->gw, e->Pim.hi, e->Pim.lo, st)))
       return r;
-    Geom g; g.W = rows; g.Kc = 768; g.N = 1024;
-    Epi ep; ep.bias = e->w.pos_patch_embed.b; ep.out = e->Xv; ep.ldo = 1024;
-    ep.op = e->P; ep.ldp = 1024; ep.stats_out = e->St1;
-    if ((r = e->gemm(pc, e->Pim, WP(e->w.pos_patch_embed.w), g, ep, st))) return r;
+    s3r_gemm_desc d = gemm_desc(e->Pim, WP(e->w.pos_patch_embed.w), 1, rows, 768, 1024);
+    d.bias = e->w.pos_patch_embed.b; d.out_f32 = e->Xv; d.ldo = 1024;
+    out_planes(d, e->P, 1024); d.stats_out = (float*)e->St1;
+    if ((r = e->gemm(pc, d, st))) return r;
   }
   if ((r = e->vit_blocks(pc, e->w.val, 6, vc, B, rope, e->Xv, st, tr ? e->pos_t : e->pos))) return r;
   if ((r = e->ln(e->Xv, e->w.value_norm, 0, 0, 1e-6f, rows, D, nullptr, 0, e->Pv, D, 0, 0, st))) return r;
   {
-    Geom g; g.W = rows; g.Kc = D; g.N = 1024;
-    Epi ep; ep.bias = e->w.value_out.b; ep.res1 = feat_k1; ep.ldr1 = 1024; ep.out = out; ep.ldo = 1024;
-    if ((r = e->gemm(pc, e->Pv, WP(e->w.value_out.w), g, ep, st))) return r;
+    s3r_gemm_desc d = gemm_desc(e->Pv, WP(e->w.value_out.w), 1, rows, D, 1024);
+    d.bias = e->w.value_out.b; d.res1 = feat_k1; d.ldr1 = 1024; d.out_f32 = out; d.ldo = 1024;
+    if ((r = e->gemm(pc, d, st))) return r;
   }
   pc.end();
   return 0;
@@ -906,10 +878,11 @@ int memory_read_slots(s3r_engine* e, const s3r_bank* bank, const SlotInts& lens,
   int r;
   if ((r = e->ln(feat, e->w.norm_q, 0, 0, 1e-5f, R, 1024, nullptr, 0, e->Qn, 1024, 0, 0, st))) return r;
   {  // S = LN_q(feat) . LN_k(mem_k)^T, one group per slot (each sequence has its own bank), Mmax columns in every group
-    Geom g; g.groups = B; g.W = N; g.Kc = 1024; g.N = Mmax; g.b_group_rows = cap; g.b_static = 0;
-    Epi ep; ep.out = e->Sm; ep.ldo = e->mem_cap;
     Planes Kn; Kn.hi = (__nv_bfloat16*)bank->kn_hi; Kn.lo = (__nv_bfloat16*)bank->kn_lo;
-    if ((r = e->gemm(pc, e->Qn, Kn, g, ep, st))) return r;
+    s3r_gemm_desc d = gemm_desc(e->Qn, Kn, B, N, 1024, Mmax);
+    d.b_group_rows = cap; d.b_static = 0;
+    d.out_f32 = e->Sm; d.ldo = e->mem_cap;
+    if ((r = e->gemm(pc, d, st))) return r;
   }
   e->launches += 3;
   if ((r = launch_mem_softmax(e->Sm, e->mem_cap, R, N, lens, Mmax, Mpad, 1.0f / 32.0f, thresh, e->Pm.hi, e->Pm.lo, e->mem_cap,
@@ -919,10 +892,11 @@ int memory_read_slots(s3r_engine* e, const s3r_bank* bank, const SlotInts& lens,
   if ((r = launch_mem_colsum(e->Pm.hi, e->Pm.lo, e->mem_cap, B, N, lens, Mmax, bank->attn, cap, e->Sm, e->mem_cap, st)))
     return r;
   {  // out = attn . LN_v(mem_v) + feat; P is zero past each slot's length, where V_n^T must only be finite
-    Geom g; g.groups = B; g.W = N; g.Kc = Mmax; g.N = 1024; g.lda = e->mem_cap; g.ldb = cap; g.b_group_rows = 1024; g.b_static = 0;
-    Epi ep; ep.res1 = feat; ep.ldr1 = 1024; ep.out = out; ep.ldo = 1024;
     Planes Vt; Vt.hi = (__nv_bfloat16*)bank->vnt_hi; Vt.lo = (__nv_bfloat16*)bank->vnt_lo;
-    if ((r = e->gemm(pc, e->Pm, Vt, g, ep, st))) return r;
+    s3r_gemm_desc d = gemm_desc(e->Pm, Vt, B, N, Mmax, 1024);
+    d.lda = e->mem_cap; d.ldb = cap; d.b_group_rows = 1024; d.b_static = 0;
+    d.res1 = feat; d.ldr1 = 1024; d.out_f32 = out; d.ldo = 1024;
+    if ((r = e->gemm(pc, d, st))) return r;
   }
   pc.end();
   return 0;

@@ -21,6 +21,8 @@
 //                 producer keeps filling the ring for the next tile meanwhile.
 #include "gemm.cuh"
 
+#include "../../include/spann3r_b200.h"
+
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
@@ -399,15 +401,6 @@ static int next_pow2(int x) {
   return p;
 }
 
-Options& options() {
-  static Options o = [] {
-    Options x;
-    if (const char* e = getenv("S3R_PREFETCH_B")) x.prefetch_b = atoi(e);
-    return x;
-  }();
-  return o;
-}
-
 static int g_num_sms[64] = {};   // per device ordinal
 int num_sms() {
   int dev = 0;
@@ -424,31 +417,27 @@ int num_sms() {
 // waves = ceil(tiles / SMs) for the persistent static schedule and 24 / 28 / 32 KB staged per k-block at BN = 64 / 96 / 128
 // (split planes; the one-product ring halves every figure, which keeps the ranking).  Ties go to the wider tile.  A
 // 64-row warpgroup holds a 64 x BN fp32 accumulator in registers next to the epilogue's working set, so 128 is the widest
-// tile; wider requests (force_bn 256, and 2064 / 2128 / 2256, the tile widths of CTA-pair kernels on other architectures)
-// run at the nearest width the kernel has.  col_align (0 = none) is a column no tile may straddle: a_swap's swap_col0,
-// since the producer and the epilogue pick the swapped A group once per tile; a width that does not divide it is never
-// chosen, and rejected when forced.
+// tile.  col_align (0 = none) is a column no tile may straddle: a_swap's swap_col0, since the producer and the epilogue
+// pick the swapped A group once per tile; a width that does not divide it is never chosen, and rejected when forced.
 int gemm_choose_bn(long long m_tiles, int N, int sms, int col_align, int force_bn) {
   auto fits = [&](int bn) { return col_align == 0 || col_align % bn == 0; };
   auto cost = [&](int bn, double kb) {
     const long long tiles = m_tiles * ((N + bn - 1) / bn);
     return (double)((tiles + sms - 1) / sms) * kb;
   };
-  const int fb = force_bn >= 2000 ? force_bn - 2000 : force_bn == 1128 ? 128 : force_bn;
-  if (fb > 0) {
-    if (fb != 64 && fb != 128 && fb != 256 && !(fb == 96 && force_bn == 96)) {
-      set_error("gemm_plan_init: force_bn %d (64, 96, 128, 256, 1128, 2064, 2128, 2256 or 0)", force_bn);
+  if (force_bn != 0) {
+    if (force_bn != 64 && force_bn != 96 && force_bn != 128) {
+      set_error("gemm planner: force_bn %d (64, 96, 128 or 0)", force_bn);
       return -1;
     }
-    const int bn = fb > 128 ? 128 : fb;
-    if (!fits(bn)) {
-      set_error("gemm_plan_init: force_bn %d: a %d-wide tile would straddle swap_col0 = %d", force_bn, bn, col_align);
+    if (!fits(force_bn)) {
+      set_error("gemm planner: force_bn %d: the tile would straddle swap_col0 = %d", force_bn, col_align);
       return -1;
     }
-    return bn;
+    return force_bn;
   }
   if (col_align % 64 != 0) {
-    set_error("gemm_plan_init: swap_col0 = %d is not a multiple of 64 (no tile width fits it)", col_align);
+    set_error("gemm planner: swap_col0 = %d is not a multiple of 64 (no tile width fits it)", col_align);
     return -1;
   }
   int bn = 64;
@@ -461,25 +450,157 @@ int gemm_choose_bn(long long m_tiles, int N, int sms, int col_align, int force_b
   return bn;
 }
 
-int gemm_plan_init(GemmPlan* plan, const __nv_bfloat16* a_hi, const __nv_bfloat16* a_lo,
-                   const __nv_bfloat16* b_hi, const __nv_bfloat16* b_lo, int groups, int NB, int H, int W, int Kc,
-                   int taps, int N, int force_bn, long long lda, long long ldb, long long b_group_rows, int precision,
-                   int col_align) {
+// Row strides and column offsets of the epilogue's fp32 (float4) and planes (uint2) accesses: multiples of 4 elements
+// that fit the kernel's int fields.
+static bool bad_ld(int64_t ld) { return ld < 0 || ld > INT32_MAX || ld % 4 != 0; }
+
+// Every descriptor rule the producer and the epilogue rely on, checked before anything touches the driver.
+static int check_desc(const s3r_gemm_desc& d) {
+  if (d.precision != GEMM_SPLIT && d.precision != GEMM_BF16) {
+    set_error("s3r_gemm: precision=%d must be 0 (split bf16) or 1 (one bf16 product)", d.precision);
+    return -1;
+  }
+  if (d.precision == GEMM_BF16 && d.epi == S3R_EPI_HEADTAIL) {
+    set_error("s3r_gemm: precision=1 does not support EPI_HEADTAIL (the DPT head tail is split-only)");
+    return -1;
+  }
+  if (d.taps != 1 && d.taps != 9) {
+    set_error("s3r_gemm: taps=%d must be 1 or 9", d.taps);
+    return -1;
+  }
+  if (d.taps == 9 && d.kc % 8 != 0) {
+    set_error("s3r_gemm: kc=%d of a 3x3 conv must be a multiple of 8 (16-byte tap stride)", d.kc);
+    return -1;
+  }
+  // TMA row strides: multiples of 16 bytes
+  const struct { const char* name; int64_t v; } strides[2] = {{"lda", d.lda ? d.lda : d.kc},
+                                                              {"ldb", d.ldb ? d.ldb : (int64_t)d.kc * d.taps}};
+  for (const auto& s : strides)
+    if (s.v < 0 || s.v % 8 != 0) {
+      set_error("s3r_gemm: %s=%lld must be a non-negative multiple of 8 (0 = dense)", s.name, (long long)s.v);
+      return -1;
+    }
+  if (d.b_group_rows < 0 || d.b_group_rows > INT32_MAX) {
+    set_error("s3r_gemm: b_group_rows=%lld must be in [0, 2^31) (0 = n)", (long long)d.b_group_rows);
+    return -1;
+  }
+  // the epilogue stores whole 32-column chunks; past n that is only harmless in a bare fp32 output wide enough for them
+  const bool chunk_tail_ok = d.epi == S3R_EPI_PLAIN && !d.out_hi && !d.stats_out && !d.res1 && !d.res2 && d.out_f32 &&
+                             d.ldo >= (d.n + 31) / 32 * 32;
+  if (d.n <= 0 || (d.n % 32 != 0 && !chunk_tail_ok)) {
+    set_error("s3r_gemm: n=%d must be a positive multiple of 32 (the epilogue stores whole 32-column chunks; only a bare "
+              "out_f32 with ldo >= n rounded up to 32 may take the tail)", d.n);
+    return -1;
+  }
+  if (d.epi == S3R_EPI_HEADTAIL && d.n != 128) {
+    set_error("s3r_gemm: EPI_HEADTAIL needs n == 128");
+    return -1;
+  }
+  if (d.epi == S3R_EPI_PIXSHUF && (d.ps_s <= 0 || d.ps_cout % 32 != 0 || d.n != d.ps_s * d.ps_s * d.ps_cout)) {
+    set_error("s3r_gemm: EPI_PIXSHUF needs n == s*s*cout and cout %% 32 == 0");
+    return -1;
+  }
+  const struct { const char* name; bool used; int64_t v; } lds[5] = {
+      {"ldr1", d.res1 != nullptr, d.ldr1}, {"ldr2", d.res2 != nullptr, d.ldr2}, {"ldo", d.out_f32 != nullptr, d.ldo},
+      {"ldp", d.out_hi != nullptr, d.ldp}, {"plane_col0", d.out_hi != nullptr, d.plane_col0}};
+  for (const auto& l : lds)
+    if (l.used && bad_ld(l.v)) {
+      set_error("s3r_gemm: %s=%lld must be a non-negative multiple of 4 below 2^31 (vector accesses)", l.name,
+                (long long)l.v);
+      return -1;
+    }
+  if (d.epi == S3R_EPI_QKV) {
+    if (d.q_c <= 0 || d.q_c % 64 != 0 || d.h != 1 || d.q_ntok <= 0 || d.w != d.q_nb * d.q_ntok) {
+      set_error("s3r_gemm: EPI_QKV needs q_c %% 64 == 0, h == 1, w == q_nb*q_ntok");
+      return -1;
+    }
+    if (d.n % d.q_c != 0) {
+      set_error("s3r_gemm: EPI_QKV n=%d must be a multiple of q_c=%d", d.n, d.q_c);
+      return -1;
+    }
+    if (d.q_role_base < 0 || d.q_role_base + d.n / d.q_c > 5) {
+      set_error("s3r_gemm: EPI_QKV q_role_base=%d + n/q_c=%d must stay within the 5 roles", d.q_role_base,
+                d.n / d.q_c);
+      return -1;
+    }
+    if (d.q_ntok_pad < d.q_ntok || d.q_ntok_pad % 4 != 0) {
+      set_error("s3r_gemm: EPI_QKV q_ntok_pad=%d must be >= q_ntok=%d and a multiple of 4", d.q_ntok_pad, d.q_ntok);
+      return -1;
+    }
+    static const char* const kRoleOut[5] = {"q_out", "k_out", "vt_out", "k2_out", "vt2_out"};
+    const float* const role_out[5] = {d.q_out, d.k_out, d.vt_out, d.k2_out, d.vt2_out};
+    for (int role = d.q_role_base; role < d.q_role_base + d.n / d.q_c; ++role)
+      if (!role_out[role]) {
+        set_error("s3r_gemm: EPI_QKV role %d is written but %s is NULL", role, kRoleOut[role]);
+        return -1;
+      }
+    if (d.q_rope && (!d.q_pos || !d.q_cs)) {
+      set_error("s3r_gemm: EPI_QKV with q_rope needs %s", d.q_pos ? "q_cs" : "q_pos");
+      return -1;
+    }
+  }
+  if (d.ln_stats) {
+    if (d.ln_cs == nullptr || d.ln_np * 32 != d.kc || d.taps != 1 || d.epi == S3R_EPI_PIXSHUF) {
+      set_error("s3r_gemm: folded LayerNorm needs ln_cs, ln_np == kc/32, taps == 1 and a non-PIXSHUF epilogue");
+      return -1;
+    }
+    if (d.ln_np < 2 || d.ln_np > 32 || d.ln_np % 2 != 0) {
+      set_error("s3r_gemm: folded LayerNorm needs an even ln_np in [2, 32] (kc %% 64 == 0, kc <= 1024), got ln_np=%d",
+                d.ln_np);
+      return -1;
+    }
+  }
+  if (d.swap_col0 % 256 != 0) {
+    set_error("s3r_gemm: swap_col0 must be a multiple of 256");
+    return -1;
+  }
+  if (d.stats_out && d.epi != S3R_EPI_PLAIN) {
+    set_error("s3r_gemm: stats_out needs EPI_PLAIN");
+    return -1;
+  }
+  return 0;
+}
+
+void gemm_set_epilogue(const s3r_gemm_desc& d, GemmArgs& a) {
+  a.epi = d.epi; a.act = d.act; a.plane_relu = d.plane_relu;
+  a.bias = d.bias;
+  a.res1 = d.res1; a.ldr1 = (int)d.ldr1;
+  a.res2 = d.res2; a.ldr2 = (int)d.ldr2;
+  a.out_f32 = d.out_f32; a.ldo = (int)d.ldo;
+  a.out_hi = (__nv_bfloat16*)d.out_hi; a.out_lo = (__nv_bfloat16*)d.out_lo; a.ldp = (int)d.ldp;
+  a.plane_col0 = d.plane_col0;
+  if (d.epi == S3R_EPI_PIXSHUF) {
+    a.ps_s = d.ps_s; a.ps_cout = d.ps_cout;
+    a.out_group_rows = (long long)d.nb * d.h * d.ps_s * d.w * d.ps_s;
+  }
+  if (d.epi == S3R_EPI_QKV) {
+    a.q_C = d.q_c; a.q_role_base = d.q_role_base; a.q_ntok = d.q_ntok; a.q_ntok_pad = d.q_ntok_pad;
+    a.q_rope = d.q_rope; a.q_nb = d.q_nb; a.q_pos = d.q_pos;
+    a.q_cs = reinterpret_cast<const float2*>(d.q_cs);
+    a.q_out = d.q_out; a.k_out = d.k_out; a.vt_out = d.vt_out; a.q_scale = d.q_scale;
+    a.k2_out = d.k2_out; a.vt2_out = d.vt2_out;
+  }
+  if (d.epi == S3R_EPI_HEADTAIL) {
+    a.ht_w = d.ht_w; a.ht_b = d.ht_b; a.ht_pts = d.ht_pts; a.ht_conf = d.ht_conf;
+  }
+  if (d.ln_stats) {
+    a.ln_stats = reinterpret_cast<const float2*>(d.ln_stats); a.ln_np = d.ln_np; a.ln_eps = d.ln_eps; a.ln_cs = d.ln_cs;
+  }
+  a.a_swap = d.a_swap ? 1 : 0;
+  a.swap_col0 = d.swap_col0;
+  a.stats_out = reinterpret_cast<float2*>(d.stats_out);
+  a.trace = reinterpret_cast<unsigned long long*>(d.trace);
+  a.b_static = d.b_static ? 1 : 0;
+}
+
+int gemm_plan(const s3r_gemm_desc& d, GemmPlan* plan) {
   memset(plan, 0, sizeof(*plan));
-  if (precision != GEMM_SPLIT && precision != GEMM_BF16) {
-    set_error("gemm_plan_init: precision %d (0 = split bf16, 1 = one bf16 product)", precision);
-    return -1;
-  }
-  plan->precision = precision;
+  if (int r = check_desc(d)) return r;
+  const int groups = d.groups, NB = d.nb, H = d.h, W = d.w, Kc = d.kc, taps = d.taps, N = d.n;
+  const long long lda = d.lda ? d.lda : Kc, ldb = d.ldb ? d.ldb : (long long)Kc * taps;
+  const long long b_group_rows = d.b_group_rows ? d.b_group_rows : N;
+  plan->precision = d.precision;
   GemmArgs& a = plan->args;
-  if (lda == 0) lda = Kc;
-  if (ldb == 0) ldb = (long long)Kc * taps;
-  if (b_group_rows == 0) b_group_rows = N;
-  if (lda % 8 != 0 || ldb % 8 != 0 || (taps != 1 && taps != 9) || (taps == 9 && Kc % 8 != 0)) {
-    set_error("gemm_plan_init: unsupported shape Kc=%d N=%d taps=%d lda=%lld ldb=%lld (row strides must be multiples "
-              "of 8 elements, taps in {1,9})", Kc, N, taps, lda, ldb);
-    return -1;
-  }
   a.b_group_rows = (int)b_group_rows;
   a.W = W; a.H = H; a.NB = NB; a.N = N; a.Kc = Kc; a.taps = taps;
   a.kpt = (Kc + BK - 1) / BK;
@@ -489,7 +610,9 @@ int gemm_plan_init(GemmPlan* plan, const __nv_bfloat16* a_hi, const __nv_bfloat1
   a.tiles_h = (H + a.bh - 1) / a.bh;
   a.out_group_rows = (long long)NB * H * W;
   const long long m_tiles = (long long)a.tiles_w * a.tiles_h * NB * groups;
-  const int bn = gemm_choose_bn(m_tiles, N, num_sms(), col_align, force_bn);
+  // the DPT head tail's hand-over pairs the two column halves of a 128-wide tile (launch_epi)
+  const int bn = gemm_choose_bn(m_tiles, N, num_sms(), d.a_swap ? d.swap_col0 : 0,
+                                d.epi == S3R_EPI_HEADTAIL ? 128 : d.force_bn);
   if (bn < 0) return -1;
   plan->bn = bn;
 
@@ -499,9 +622,9 @@ int gemm_plan_init(GemmPlan* plan, const __nv_bfloat16* a_hi, const __nv_bfloat1
     uint64_t str[3] = {(uint64_t)lda * esz, (uint64_t)lda * W * esz, (uint64_t)lda * W * H * esz};
     uint32_t box[4] = {(uint32_t)BK, (uint32_t)a.bw, (uint32_t)a.bh, 1};
     int r;
-    if ((r = encode_tmap(&a.tmA_hi, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, a_hi, dims, str, box, kSwizzle))) return r;
-    if (precision == GEMM_SPLIT &&
-        (r = encode_tmap(&a.tmA_lo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, a_lo, dims, str, box, kSwizzle)))
+    if ((r = encode_tmap(&a.tmA_hi, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, d.a_hi, dims, str, box, kSwizzle))) return r;
+    if (d.precision == GEMM_SPLIT &&
+        (r = encode_tmap(&a.tmA_lo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, d.a_lo, dims, str, box, kSwizzle)))
       return r;
   }
   {
@@ -510,9 +633,9 @@ int gemm_plan_init(GemmPlan* plan, const __nv_bfloat16* a_hi, const __nv_bfloat1
     uint64_t str[2] = {(uint64_t)(taps == 1 ? ldb : Kc) * esz, (uint64_t)ldb * esz};
     uint32_t box[3] = {(uint32_t)BK, 1, (uint32_t)bn};
     int r;
-    if ((r = encode_tmap(&a.tmB_hi, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, b_hi, dims, str, box, kSwizzle))) return r;
-    if (precision == GEMM_SPLIT &&
-        (r = encode_tmap(&a.tmB_lo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, b_lo, dims, str, box, kSwizzle)))
+    if ((r = encode_tmap(&a.tmB_hi, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, d.b_hi, dims, str, box, kSwizzle))) return r;
+    if (d.precision == GEMM_SPLIT &&
+        (r = encode_tmap(&a.tmB_lo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, d.b_lo, dims, str, box, kSwizzle)))
       return r;
   }
   const long long n_tiles = (N + bn - 1) / bn;
@@ -520,6 +643,7 @@ int gemm_plan_init(GemmPlan* plan, const __nv_bfloat16* a_hi, const __nv_bfloat1
   a.groups = groups;
   plan->grid = dim3((unsigned)((total < num_sms()) ? total : num_sms()), 1, 1);  // persistent: <= 1 CTA per SM
   plan->flops = 2.0 * (double)NB * H * W * groups * (double)N * (double)Kc * taps;
+  gemm_set_epilogue(d, a);
   return 0;
 }
 

@@ -5,6 +5,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+struct s3r_gemm_desc;   // include/spann3r_b200.h
+
 namespace s3r {
 
 enum EpiMode : int {
@@ -77,34 +79,23 @@ struct GemmPlan {
   dim3 grid;
   int bn;          // 64 / 96 / 128
   int precision;   // GemmPrecision
-  int b_static;    // engine: B is a packed weight and the prefetch option was on when the plan was built
   double flops;    // algorithmic 2*M*N*K (all groups), for roofline accounting
 };
 
-// Encodes the tensor maps (four; two -- the hi planes -- at GEMM_BF16, where a_lo / b_lo may be null) and picks the tile
-// shape.  Returns 0 or a negative error.
-// lda / ldb: row strides (elements) of A pixels / B rows (0 = dense: Kc resp. taps*Kc);
-// b_group_rows: rows between consecutive groups of B (0 = N).
-// force_bn: 0 = planner's choice; 64 / 96 / 128 = that tile width; 256, 1128, 2064, 2128, 2256 = the nearest width the
-// kernel has (128, 128, 64, 128, 128).
-// col_align: a_swap's swap_col0 when only the columns from there on are swapped (0 = none): no tile may straddle it.
-int gemm_plan_init(GemmPlan* plan,
-                   const __nv_bfloat16* a_hi, const __nv_bfloat16* a_lo,   // [G*NB, H, W, Kc]
-                   const __nv_bfloat16* b_hi, const __nv_bfloat16* b_lo,   // [G*N, taps, Kc]
-                   int groups, int NB, int H, int W, int Kc, int taps, int N, int force_bn = 0,
-                   long long lda = 0, long long ldb = 0, long long b_group_rows = 0, int precision = GEMM_SPLIT,
-                   int col_align = 0);
+// Checks every rule of s3r_gemm_desc (include/spann3r_b200.h) before the driver is touched, picks the tile width,
+// encodes the tensor maps (four; two -- the hi planes -- at GEMM_BF16, where a_lo / b_lo may be null) and fills the
+// epilogue.  Returns 0 or a negative error with last_error() naming the offending field.
+int gemm_plan(const s3r_gemm_desc& d, GemmPlan* plan);
+// Writes the epilogue fields of `a` from `d` (the only function that does): a plan replayed with new output, residual or
+// statistics buffers of the same shapes.  No validation, no driver call.
+void gemm_set_epilogue(const s3r_gemm_desc& d, GemmArgs& a);
 // The planner's tile width for m_tiles 128-row tiles x N columns on `sms` SMs (pure host function; gemm.cu explains the
-// rule).  Returns 64, 96 or 128, or -1 with last_error() set.
+// rule).  force_bn: 0 = planner's choice, 64 / 96 / 128 = that width.  col_align: a_swap's swap_col0 when only the
+// columns from there on are swapped (0 = none): no tile may straddle it.  Returns 64, 96 or 128, or -1 with
+// last_error() set.
 int gemm_choose_bn(long long m_tiles, int N, int sms, int col_align, int force_bn);
 int gemm_launch(const GemmPlan& plan, cudaStream_t stream);
 
-// Tuning knobs of the tile planner / producers (s3r_set_option): read when a plan is BUILT, so two engines of one
-// process can be planned under different settings and timed alternately (tools/ab_inproc.py).
-struct Options {
-  int prefetch_b = 1;   // stage the first weight tiles before griddepcontrol.wait
-};
-Options& options();
 int num_sms();
 
 int encode_tmap(CUtensorMap* out, CUtensorMapDataType dt, int rank, const void* base, const uint64_t* dims,

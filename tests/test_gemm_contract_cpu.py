@@ -70,6 +70,19 @@ def test_n_must_be_whole_32_column_chunks(L, n):
     _rejects(L, d, f"n={n}")
 
 
+@pytest.mark.parametrize("change", [dict(ldo=96), dict(res1=_p(6)), dict(res2=_p(7)), dict(out_hi=_p(9)),
+                                    dict(stats_out=_p(13))])
+def test_only_a_bare_wide_enough_fp32_output_takes_a_chunk_tail(L, change):
+    """The memory read's scores (n = bank length, out_f32 alone, ldo >= n rounded up to 32) are the one launch whose n
+    is not whole chunks: anything else the tail chunk would touch past n rejects it."""
+    d = _plain(L)
+    d.n, d.ln_stats, d.res1, d.res2, d.out_hi, d.out_lo, d.ldo = 100, None, None, None, None, None, 128
+    assert L.lib().s3r_gemm_tile_n(C.byref(d)) != -1, L.lib().s3r_last_error()   # accepted (-3 without a driver)
+    for k, v in change.items():
+        setattr(d, k, v)
+    _rejects(L, d, "n=100")
+
+
 @pytest.mark.parametrize("field,value", [
     ("ldr1", 770), ("ldr2", 6), ("ldo", 770), ("ldp", 2), ("plane_col0", 2), ("ldo", 1 << 32), ("ldp", -768),
 ])
@@ -77,6 +90,22 @@ def test_strides_and_offsets_are_vector_aligned_ints(L, field, value):
     d = _plain(L)
     setattr(d, field, value)
     _rejects(L, d, field)
+
+
+@pytest.mark.parametrize("field,value", [
+    ("lda", 772), ("lda", -768), ("ldb", 6), ("ldb", -8), ("b_group_rows", -1), ("b_group_rows", 1 << 31),
+    ("kc", 100),   # the dense lda / ldb of kc = 100 are not 16-byte strides
+    ("taps", 3),
+])
+def test_operand_layout_is_tma_aligned(L, field, value):
+    """lda / ldb are TMA row strides (multiples of 16 bytes); b_group_rows fits the kernel's int; taps is 1 or 9."""
+    d = _plain(L)
+    d.ln_stats = None
+    d.lda, d.ldb, d.b_group_rows, d.b_static = 1024, 776, 800, 1   # a memory-read-like layout is accepted
+    assert L.lib().s3r_gemm_tile_n(C.byref(d)) != -1, L.lib().s3r_last_error()
+    d.lda, d.ldb = 0, 0
+    setattr(d, field, value)
+    _rejects(L, d, {"kc": "lda"}.get(field, field))
 
 
 @pytest.mark.parametrize("change,field", [

@@ -160,6 +160,61 @@ def test_gemm_groups_a_swap(L, geom, swap_col0, force_bn):
     _gemm(L, *geom, force_bn=force_bn, a_swap=True, swap_col0=swap_col0, seed=7 + swap_col0)
 
 
+MEMORY_READ = {   # G (slots), rows, Kc, N, lda, ldb, b_group_rows, res1
+    # out = P V^T + feat: P rows mem_cap apart, Kc = bank length; V^T [1024, cap] per slot
+    "value": (2, 77, 196, 96, 264, 200, 128, True),
+    # S = Q K^T: each slot's keys cap rows apart, N = bank length (the chunk tail past N is unspecified)
+    "score": (2, 77, 96, 100, 0, 0, 136, False),
+}
+
+
+@pytest.mark.parametrize("precision", [0, 1])
+@pytest.mark.parametrize("layout", list(MEMORY_READ))
+def test_gemm_memory_read_layout(L, layout, precision):
+    """lda, ldb and b_group_rows as the engine's memory read sets them, with B staged before the dependency wait
+    (b_static = 1).  The operands sit in NaN-padded buffers: a read of the padding would poison the result."""
+    G, rows, Kc, N, lda, ldb, bgr, res = MEMORY_READ[layout]
+    gen = E.pick_gen(Kc)
+    q = gen.q
+    a = E.planes((G, 1, rows, Kc), gen, 51, "cuda")
+    b = E.planes((G * N, Kc), gen, 52, "cuda")
+    bias = E.ints((G * N,), E.EPI_MAX, q, 53, "cuda")
+    r1 = E.ints((G * rows, N), E.EPI_MAX, q, 54, "cuda") if res else None
+
+    def b_rows(t):   # [G * b_group_rows, ldb]: group g's N rows from row g * b_group_rows on, NaN elsewhere
+        buf = torch.full((G * bgr + 2, ldb or Kc), float("nan"), dtype=t.dtype, device="cuda")
+        for g in range(G):
+            buf[g * bgr:g * bgr + N, :Kc] = t[g * N:(g + 1) * N]
+        return buf
+
+    ap = [_strided(t.reshape(G * rows, Kc), lda or Kc) for t in a[:1 + (precision == 0)]]
+    bp = [b_rows(t) for t in b[:1 + (precision == 0)]]
+    bg = _guarded(bias)
+    d = L.GemmDesc()
+    d.a_hi, d.b_hi = ap[0].data_ptr(), bp[0].data_ptr()
+    d.a_lo, d.b_lo = (ap[1].data_ptr(), bp[1].data_ptr()) if precision == 0 else (None, None)
+    d.groups, d.nb, d.h, d.w, d.kc, d.taps, d.n, d.precision = G, 1, 1, rows, Kc, 1, N, precision
+    d.lda, d.ldb, d.b_group_rows, d.b_static = lda, ldb, bgr, 1
+    d.epi, d.bias = L.EPI_PLAIN, bg.data_ptr()
+    ldo = N + 32
+    out = torch.full((G * rows + 3, ldo), SENT, device="cuda")
+    d.out_f32, d.ldo = out.data_ptr(), ldo
+    if r1 is not None:
+        rg = _strided(r1, N + 8)
+        d.res1, d.ldr1 = rg.data_ptr(), N + 8
+    L.gemm(d)
+    torch.cuda.synchronize()
+
+    acc = E.gemm_ref(a, b, G, 1, precision).reshape(G * rows, N)
+    bias_rows = bias.view(G, 1, N).expand(G, rows, N).reshape(G * rows, N)
+    terms = E.gemm_ref(a, b, G, 1, precision, terms=True).reshape(G * rows, N) + bias_rows.double().abs()
+    if r1 is not None:
+        terms = terms + r1.double().abs()
+    _premise(terms, q)
+    out[:G * rows, N:(N + 31) // 32 * 32] = SENT   # the last chunk's columns past N hold unspecified values
+    _check_window("out_f32", out, E.plain_epilogue(acc, bias_rows, False, r1).float(), tiles=E.tile_ids(G, 1, rows, N))
+
+
 EPILOGUES = {
     "bare": dict(bias=False, res1=False),
     "bias": dict(res1=False),

@@ -1,4 +1,4 @@
-"""The GEMM tile planner without a GPU: s3r_gemm_plan_bn is the rule gemm_plan_init applies (waves x bytes staged per
+"""The GEMM tile planner without a GPU: s3r_gemm_plan_bn is the rule gemm_plan applies (waves x bytes staged per
 k-block, 24 / 28 / 32 KB at 64 / 96 / 128 columns), checked on the launches of a 512 x 384 sequence at 132 SMs, and the
 rule that no tile may straddle a_swap's swap_col0."""
 import ctypes as C
@@ -83,9 +83,11 @@ def test_forced_width_that_straddles_swap_col0_is_rejected(L):
     assert b"swap_col0" in L.lib().s3r_last_error()
 
 
-def test_forced_widths(L):
-    for fb, bn in [(64, 64), (96, 96), (128, 128), (256, 128), (1128, 128), (2064, 64), (2128, 128), (2256, 128)]:
-        assert _plan(L, 12, 768, force_bn=fb) == bn
-    for fb in (32, 2096):
+def test_forced_widths_are_the_kernels_own(L):
+    """force_bn takes 64, 96 or 128 (0 = the planner's choice); any other value, the CTA-pair widths of other
+    architectures included, is rejected."""
+    for fb in (64, 96, 128):
+        assert _plan(L, 12, 768, force_bn=fb) == fb
+    for fb in (32, 2096, 256, 1128, 2064, 2128, 2256):
         assert _plan(L, 12, 768, force_bn=fb) == -1
         assert b"force_bn" in L.lib().s3r_last_error()

@@ -383,11 +383,7 @@ def test_decoder_takes_the_grid_from_the_positions(monkeypatch):
         m.dust3r._decoder(torch.zeros(1, 20, 1024), pos, torch.zeros(1, 20, 1024), pos)
 
 
-def test_set_option_validates_names_without_a_device():
-    """s3r_set_option: planner knobs read when an engine builds its plans; unknown names are refused with a message."""
+def test_dropout_mask_rejects_a_null_output_without_a_device():
     from spann3r_b200 import _lib
     L = _lib.lib()
-    assert L.s3r_set_option(b"prefetch_b", 0) == 0 and L.s3r_set_option(b"prefetch_b", 1) == 0
-    assert L.s3r_set_option(b"no_such_knob", 1) == -1 and b"no_such_knob" in L.s3r_last_error()
-    assert L.s3r_set_option(None, 1) == -1
     assert L.s3r_dropout_mask(None, 4, 1, 0.15, None) == -1 and b"dropout_mask" in L.s3r_last_error()

@@ -41,11 +41,13 @@ def test_split_roundtrip(L):
 @pytest.mark.parametrize("rows,K,N,groups,bn", [
     (768, 1024, 3072, 1, 0), (768, 1024, 1024, 1, 0), (768, 4096, 1024, 1, 0), (196, 768, 2304, 1, 0),
     (300, 96, 1536, 1, 0), (768, 768, 768, 2, 0), (768, 1792, 1792, 2, 0),
-    (1000, 512, 512, 1, 64), (1000, 512, 512, 1, 128), (1000, 512, 512, 1, 256), (7680, 1024, 1024, 1, 0),
+    (1000, 512, 512, 1, 64), (1000, 512, 512, 1, 96), (1000, 512, 512, 1, 128), (7680, 1024, 1024, 1, 0),
     (130, 64, 32, 1, 0),
-    # force_bn 2128 / 2256: CTA-pair tile widths of other architectures, the nearest width on sm_90a
-    (768, 1024, 3072, 1, 2128), (768, 1024, 3072, 1, 2256), (768, 768, 768, 2, 2128), (7680, 1024, 1024, 1, 2256),
-    (1536, 768, 96, 1, 2128), (768, 4096, 1024, 1, 2256),
+    # forced widths on the model's shapes
+    (768, 1024, 3072, 1, 128), (768, 1024, 3072, 1, 64), (768, 768, 768, 2, 128), (7680, 1024, 1024, 1, 128),
+    (1536, 768, 96, 1, 128), (768, 4096, 1024, 1, 128),
+    (768, 768, 768, 2, 64), (768, 3072, 768, 2, 64), (768, 1024, 1024, 1, 64), (768, 4096, 1024, 1, 64),
+    (1536, 768, 96, 1, 64), (512, 96, 1536, 1, 64),
     # K-heavy shapes with few tiles (value-encoder fc2, decoder fc2, tiny-M long-K)
     (768, 4096, 1024, 1, 0), (768, 3072, 768, 2, 0), (256, 6912, 768, 2, 0), (196, 1024, 1024, 1, 0),
 ])
@@ -68,8 +70,9 @@ def test_linear_bias_gelu_residual(L, rows, K, N, groups, bn):
 @pytest.mark.parametrize("NB,H,W,Cin,Cout,groups,bn", [
     (1, 12, 16, 256, 256, 2, 0), (1, 24, 32, 96, 256, 1, 0), (2, 7, 7, 256, 256, 1, 0), (1, 96, 128, 256, 128, 2, 0),
     (1, 14, 14, 384, 256, 1, 0), (1, 48, 64, 192, 256, 1, 0), (1, 12, 16, 768, 256, 2, 0),
-    # force_bn 2128 / 2256 on a 3x3 conv
-    (1, 96, 128, 256, 256, 2, 2256), (1, 96, 128, 256, 128, 1, 2128), (2, 24, 32, 96, 256, 1, 2256),
+    # forced widths on a 3x3 conv
+    (1, 96, 128, 256, 256, 2, 128), (1, 96, 128, 256, 128, 1, 128), (2, 24, 32, 96, 256, 1, 128),
+    (1, 24, 32, 96, 256, 1, 64), (1, 96, 128, 256, 128, 2, 64),
 ])
 def test_conv3x3(L, NB, H, W, Cin, Cout, groups, bn):
     x = _rand(groups * NB, Cin, H, W, seed=6)
@@ -206,8 +209,8 @@ def test_cross_attention_shapes(L, BH, heads, nq, nk):
 
 @pytest.mark.parametrize("H,W,bn", [(48, 64, 0), (48, 64, 128), (24, 40, 0), (96, 128, 0)])
 def test_head_tail(L, H, W, bn):
-    """bn 0: the planner's choice (256 x 128 CTA-pair tiles where the pixel-tile count is even, the two column halves'
-    partial dot products meet in shared memory), 128: the 1-CTA kernel."""
+    """The DPT head tail runs 128 wide whatever force_bn asks (the two column halves' partial dot products meet in
+    shared memory): bn 0 and 128 give the same launch."""
     groups, NB, Cin = 2, 1, 128
     x = _rand(groups * NB, Cin, H, W, seed=30)
     w = _rand(groups * 128, Cin, 3, 3, seed=31, scale=(9 * Cin) ** -0.5)
@@ -275,7 +278,8 @@ def test_layernorm_upsample_im2col_rope(L):
 
 @pytest.mark.parametrize("rows,C,N,groups,swap,bn", [
     (768, 768, 2304, 2, 0, 0), (768, 768, 1536, 2, 1, 0), (768, 1024, 4096, 1, 0, 0), (196, 1024, 3072, 1, 0, 0),
-    (7680, 1024, 3072, 1, 0, 0), (768, 768, 768, 2, 1, 2128), (1000, 768, 768, 1, 0, 64),
+    (7680, 1024, 3072, 1, 0, 0), (768, 768, 768, 2, 1, 128), (1000, 768, 768, 1, 0, 64),
+    (768, 768, 768, 2, 1, 64), (768, 768, 2304, 2, 0, 64), (1024, 768, 768, 1, 0, 64),
 ])
 def test_folded_layernorm_chain(L, rows, C, N, groups, swap, bn):
     """Producer GEMM (x = r + a W0^T + b0: writes x fp32, planes(x) and the per-row chunk statistics) followed by a
