@@ -262,7 +262,7 @@ int s3r_pcl_icp(const void* source, int is_f64, int64_t ns, const void* target_i
                 double max_correspondence_distance, const double* init, int max_iteration, double relative_fitness,
                 double relative_rmse, void* workspace, double* out, void* stream);
 /* x [n] fp64, non-negative -> out[0] mean (fixed-order sum), out[1] exact median (np.median: the mean of the two middle
- * order statistics for even n), out[2] count of x < threshold.  workspace: s3r_pcl_stats_workspace_bytes() bytes. */
+ * order statistics for even n; a -0.0 in the middle comes back as +0.0), out[2] count of x < threshold.  workspace: s3r_pcl_stats_workspace_bytes() bytes. */
 size_t s3r_pcl_stats_workspace_bytes(void);
 int s3r_pcl_stats(const double* x, int64_t n, double threshold, void* workspace, double* out, void* stream);
 /* out[i] = |a[i] . b[idx[i]]| for a [n, 3], b [*, 3] fp64, idx [n] int64 (eval_recon.py's normal consistency). */

@@ -18,7 +18,7 @@
 //   ICP: pcl_icp_corr_kernel / pcl_icp_update_kernel x (max_iteration + 1) -- fixed launch count, a device-side done flag,
 //   per-pass sums in a fixed block order relative to the target's box centre, the Umeyama update on one thread.
 //   Statistics of an fp64 vector: fixed-order mean, exact median by a 64-bit radix select (8 x 8-bit passes on the bit
-//   pattern, which orders like the value for non-negative doubles), count below a threshold.
+//   pattern, which orders like the value for non-negative doubles once -0.0 is keyed as +0.0), count below a threshold.
 #include "kernels.cuh"
 
 #include <climits>
@@ -41,6 +41,7 @@ constexpr int kIcpThreads = 128;
 constexpr int kAccN = 17;            // ICP sums: count, sum d^2, sum src (3), sum dst (3), sum src dst^T (9)
 constexpr int kStatBlocks = 264;
 constexpr int kIcpHeader = 19;       // out: T 4x4, fitness, rmse, passes; then per-pass counts, per-pass rmse
+constexpr unsigned long long kNegZero = 0x8000000000000000ULL;   // bit pattern of -0.0
 
 inline size_t align256(size_t x) { return (x + 255) / 256 * 256; }
 
@@ -575,7 +576,8 @@ __global__ void __launch_bounds__(256) pcl_select_hist(const double* __restrict_
   const int shift = 56 - 8 * pass;
   const unsigned long long prefix = S.prefix;
   for (long long i = blockIdx.x * 256LL + threadIdx.x; i < n; i += 256LL * kStatBlocks) {
-    const unsigned long long key = (unsigned long long)__double_as_longlong(x[i]);
+    unsigned long long key = (unsigned long long)__double_as_longlong(x[i]);
+    if (key == kNegZero) key = 0;   // -0.0 == +0.0; its sign bit alone would sort it above +inf
     if (pass > 0 && (key >> (shift + 8)) != prefix) continue;
     atomicAdd(&h[(key >> shift) & 255], 1u);
   }
