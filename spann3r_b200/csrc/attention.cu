@@ -11,6 +11,14 @@
 // block into a 3-stage ring), warpgroups 1 and 2 each own 64 query rows for ALL KV blocks: S = Q K^T into registers
 // (wgmma, A and B from shared memory), exact online softmax in registers, O += P V with P as the register A operand.
 // Output: split-bf16 planes (A operand of the following projection GEMM) and/or fp32.
+//
+// Arithmetic contract, held bit for bit by tests/test_attn_core_exact_gpu.py: these roundings are part of the
+// interface, and a rewrite that changes one changes that test's expected bits on purpose.  Per 128-query tile, head and
+// 128-key block: S = Q K^T on tf32 wgmma with fp32 accumulation; keys >= nk set to -inf; running max n = max(m, block
+// max); al = exp2f((m - n) * log2e), 0 on the first block; e = exp2f(fmaf(s, log2e, -n * log2e)); P = RN_tf32(e) as
+// (bits + 0x1000) & ~0x1fff; l = l * al + sum P (per-thread partials, quad-reduced at the end); O = O * al + P V on tf32
+// wgmma with P as the register A operand; out = O * (1.0f / l), the division correctly rounded, written as fp32 and/or
+// split2_bf16 planes at [b * nq + q, h * 64 + c] with row stride ldo.
 #include "common.cuh"
 #include "kernels.cuh"
 #include "wgmma.cuh"

@@ -34,6 +34,10 @@ rows are relied on to tell the two apart (`test_bound_holds_for_rn_emulation_and
 Largest |O - ref| / bound measured on H100 80GB HBM3 cards at 400 W and at 700 W power limits (the same on both):
 engine shapes 0.63, ragged sizes 0.71, two-key rows 0.47, peaked rows 0.045, uniform rows 1.1e-4.  The bound is rigorous
 under the model above, so each test asserts the ratio stays below 1.
+
+The bound cannot see changes of about one ulp to the kernel's arithmetic, such as l summing the unrounded e, an
+approximate 1 / l or a stale rescale.  test_attn_core_exact_gpu.py pins those: on exactly representable inputs
+(attn_core_exact.py) it holds the kernel to its one correct fp32 answer bit for bit, at the same shapes as this file.
 """
 import math
 
