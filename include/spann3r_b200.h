@@ -175,8 +175,10 @@ int s3r_gemm_plan_bn(int64_t m_tiles, int n, int sms, int col_align, int force_b
 
 /* Fused multi-head attention core, head dim 64: O = softmax(Q K^T) V per (batch*head) on tf32 wgmma.
  *   q [bh, nq, 64], k [bh, nk, 64] (already RoPE'd / scaled by the QKV epilogue), vt [bh, 64, nk_pad];
- *   output [b*nq, heads*64] as planes and/or fp32 (row stride ldo, even); bh a multiple of heads; nk_pad >= nk, a
- *   multiple of 4: columns nk .. nk_pad-1 of vt are never read.
+ *   output [b*nq, heads*64] as planes (o_hi and o_lo both, or neither) and/or fp32, row stride ldo: even and
+ *   >= heads*64; bh a multiple of heads and <= 65535; nk_pad >= nk, a multiple of 4: columns nk .. nk_pad-1 of vt are
+ *   never read.  q, k, vt 16-byte aligned, o_f32 8-byte, o_hi / o_lo 4-byte.  Every rule is checked before any CUDA
+ *   call (-1, last error naming the field); then nq, nk or bh <= 0 returns 0 and launches nothing.
  * croco/models/blocks.py:106-110 (self), :162-166 (cross). */
 int s3r_attention(const float* q, const float* k, const float* vt, int bh, int heads, int nq, int nk, int nk_pad,
                   void* o_hi, void* o_lo, float* o_f32, int64_t ldo, void* stream);

@@ -228,44 +228,57 @@ __global__ void __launch_bounds__(attn::kThreads, 1) attention_kernel(const __gr
   }
 }
 
-int attn_plan_init(AttnPlan* plan, const float* q, const float* k, const float* vt, int BH, int heads, int nq, int nk,
-                   int nk_pad) {
+int attn_plan(const AttnDesc& d, AttnPlan* plan) {
   using namespace attn;
   memset(plan, 0, sizeof(*plan));
-  if (nk_pad % 4 != 0 || nk_pad < nk) {
-    set_error("attention: nk_pad=%d must be >= nk=%d and a multiple of 4", nk_pad, nk);
+  // Every rule the kernel relies on, before any CUDA call: grid.y holds bh, the paired stores stay in even rows wide
+  // enough for every head, V^T rows are whole 16-byte groups, o_lo is written whenever o_hi is, TMA bases are aligned.
+  if (d.heads <= 0 || d.bh % d.heads != 0 || d.bh > 65535) {
+    set_error("attention: bh=%d must be a multiple of heads=%d and at most 65535 (grid.y)", d.bh, d.heads);
     return -1;
   }
+  if (d.ldo % 2 != 0 || d.ldo < 64LL * d.heads) {
+    set_error("attention: ldo=%lld must be even and at least heads * 64 = %lld", d.ldo, 64LL * d.heads);
+    return -1;
+  }
+  if (d.nk_pad % 4 != 0 || d.nk_pad < d.nk) {
+    set_error("attention: nk_pad=%d must be >= nk=%d and a multiple of 4", d.nk_pad, d.nk);
+    return -1;
+  }
+  if (!d.o_hi != !d.o_lo) {
+    set_error("attention: o_hi and o_lo must both be given or both be null");
+    return -1;
+  }
+  const struct { const char* name; const void* p; unsigned align; } ptrs[] = {
+      {"q", d.q, 16}, {"k", d.k, 16}, {"vt", d.vt, 16}, {"o_f32", d.o_f32, 8}, {"o_hi", d.o_hi, 4}, {"o_lo", d.o_lo, 4}};
+  for (const auto& x : ptrs)
+    if (reinterpret_cast<uintptr_t>(x.p) % x.align != 0) {
+      set_error("attention: %s=%p must be %u-byte aligned", x.name, x.p, x.align);
+      return -1;
+    }
+  if (d.nq <= 0 || d.nk <= 0 || d.bh <= 0) return 0;
   AttnArgs& a = plan->args;
-  {
-    uint64_t dims[3] = {64, (uint64_t)nq, (uint64_t)BH};
-    uint64_t str[2] = {64 * 4, (uint64_t)nq * 64 * 4};
-    uint32_t box[3] = {32, (uint32_t)BQ, 1};
-    int r = encode_tmap(&a.tmQ, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, q, dims, str, box);
-    if (r) return r;
-  }
-  {
-    uint64_t dims[3] = {64, (uint64_t)nk, (uint64_t)BH};
-    uint64_t str[2] = {64 * 4, (uint64_t)nk * 64 * 4};
-    uint32_t box[3] = {32, (uint32_t)BKV, 1};
-    int r = encode_tmap(&a.tmK, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, k, dims, str, box);
-    if (r) return r;
-  }
-  {
-    uint64_t dims[3] = {(uint64_t)nk, 64, (uint64_t)BH};
-    uint64_t str[2] = {(uint64_t)nk_pad * 4, (uint64_t)nk_pad * 64 * 4};
-    uint32_t box[3] = {32, 64, 1};
-    int r = encode_tmap(&a.tmV, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, vt, dims, str, box);
-    if (r) return r;
-  }
-  a.nq = nq; a.nk = nk; a.heads = heads;
-  plan->grid = dim3((nq + BQ - 1) / BQ, BH);
-  plan->flops = 4.0 * BH * (double)nq * nk * 64;
+  // q, k and V^T are each a stack of bh row-major [d1, d0] fp32 matrices with row stride ld, loaded in [b1, b0] boxes
+  auto encode = [&](CUtensorMap* m, const float* base, int d0, int d1, int ld, uint32_t b0, uint32_t b1) {
+    const uint64_t dims[3] = {(uint64_t)d0, (uint64_t)d1, (uint64_t)d.bh};
+    const uint64_t str[2] = {(uint64_t)ld * 4, (uint64_t)ld * d1 * 4};
+    const uint32_t box[3] = {b0, b1, 1};
+    return encode_tmap(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, base, dims, str, box);
+  };
+  int r;
+  if ((r = encode(&a.tmQ, d.q, D, d.nq, D, 32, BQ)) || (r = encode(&a.tmK, d.k, D, d.nk, D, 32, BKV)) ||
+      (r = encode(&a.tmV, d.vt, d.nk, D, d.nk_pad, 32, D)))
+    return r;
+  a.nq = d.nq; a.nk = d.nk; a.heads = d.heads;
+  a.o_hi = d.o_hi; a.o_lo = d.o_lo; a.o_f32 = d.o_f32; a.ldo = d.ldo;
+  plan->grid = dim3((d.nq + BQ - 1) / BQ, d.bh);
+  plan->flops = 4.0 * d.bh * (double)d.nq * d.nk * 64;
   return 0;
 }
 
-static int attn_launch_args(const AttnPlan& plan, const AttnArgs& a, cudaStream_t st) {
+int attn_launch(const AttnPlan& plan, cudaStream_t st) {
   using namespace attn;
+  if (plan.grid.x == 0) return 0;   // empty sizes: attn_plan left the grid 0
   static PerDeviceOnce once;
   bool& attr_set = once.cur();
   if (!attr_set) {
@@ -276,32 +289,12 @@ static int attn_launch_args(const AttnPlan& plan, const AttnArgs& a, cudaStream_
     }
     attr_set = true;
   }
-  cudaError_t e = launch_pdl(attention_kernel, plan.grid, dim3(kThreads), SMEM, st, a);
+  cudaError_t e = launch_pdl(attention_kernel, plan.grid, dim3(kThreads), SMEM, st, plan.args);
   if (e != cudaSuccess) {
     set_error("attention launch failed: %s", cudaGetErrorString(e));
     return -6;
   }
   return 0;
-}
-
-int attn_launch(const AttnPlan& plan, __nv_bfloat16* o_hi, __nv_bfloat16* o_lo, float* o_f32, long long ldo,
-                cudaStream_t st) {
-  AttnArgs a = plan.args;
-  a.o_hi = o_hi; a.o_lo = o_lo; a.o_f32 = o_f32; a.ldo = ldo;
-  return attn_launch_args(plan, a, st);
-}
-
-int launch_attention(const float* q, const float* k, const float* vt, int BH, int heads, int nq, int nk, int nk_pad,
-                     __nv_bfloat16* o_hi, __nv_bfloat16* o_lo, float* o_f32, long long ldo, cudaStream_t st) {
-  if (heads <= 0 || BH % heads != 0 || ldo % 2 != 0) {
-    set_error("attention: bh=%d must be a multiple of heads=%d, and ldo=%lld even (paired stores)", BH, heads, ldo);
-    return -1;
-  }
-  if (nq <= 0 || nk <= 0 || BH <= 0) return 0;
-  AttnPlan plan;
-  int r = attn_plan_init(&plan, q, k, vt, BH, heads, nq, nk, nk_pad);
-  if (r) return r;
-  return attn_launch(plan, o_hi, o_lo, o_f32, ldo, st);
 }
 
 }  // namespace s3r

@@ -209,7 +209,10 @@ int s3r_dropout_mask(float* out, int64_t n, uint64_t seed, float p, void* stream
 
 int s3r_attention(const float* q, const float* k, const float* vt, int bh, int heads, int nq, int nk, int nk_pad,
                   void* o_hi, void* o_lo, float* o_f32, int64_t ldo, void* stream) {
-  return launch_attention(q, k, vt, bh, heads, nq, nk, nk_pad, B(o_hi), B(o_lo), o_f32, ldo, S(stream));
+  const AttnDesc d = {q, k, vt, bh, heads, nq, nk, nk_pad, B(o_hi), B(o_lo), o_f32, ldo};
+  AttnPlan plan;
+  if (int r = attn_plan(d, &plan)) return r;
+  return attn_launch(plan, S(stream));
 }
 
 }  // extern "C"

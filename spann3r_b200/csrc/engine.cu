@@ -147,6 +147,26 @@ struct s3r_engine {
     d.ln_cs = pc.precision == GEMM_BF16 ? w.cs_hi : w.cs;
   }
 
+  // Runs the next plan of a cache's list (replayed in the order the first pass built it) through launch(plan), counting
+  // its flops and the launch; while profiling, between two CUDA events recorded as `kind` (see Timed).
+  template <typename Plan, typename Launch>
+  int run_plan(std::vector<Plan>& plans, size_t& next, int kind, cudaStream_t st, Launch launch) {
+    if (next >= plans.size()) {
+      set_error("engine: plan cache out of sync");
+      return -8;
+    }
+    Plan& p = plans[next++];
+    flops += p.flops;
+    ++launches;
+    if (!profiling) return launch(p);
+    Timed t; t.a = get_event(); t.b = get_event(); t.flops = p.flops; t.kind = kind;
+    cudaEventRecord(t.a, st);
+    int r = launch(p);
+    cudaEventRecord(t.b, st);
+    timed.push_back(t);
+    return r;
+  }
+
   int gemm(PlanCache& pc, s3r_gemm_desc d, cudaStream_t st) {
     if (d.ln_stats && !d.ln_cs) {
       set_error("engine: a LayerNorm-folded linear lacks its %s column sums", pc.precision == GEMM_BF16 ? "cs_hi" : "cs");
@@ -157,44 +177,21 @@ struct s3r_engine {
       pc.gemms.emplace_back();
       if (int r = gemm_plan(d, &pc.gemms.back())) return r;
     }
-    if (pc.gc >= pc.gemms.size()) {
-      set_error("engine: plan cache out of sync");
-      return -8;
-    }
-    GemmPlan& p = pc.gemms[pc.gc++];
-    gemm_set_epilogue(d, p.args);
-    flops += p.flops;
-    ++launches;
-    if (!profiling) return gemm_launch(p, st);
-    Timed t; t.a = get_event(); t.b = get_event(); t.flops = p.flops; t.kind = p.precision == GEMM_BF16 ? 2 : 0;
-    cudaEventRecord(t.a, st);
-    int r = gemm_launch(p, st);
-    cudaEventRecord(t.b, st);
-    timed.push_back(t);
-    return r;
+    return run_plan(pc.gemms, pc.gc, pc.precision == GEMM_BF16 ? 2 : 0, st, [&](GemmPlan& p) {
+      gemm_set_epilogue(d, p.args);
+      return gemm_launch(p, st);
+    });
   }
 
+  // Inputs and outputs are fixed workspace buffers of the call site, so the plan holds them and a replay only launches.
   int attention(PlanCache& pc, const float* q, const float* k, const float* vt, int BH, int heads, int nq, int nk,
                 Planes out, long long ldo, cudaStream_t st) {
     if (pc.building) {
+      const AttnDesc d = {q, k, vt, BH, heads, nq, nk, Npad, out.hi, out.lo, nullptr, ldo};
       pc.attns.emplace_back();
-      int r = attn_plan_init(&pc.attns.back(), q, k, vt, BH, heads, nq, nk, Npad);
-      if (r) return r;
+      if (int r = attn_plan(d, &pc.attns.back())) return r;
     }
-    if (pc.ac >= pc.attns.size()) {
-      set_error("engine: attention plan cache out of sync");
-      return -8;
-    }
-    AttnPlan& p = pc.attns[pc.ac++];
-    flops += p.flops;
-    ++launches;
-    if (!profiling) return attn_launch(p, out.hi, out.lo, nullptr, ldo, st);
-    Timed t; t.a = get_event(); t.b = get_event(); t.flops = p.flops; t.kind = 1;
-    cudaEventRecord(t.a, st);
-    int r = attn_launch(p, out.hi, out.lo, nullptr, ldo, st);
-    cudaEventRecord(t.b, st);
-    timed.push_back(t);
-    return r;
+    return run_plan(pc.attns, pc.ac, 1, st, [&](AttnPlan& p) { return attn_launch(p, st); });
   }
 
   int ln(const float* x, const s3r_ln& w, long long wb_stride, long long rows_per_group, float eps, long long rows, int C,

@@ -40,15 +40,24 @@ struct AttnArgs {
   float* o_f32;
   long long ldo;
 };
+// One launch of the fused attention core (attention.cu): the arguments of s3r_attention (include/spann3r_b200.h)
+struct AttnDesc {
+  const float *q, *k, *vt;
+  int bh, heads, nq, nk, nk_pad;
+  __nv_bfloat16 *o_hi, *o_lo;
+  float* o_f32;
+  long long ldo;
+};
 struct AttnPlan {
   AttnArgs args;
   dim3 grid;
   double flops;
 };
-int attn_plan_init(AttnPlan* plan, const float* q, const float* k, const float* vt, int BH, int heads, int nq, int nk,
-                   int nk_pad);
-int attn_launch(const AttnPlan& plan, __nv_bfloat16* o_hi, __nv_bfloat16* o_lo, float* o_f32, long long ldo,
-                cudaStream_t st);
+// Checks every rule of s3r_attention before any CUDA call, then encodes the three tensor maps and fills the arguments,
+// outputs included; nq, nk or bh <= 0 leaves an empty plan.  Returns 0 or a negative error, last_error() naming the field.
+int attn_plan(const AttnDesc& d, AttnPlan* plan);
+// Launches the plan as it is (an empty one: nothing), without validation or tensor-map encoding.
+int attn_launch(const AttnPlan& plan, cudaStream_t st);
 
 // spatial memory (memory.cu)
 // longest bank the softmax takes: one fp32 score row in shared memory, up to 200 KB of it
@@ -137,10 +146,6 @@ int launch_loss_forward(const s3r_loss_desc* d, void* ws, size_t ws_bytes, float
                         uint8_t* valid_out, double* results, cudaStream_t st);
 int launch_loss_backward(const s3r_loss_desc* d, const void* ws, size_t ws_bytes, const float* upstream,
                          float* grad_pred, float* grad_conf, cudaStream_t st);
-
-// fused attention (attention.cu): O = softmax(Q K^T) V per (batch*head), tf32 wgmma, split-bf16 output
-int launch_attention(const float* q, const float* k, const float* vt, int BH, int heads, int nq, int nk, int nk_pad,
-                     __nv_bfloat16* o_hi, __nv_bfloat16* o_lo, float* o_f32, long long ldo, cudaStream_t st);
 
 // attention of the training backward (attention_train.cu): split-bf16 flash forward / backward; validate before any
 // CUDA call

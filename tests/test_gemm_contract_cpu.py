@@ -154,3 +154,28 @@ def test_attention_rejects_partial_batches_and_odd_strides(L):
     assert b"heads" in lib.s3r_last_error()
     assert lib.s3r_attention(_p(1), _p(2), _p(3), 24, 12, 196, 196, 196, None, None, _p(4), 769, None) == -1
     assert b"ldo" in lib.s3r_last_error()
+    good = dict(q=_p(1), k=_p(2), vt=_p(3), bh=24, heads=12, nq=196, nk=196, nk_pad=196, o_hi=_p(5), o_lo=_p(6),
+                o_f32=_p(4), ldo=768)
+
+    def attention(**change):
+        a = {**good, **change}
+        return lib.s3r_attention(*a.values(), None)
+
+    for change, field in [
+        (dict(o_lo=None), "o_hi and o_lo"),           # the kernel writes o_lo whenever o_hi is set
+        (dict(o_hi=None), "o_hi and o_lo"),
+        (dict(ldo=766), "ldo=766"),                   # narrower than heads * 64
+        (dict(bh=65536, heads=16, ldo=1024), "bh=65536"),   # grid.y
+        (dict(q=_p(1) + 8), "attention: q="),         # TMA bases: 16 bytes
+        (dict(k=_p(2) + 4), "attention: k="),
+        (dict(vt=_p(3) + 8), "attention: vt="),
+        (dict(o_f32=_p(4) + 4), "attention: o_f32="),  # paired fp32 stores: 8 bytes
+        (dict(o_hi=_p(5) + 2), "attention: o_hi="),    # paired bf16 stores: 4 bytes
+        (dict(o_lo=_p(6) + 2), "attention: o_lo="),
+        (dict(nk_pad=198), "nk_pad=198"),             # V^T rows of whole 16-byte groups
+        (dict(nk_pad=192), "nk_pad=192"),             # shorter than nk
+        (dict(nq=0, o_lo=None), "o_hi and o_lo"),     # empty sizes are checked too
+    ]:
+        assert attention(**change) == -1, change
+        assert field.encode() in lib.s3r_last_error(), (change, lib.s3r_last_error())
+    assert attention(nq=0) == 0   # empty: nothing to launch
