@@ -288,6 +288,37 @@ int s3r_render_splat(const float* pts, const uint8_t* mask, int64_t n, int64_t i
                      int width, int height, void* keys, void* stream);
 int s3r_render_resolve(const void* keys, const float* colors, int width, int height, uint8_t* rgb, void* stream);
 
+/* ---- triangle meshes: app.py's pts3d_to_trimesh + cat_meshes, and a z-buffered triangle rasteriser ---------------------
+ * Pixel-grid mesh of T frames of H x W pixels (T * H * W < 2^31), valid [T, H, W] uint8, images [T, H, W, 3] fp32.
+ * Candidate faces in app.py's order: per frame the blocks [i1,i2,i3], [i3,i2,i1], [i2,i3,i4], [i4,i3,i2] (i1..i4 the
+ * quad's top-left, top-right, bottom-left, bottom-right pixel), quads row-major inside a block, indices offset by t H W.
+ * A face is kept when its three corners are valid; kept faces keep their order.  Colour: blocks 0-1 the quad's top-left
+ * pixel, blocks 2-3 its bottom-right pixel.
+ *   s3r_mesh_grid_workspace_bytes(T, H, W): device workspace bytes (0 = size out of range), 8-byte aligned.
+ *   s3r_mesh_grid_count: per-tile counts and their scan into the workspace; *n_faces (HOST) <- the number of kept
+ *     faces.  Synchronises `stream` (one device -> host read).
+ *   s3r_mesh_grid_faces: with that workspace, faces [n_faces, 3] int32 and colors [n_faces, 3] fp32.
+ * s3r_raster_triangles draws n_faces triangles faces [n_faces, 3] int32 (indices into verts [n_verts, 3] fp32; faces
+ * with an index out of range are skipped) with face ids id0 .. id0 + n_faces - 1 (id0 + n_faces < 2^31) into the key
+ * buffer of s3r_render_workspace_bytes / s3r_render_clear:
+ *   camera (HOST, 16 doubles) as for s3r_render_splat; pixel centres at integer (u, v), row 0 at the top;
+ *   a triangle is skipped when a vertex is not finite or has camera depth <= z_near (finite, >= 0), when it is a back
+ *   face (clockwise on the image) or degenerate; a centre is covered by fp64 edge functions with a top-left rule, so a
+ *   centre on an edge shared by two triangles goes to exactly one of them;
+ *   depth = fp32(1 / ((b0 / z0 + b1 / z1) + b2 / z2)) with fp64 barycentrics b; depths > z_far (> z_near; inf allowed)
+ *   are dropped; key = bits(depth) << 32 | face id, atomicMin: nearest depth wins, ties -> smaller face id.
+ * s3r_raster_resolve writes depth [height, width] fp32 (0 where empty) and face [height, width] int32 (-1 where empty).
+ * Deterministic: the result depends neither on scheduling nor on the order faces are submitted in. */
+size_t s3r_mesh_grid_workspace_bytes(int T, int H, int W);
+int s3r_mesh_grid_count(const uint8_t* valid, int T, int H, int W, void* workspace, size_t workspace_bytes,
+                        int64_t* n_faces, void* stream);
+int s3r_mesh_grid_faces(const uint8_t* valid, const float* images, int T, int H, int W, const void* workspace,
+                        size_t workspace_bytes, int32_t* faces, float* colors, void* stream);
+int s3r_raster_triangles(const float* verts, int64_t n_verts, const int32_t* faces, int64_t n_faces, int64_t id0,
+                         const double* camera, double z_near, double z_far, int width, int height, void* keys,
+                         void* stream);
+int s3r_raster_resolve(const void* keys, int width, int height, float* depth, int32_t* face, void* stream);
+
 /* ---- training / test criteria: spann3r/loss.py:129-369 (Regr3D_t, its ShiftInv / ScaleInv / ScaleShiftInv variants,
  * ConfLoss_t) with L21 (dust3r/losses.py:52-59), forward and backward --------------------------------------------------
  * F >= 2 views of B sequences of H x W pixels.  Pred slot k < F-1 is preds_all[k][0] (frame k: 'pts3d' for k = 0, else

@@ -105,6 +105,11 @@ _PROTOS = {
     "s3r_render_clear": (_i, [_vp, _i, _i, _vp]),
     "s3r_render_splat": (_i, [_vp, _vp, _i64, _i64, _vp, C.c_double, _i, _i, _vp, _vp]),
     "s3r_render_resolve": (_i, [_vp, _vp, _i, _i, _vp, _vp]),
+    "s3r_mesh_grid_workspace_bytes": (C.c_size_t, [_i, _i, _i]),
+    "s3r_mesh_grid_count": (_i, [_vp, _i, _i, _i, _vp, C.c_size_t, _vp, _vp]),
+    "s3r_mesh_grid_faces": (_i, [_vp, _vp, _i, _i, _i, _vp, C.c_size_t, _vp, _vp, _vp]),
+    "s3r_raster_triangles": (_i, [_vp, _i64, _vp, _i64, _i64, _vp, C.c_double, C.c_double, _i, _i, _vp, _vp]),
+    "s3r_raster_resolve": (_i, [_vp, _i, _i, _vp, _vp, _vp]),
     "s3r_loss_workspace_bytes": (C.c_size_t, [C.POINTER(LossDesc)]),
     "s3r_loss_forward": (_i, [C.POINTER(LossDesc), _vp, C.c_size_t, _vp, _vp, _vp, _vp, _vp]),
     "s3r_loss_backward": (_i, [C.POINTER(LossDesc), _vp, C.c_size_t, _vp, _vp, _vp, _vp]),

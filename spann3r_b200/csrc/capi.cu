@@ -173,6 +173,26 @@ int s3r_render_resolve(const void* keys, const float* colors, int width, int hei
   return launch_render_resolve(keys, colors, width, height, rgb, S(stream));
 }
 
+size_t s3r_mesh_grid_workspace_bytes(int T, int H, int W) { return mesh_grid_workspace_bytes(T, H, W); }
+int s3r_mesh_grid_count(const uint8_t* valid, int T, int H, int W, void* workspace, size_t workspace_bytes,
+                        int64_t* n_faces, void* stream) {
+  return launch_mesh_grid_count(valid, T, H, W, workspace, workspace_bytes, reinterpret_cast<long long*>(n_faces),
+                                S(stream));
+}
+int s3r_mesh_grid_faces(const uint8_t* valid, const float* images, int T, int H, int W, const void* workspace,
+                        size_t workspace_bytes, int32_t* faces, float* colors, void* stream) {
+  return launch_mesh_grid_faces(valid, images, T, H, W, workspace, workspace_bytes, faces, colors, S(stream));
+}
+int s3r_raster_triangles(const float* verts, int64_t n_verts, const int32_t* faces, int64_t n_faces, int64_t id0,
+                         const double* camera, double z_near, double z_far, int width, int height, void* keys,
+                         void* stream) {
+  return launch_raster_triangles(verts, n_verts, faces, n_faces, id0, camera, z_near, z_far, width, height, keys,
+                                 S(stream));
+}
+int s3r_raster_resolve(const void* keys, int width, int height, float* depth, int32_t* face, void* stream) {
+  return launch_raster_resolve(keys, width, height, depth, face, S(stream));
+}
+
 size_t s3r_loss_workspace_bytes(const s3r_loss_desc* d) { return loss_workspace_bytes(d); }
 int s3r_loss_forward(const s3r_loss_desc* d, void* workspace, size_t workspace_bytes, float* gt_out, float* pred_out,
                      uint8_t* valid_out, double* results, void* stream) {

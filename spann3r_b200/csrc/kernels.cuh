@@ -132,6 +132,18 @@ int launch_render_splat(const float* pts, const uint8_t* mask, long long n, long
                         double z_near, int w, int h, void* keys, cudaStream_t st);
 int launch_render_resolve(const void* keys, const float* colors, int w, int h, uint8_t* out, cudaStream_t st);
 
+// triangle meshes (mesh.cu): app.py's pixel-grid faces (count + scan, then ordered writes) and the triangle rasteriser
+// into the render key buffer, with its depth / face resolve
+size_t mesh_grid_workspace_bytes(int T, int H, int W);
+int launch_mesh_grid_count(const uint8_t* valid, int T, int H, int W, void* workspace, size_t workspace_bytes,
+                           long long* n_faces, cudaStream_t st);
+int launch_mesh_grid_faces(const uint8_t* valid, const float* images, int T, int H, int W, const void* workspace,
+                           size_t workspace_bytes, int* faces, float* colors, cudaStream_t st);
+int launch_raster_triangles(const float* verts, long long n_verts, const int* faces, long long n_faces, long long id0,
+                            const double* camera, double z_near, double z_far, int w, int h, void* keys,
+                            cudaStream_t st);
+int launch_raster_resolve(const void* keys, int w, int h, float* depth, int* face, cudaStream_t st);
+
 // conv backward (conv_wgrad.cu): weight gradient over pixels (split-bf16 wgmma, split contraction + fixed-order reduce)
 // and the col2im of the 3x3 stride-2 conv; both validate their arguments before any CUDA call
 size_t conv_wgrad_workspace_bytes(int NB, int H, int W, int N, int Kc, int taps);

@@ -169,6 +169,50 @@ def render_frames(pts_all, image_all, camera_parameters, output_dir=None, mask=N
     return frames
 
 
+def render_mesh_frames(pts_all, image_all, camera_parameters, output_dir=None, mask=None, save_video=True,
+                       save_camera=True, dynamic=False, z_near=0.0):
+    """`render_frames`' contract, drawing app.py's reconstruction mesh (`mesh.pts3d_to_mesh`) instead of points.
+
+    Frame i draws the triangles of frame i (dynamic=True) or of frames 0..i with the triangle rasteriser of
+    `mesh.rasterize` (back faces culled: app.py's mesh carries both windings, so none of it is hidden); each pixel takes
+    the colour of its face, rounded as render_frames rounds.  Static mode keeps the key buffer across frames and draws
+    only each new frame's triangles.  mask: [T, H, W] bool (the valid pixels) or None; points and colours of valid
+    pixels must be finite.  Returns uint8 [T, h, w, 3] CUDA frames and writes render_frames' files with `write_frames`."""
+    from . import mesh
+    pts_all, image_all, mask = _frames_input(pts_all, image_all, mask)
+    cam, w, h = _camera_array(camera_parameters)
+    if not (math.isfinite(z_near) and z_near >= 0):
+        raise ValueError(f"z_near must be finite and >= 0, got {z_near}")
+    T, H, W, _ = pts_all.shape
+    verts, faces, colors = mesh.pts3d_to_mesh(pts_all, image_all, None if mask is None else mask.view(torch.bool))
+    # faces come frame by frame: the frame of a face is its first vertex // (H W)
+    bounds = torch.searchsorted(torch.div(faces[:, 0], H * W, rounding_mode="floor").contiguous(),
+                                torch.arange(T + 1, dtype=torch.int32, device=faces.device)).cpu().tolist()
+    if len(colors) == 0:
+        colors = torch.zeros((1, 3), dtype=torch.float32, device=pts_all.device)   # never read: no face is drawn
+    L = _lib.lib()
+    dev = pts_all.device
+    keys = torch.empty(int(L.s3r_render_workspace_bytes(w, h)) // 8, dtype=torch.int64, device=dev)
+    frames = torch.empty((T, h, w, 3), dtype=torch.uint8, device=dev)
+    cam_p = C.c_void_p(cam.ctypes.data)
+    with _lib.on_device(dev):
+        st = _lib.stream_ptr(dev)
+        for i in range(T):
+            if dynamic or i == 0:
+                _lib.check(L.s3r_render_clear(_lib.ptr(keys), w, h, st), "s3r_render_clear")
+            f = faces[bounds[i]:bounds[i + 1]]
+            if len(f):
+                _lib.check(L.s3r_raster_triangles(_lib.ptr(verts), len(verts), _lib.ptr(f), len(f), bounds[i], cam_p,
+                                                  float(z_near), math.inf, w, h, _lib.ptr(keys), st),
+                           "s3r_raster_triangles")
+            # the keys hold face ids: the render resolve gathers the face colours
+            _lib.check(L.s3r_render_resolve(_lib.ptr(keys), _lib.ptr(colors), w, h, _lib.ptr(frames[i]), st),
+                       "s3r_render_resolve")
+    if output_dir is not None:
+        write_frames(frames, output_dir, camera_parameters if save_camera else None, save_video)
+    return frames
+
+
 def write_frames(frames: torch.Tensor, output_dir: str, camera_parameters=None, save_video: bool = True) -> None:
     """The files of render_frames: output_dir/render_frames/frame_{i:03d}.png, .../camera.json (when a camera is given)
     and output_dir/render_frame.mp4 (10 fps, 'mp4v'), from RGB uint8 frames [T, h, w, 3] on any device.  Host I/O by
