@@ -24,7 +24,9 @@ def _nanmed(vals, masks):
 
 
 def criterion(gts, preds, norm_mode="avg_dis", gt_scale=False, fix_first=True, shift=False, scale=False,
-              conf_alpha=None, dist_clip=None, name=None, dtype=torch.float64):
+              conf_alpha=None, dist_clip=None, name=None, dtype=torch.float64, check_empty=True):
+    """check_empty: under ConfLoss_t (conf_alpha set) a loss term without a valid pixel raises ValueError, as
+    spann3r_b200.loss does (the reference fails in torch.stack there); False returns NaN for it."""
     F = len(gts)
     L, R, cl, cr = pred_slots(preds, F)
     L = [p.to(dtype) for p in L]
@@ -113,6 +115,8 @@ def criterion(gts, preds, norm_mode="avg_dis", gt_scale=False, fix_first=True, s
     details = {name + "_pts3d_1": float(means[0]), name + "_pts3d_2": float(means[1]), name + "loss_left": left,
                name + "loss_right": right, name + "conf_left": conf_l, name + "conf_right": conf_r}
     details.update({k: float(v) for k, v in monitoring.items()})
+    if conf_alpha is not None and check_empty and any(d.numel() == 0 for d in dists):
+        raise ValueError("a loss term without a valid pixel: ConfLoss_t is undefined there")
     if conf_alpha is None:
         loss = sum(means)
     else:

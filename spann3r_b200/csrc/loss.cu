@@ -222,12 +222,13 @@ __global__ void __launch_bounds__(kThreads) loss_prep_reduce_kernel(Cfg c, Ws w)
       sg += o[1];
       sp += o[2];
     }
-    // norm_factor = sum / (pooled count + 1e-8), clipped at 1e-8, held in fp32 as the reference holds it
+    // norm_factor = sum / (pooled count + 1e-8), clipped at 1e-8, held in fp32 as the reference holds it; a NaN
+    // factor (a NaN point among the valid ones) stays NaN, as torch's clip keeps it, where fmax would give 1e-8
     const double fg = sg / (ntot + 1e-8), fp = sp / (ntot + 1e-8);
     double* sb = st + c.F + 1 + b * kPerB;
     for (int i = 0; i < kPerB; ++i) sb[i] = 0.0;
-    sb[SB_FG] = (norm && !c.gt_scale) ? (double)(float)fmax(fg, kFactorMin) : 1.0;
-    sb[SB_FP] = norm ? (double)(float)fmax(fp, kFactorMin) : 1.0;
+    sb[SB_FG] = (norm && !c.gt_scale) ? (double)(float)(fg == fg ? fmax(fg, kFactorMin) : fg) : 1.0;
+    sb[SB_FP] = norm ? (double)(float)(fp == fp ? fmax(fp, kFactorMin) : fp) : 1.0;
     sb[SB_FP_RAW] = fp;
   }
 }

@@ -364,6 +364,136 @@ LOSS_CASES = {
 }
 
 
+def loss_slot(preds, k, side):
+    """The pts map of pred slot (pair k, side 0 = left / 1 = right) in `preds_all`."""
+    return preds[k][side]["pts3d" if (k == 0 and side == 0) else "pts3d_in_other_view"]
+
+
+def _adv_empty_b(gts, preds):          # batch element 1 has no valid pixel in any frame
+    for g in gts:
+        g["valid_mask"][1] = False
+
+
+def _adv_single_px(gts, preds):        # batch element 0 has exactly one valid pixel, in frame 1
+    for g in gts:
+        g["valid_mask"][0] = False
+    gts[1]["valid_mask"][0, 5, 7] = True
+
+
+def _adv_planar(gts, preds):
+    """Planar steps: every view's depth is 2 (top half) or 3 (bottom half) in one common camera, so half of all values
+    tie at each of the two middle ranks; x / y are column / row constant with exact -0.0 and +0.0 columns; predictions
+    are column-constant in z.  All pixels valid: an even count, the lower median a real choice."""
+    B, H, W, _ = gts[0]["pts3d"].shape
+    col = (torch.arange(W, dtype=torch.float32) - W // 2) / 8
+    row = (torch.arange(H, dtype=torch.float32) - H // 2) / 8
+    z = torch.where(torch.arange(H)[:, None] < H // 2, 2.0, 3.0).expand(H, W)
+    for f, g in enumerate(gts):
+        x = col.expand(H, W).clone()
+        x[:, W // 2] = -0.0 if f % 2 == 0 else 0.0
+        g["pts3d"] = torch.stack((x, row[:, None].expand(H, W), z), -1).expand(B, H, W, 3).contiguous()
+        g["camera_pose"] = torch.eye(4).repeat(B, 1, 1)
+    for k in range(len(preds)):
+        for side in (0, 1):
+            p = loss_slot(preds, k, side)
+            p[..., 2] = (1.0 + torch.arange(W, dtype=torch.float32) / 4).expand(H, W)
+
+
+def _adv_nan_invalid(gts, preds):      # real depth maps: NaN (and a few +-inf) at the invalid pixels of the ground truth
+    for g in gts:
+        inv = ~g["valid_mask"]
+        g["pts3d"][inv] = float("nan")
+        idx = inv.nonzero()[:4]
+        for j, (b, i, w) in enumerate(idx.tolist()):
+            g["pts3d"][b, i, w] = float("inf") if j % 2 else -float("inf")
+
+
+def _adv_clipped_factor(gts, preds):   # batch element 0's predictions are so small that its norm factor is clipped
+    for k in range(len(preds)):
+        for side in (0, 1):
+            loss_slot(preds, k, side)[0] *= 1e-10
+
+
+def _adv_dist_clip_eq(gts, preds):
+    """Ground-truth points at exactly dist_clip = 3 from the origin and one ulp either side, forced valid: the clip
+    keeps a point at the radius (<=) and drops the next float up."""
+    up32 = float(np.nextafter(np.float32(3.0), np.float32(4.0)))
+    down32 = float(np.nextafter(np.float32(3.0), np.float32(0.0)))
+    pts = [(3, 0, 0), (0, -3, 0), (1, 2, 2), (-2, 1, -2), (up32, 0, 0), (0, 0, -up32), (down32, 0, 0), (0, down32, 0)]
+    for f, g in enumerate(gts):
+        for j, p in enumerate(pts):
+            b, i, w = j % 2, 1 + j, 2 + 2 * j + f
+            g["pts3d"][b, i, w] = torch.tensor(p, dtype=torch.float32)
+            g["valid_mask"][b, i, w] = True
+
+
+def _adv_empty_term(gts, preds):       # frame 2 has no valid pixel in any batch element
+    gts[2]["valid_mask"][:] = False
+
+
+def _adv_d_zero(gts, preds):
+    """View 0's camera at the identity, so the ground truth reaches the criterion unchanged; on even columns the
+    predictions equal it exactly (d == 0); conf exactly 1 on even rows and 1e30 on every fourth odd row."""
+    for g in gts:
+        g["pts3d"] = g["pts3d"].contiguous()
+    gts[0]["camera_pose"] = torch.eye(4).repeat(gts[0]["camera_pose"].shape[0], 1, 1)
+    for k in range(len(preds)):
+        for side in (0, 1):
+            p = loss_slot(preds, k, side)
+            p[:, :, 0::2] = gts[k + side]["pts3d"][:, :, 0::2]
+            c = preds[k][side]["conf"]
+            c[:, 0::2] = 1.0
+            c[:, 1::4] = 1e30
+
+
+# adversarial cases of tests/golden/loss_adv_<name>.npz (tools/make_golden_loss_adv.py): as LOSS_CASES, plus the edit
+# applied to make_loss_case's views and predictions (make_loss_adv_case)
+LOSS_ADV_CASES = {
+    "empty_b": {"criterion": "Regr3D_t(L21, norm_mode='avg_dis', fix_first=False)", "call": "loss", "edit": "empty_b",
+                "data": {"batch": 2, "frames": 3, "height": 16, "width": 24, "invalid": 0.3, "seed": 41}},
+    "empty_b_ssi": {"criterion": "Regr3D_t_ScaleShiftInv(L21, gt_scale=False)", "call": "pts", "edit": "empty_b",
+                    "data": {"batch": 2, "frames": 3, "height": 16, "width": 24, "invalid": 0.3, "seed": 42}},
+    "single_px": {"criterion": "Regr3D_t_ScaleShiftInv(L21, gt_scale=True)", "call": "loss", "edit": "single_px",
+                  "data": {"batch": 2, "frames": 3, "height": 16, "width": 24, "invalid": 0.3, "seed": 43}},
+    "planar": {"criterion": "Regr3D_t_ScaleShiftInv(L21, gt_scale=False)", "call": "pts", "edit": "planar",
+               "data": {"batch": 2, "frames": 3, "height": 16, "width": 24, "invalid": 0.0, "seed": 44}},
+    "planar_loss": {"criterion": "Regr3D_t_ScaleShiftInv(L21, gt_scale=True)", "call": "loss", "edit": "planar",
+                    "data": {"batch": 2, "frames": 3, "height": 16, "width": 24, "invalid": 0.0, "seed": 45}},
+    "nan_invalid": {"criterion": "ConfLoss_t(Regr3D_t(L21, norm_mode='avg_dis', fix_first=False), alpha=0.4)",
+                    "call": "loss", "edit": "nan_invalid",
+                    "data": {"batch": 2, "frames": 3, "height": 16, "width": 24, "invalid": 0.3, "seed": 46}},
+    "clipped_factor": {"criterion": "Regr3D_t(L21, norm_mode='avg_dis', fix_first=False)", "call": "loss",
+                       "edit": "clipped_factor",
+                       "data": {"batch": 2, "frames": 3, "height": 16, "width": 24, "invalid": 0.3, "seed": 47}},
+    "dist_clip_eq": {"criterion": "ConfLoss_t(Regr3D_t(L21, norm_mode='avg_log1p', fix_first=True), alpha=0.2)",
+                     "call": "loss", "kw": {"dist_clip": 3.0}, "edit": "dist_clip_eq",
+                     "data": {"batch": 2, "frames": 3, "height": 16, "width": 24, "invalid": 0.3, "seed": 48}},
+    "f2": {"criterion": "ConfLoss_t(Regr3D_t(L21, norm_mode='avg_dis', fix_first=False), alpha=0.4)", "call": "loss",
+           "edit": None, "data": {"batch": 2, "frames": 2, "height": 16, "width": 24, "invalid": 0.3, "seed": 49}},
+    "empty_term": {"criterion": "ConfLoss_t(Regr3D_t(L21, norm_mode='avg_dis', fix_first=False), alpha=0.4)",
+                   "call": "loss", "edit": "empty_term",
+                   "data": {"batch": 2, "frames": 3, "height": 16, "width": 24, "invalid": 0.3, "seed": 50}},
+    "d_zero": {"criterion": "ConfLoss_t(Regr3D_t(L21, norm_mode=False), alpha=0.4)", "call": "loss", "edit": "d_zero",
+               "data": {"batch": 2, "frames": 3, "height": 16, "width": 24, "invalid": 0.3, "seed": 51}},
+}
+
+_ADV_EDITS = {"empty_b": _adv_empty_b, "single_px": _adv_single_px, "planar": _adv_planar,
+              "nan_invalid": _adv_nan_invalid, "clipped_factor": _adv_clipped_factor,
+              "dist_clip_eq": _adv_dist_clip_eq, "empty_term": _adv_empty_term, "d_zero": _adv_d_zero}
+
+
+def make_loss_adv_case(name: str, device="cpu"):
+    """Views and `preds_all` of LOSS_ADV_CASES[name]: make_loss_case's, edited; fp32 CPU tensors (moved to `device`)."""
+    case = LOSS_ADV_CASES[name]
+    gts, preds = make_loss_case(**case["data"])
+    if case["edit"]:
+        _ADV_EDITS[case["edit"]](gts, preds)
+    if device != "cpu":
+        gts = [{k: t.to(device) for k, t in d.items()} for d in gts]
+        preds = [tuple({k: t.to(device) for k, t in d.items()} for d in p) for p in preds]
+    return gts, preds
+
+
 # ---- dataset views (spann3r_b200/views.py): golden cases of tests/golden/views.json (tools/make_golden_views.py),
 # regenerated from their parameters by the tests, and a 7Scenes-layout scene on disk for the loader tests / benchmark
 
