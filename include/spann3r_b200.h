@@ -319,6 +319,48 @@ int s3r_raster_triangles(const float* verts, int64_t n_verts, const int32_t* fac
                          void* stream);
 int s3r_raster_resolve(const void* keys, int width, int height, float* depth, int32_t* face, void* stream);
 
+/* ---- screened Poisson reconstruction: render_dtu.py's get_mesh_from_ply (Open3D's create_from_point_cloud_poisson) ---
+ * A dense-grid screened Poisson problem (definitions in spann3r_b200/csrc/poisson_math.cuh) on n samples (4 <= n < 2^31) at depth 1..10: R = 2^depth cells per side, (R + 1)^3 nodes.
+ * One caller-owned device workspace of s3r_poisson_workspace_bytes(n, depth) bytes (0 = out of range), 256-byte
+ * aligned, carries every stage; the stages run in this order on one stream:
+ *   s3r_poisson_setup: points and normals [n, 3] (fp32, or fp64 when is_f64), finite; scale >= 1.  Bounding box, cube,
+ *     sort of the samples by cell, screening blocks, right-hand side b, density grid.  info (HOST, 8 doubles) <- origin
+ *     xyz, L, h, a, beta, occupied cells.  Returns -2 when the bounding box has zero extent.  Synchronises `stream`.
+ *   s3r_poisson_solve: conjugate gradients preconditioned by a multigrid V-cycle, from chi = 0, until the TRUE relative
+ *     residual |b - A chi| / |b| <= tol; -7 after max_iter iterations.  info (HOST, 3 doubles) <- iterations, relative
+ *     residual, iso value (mean of chi at the samples).  Synchronises `stream` once per dot product.
+ *   s3r_poisson_extract_count: sizes (HOST, 2) <- vertex and face counts of the marching-tetrahedra surface.
+ *     Synchronises `stream` (one device -> host read).
+ *   s3r_poisson_extract: vertices [V, 3] fp32, faces [F, 3] int64 (wound outward for outward normals), densities [V]
+ *     fp64 (the sample density of the depth max(depth - 2, 1) grid, interpolated at each vertex).
+ * s3r_poisson_offset(n, depth, which): byte offset into the workspace of 0 sorted sample order (int32 [n]), 1 b,
+ *   2 chi (fp64 [(R + 1)^3]), 3 screening blocks (fp64 [n, 8, 8], cell c's block at the slot of its first sorted
+ *   sample), 4 / 5 the cells' first / one-past-last sorted sample (int32 [R^3]), 6 density grid, 7 header;
+ *   (size_t)-1 when out of range.
+ * s3r_pcl_quantile: out[0] (device) <- np.quantile(x, q) (method 'linear', bit for bit) of non-negative fp64 x [n], by two
+ *   exact order statistics; workspace: s3r_pcl_stats_workspace_bytes() bytes.
+ * Open3D's remove_vertices_by_mask: mask [n_verts] uint8 (1 = remove), faces [n_faces, 3] int64.
+ *   s3r_mesh_compact_workspace_bytes(n_verts, n_faces): workspace bytes (0 = out of range; n_verts >= 1), 256-byte aligned.
+ *   s3r_mesh_compact_count: sizes (HOST, 2) <- kept vertices and kept faces (every index kept).  Synchronises `stream`.
+ *   s3r_mesh_compact: kept vertices [.., 3] fp32 in order, kept faces renumbered, in order. */
+size_t s3r_poisson_workspace_bytes(int64_t n, int depth);
+size_t s3r_poisson_offset(int64_t n, int depth, int which);
+int s3r_poisson_setup(const void* points, const void* normals, int is_f64, int64_t n, int depth, double scale,
+                      void* workspace, size_t workspace_bytes, double* info, void* stream);
+int s3r_poisson_solve(int64_t n, int depth, double tol, int max_iter, void* workspace, size_t workspace_bytes,
+                      double* info, void* stream);
+int s3r_poisson_extract_count(int64_t n, int depth, void* workspace, size_t workspace_bytes, int64_t* sizes,
+                              void* stream);
+int s3r_poisson_extract(int64_t n, int depth, void* workspace, size_t workspace_bytes, float* vertices, int64_t* faces,
+                        double* densities, void* stream);
+int s3r_pcl_quantile(const double* x, int64_t n, double q, void* workspace, double* out, void* stream);
+size_t s3r_mesh_compact_workspace_bytes(int64_t n_verts, int64_t n_faces);
+int s3r_mesh_compact_count(const uint8_t* mask, const int64_t* faces, int64_t n_verts, int64_t n_faces, void* workspace,
+                           size_t workspace_bytes, int64_t* sizes, void* stream);
+int s3r_mesh_compact(const float* vertices, const int64_t* faces, int64_t n_verts, int64_t n_faces,
+                     const void* workspace, size_t workspace_bytes, float* out_vertices, int64_t* out_faces,
+                     void* stream);
+
 /* ---- training / test criteria: spann3r/loss.py:129-369 (Regr3D_t, its ShiftInv / ScaleInv / ScaleShiftInv variants,
  * ConfLoss_t) with L21 (dust3r/losses.py:52-59), forward and backward --------------------------------------------------
  * F >= 2 views of B sequences of H x W pixels.  Pred slot k < F-1 is preds_all[k][0] (frame k: 'pts3d' for k = 0, else

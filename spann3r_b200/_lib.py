@@ -110,6 +110,16 @@ _PROTOS = {
     "s3r_mesh_grid_faces": (_i, [_vp, _vp, _i, _i, _i, _vp, C.c_size_t, _vp, _vp, _vp]),
     "s3r_raster_triangles": (_i, [_vp, _i64, _vp, _i64, _i64, _vp, C.c_double, C.c_double, _i, _i, _vp, _vp]),
     "s3r_raster_resolve": (_i, [_vp, _i, _i, _vp, _vp, _vp]),
+    "s3r_poisson_workspace_bytes": (C.c_size_t, [_i64, _i]),
+    "s3r_poisson_offset": (C.c_size_t, [_i64, _i, _i]),
+    "s3r_poisson_setup": (_i, [_vp, _vp, _i, _i64, _i, C.c_double, _vp, C.c_size_t, _vp, _vp]),
+    "s3r_poisson_solve": (_i, [_i64, _i, C.c_double, _i, _vp, C.c_size_t, _vp, _vp]),
+    "s3r_poisson_extract_count": (_i, [_i64, _i, _vp, C.c_size_t, _vp, _vp]),
+    "s3r_poisson_extract": (_i, [_i64, _i, _vp, C.c_size_t, _vp, _vp, _vp, _vp]),
+    "s3r_pcl_quantile": (_i, [_vp, _i64, C.c_double, _vp, _vp, _vp]),
+    "s3r_mesh_compact_workspace_bytes": (C.c_size_t, [_i64, _i64]),
+    "s3r_mesh_compact_count": (_i, [_vp, _vp, _i64, _i64, _vp, C.c_size_t, _vp, _vp]),
+    "s3r_mesh_compact": (_i, [_vp, _vp, _i64, _i64, _vp, C.c_size_t, _vp, _vp, _vp]),
     "s3r_loss_workspace_bytes": (C.c_size_t, [C.POINTER(LossDesc)]),
     "s3r_loss_forward": (_i, [C.POINTER(LossDesc), _vp, C.c_size_t, _vp, _vp, _vp, _vp, _vp]),
     "s3r_loss_backward": (_i, [C.POINTER(LossDesc), _vp, C.c_size_t, _vp, _vp, _vp, _vp]),

@@ -193,6 +193,44 @@ int s3r_raster_resolve(const void* keys, int width, int height, float* depth, in
   return launch_raster_resolve(keys, width, height, depth, face, S(stream));
 }
 
+size_t s3r_poisson_workspace_bytes(int64_t n, int depth) { return poisson_workspace_bytes(n, depth); }
+size_t s3r_poisson_offset(int64_t n, int depth, int which) { return poisson_offset(n, depth, which); }
+int s3r_poisson_setup(const void* points, const void* normals, int is_f64, int64_t n, int depth, double scale,
+                      void* workspace, size_t workspace_bytes, double* info, void* stream) {
+  return launch_poisson_setup(points, normals, is_f64, n, depth, scale, workspace, workspace_bytes, info, S(stream));
+}
+int s3r_poisson_solve(int64_t n, int depth, double tol, int max_iter, void* workspace, size_t workspace_bytes,
+                      double* info, void* stream) {
+  return launch_poisson_solve(n, depth, tol, max_iter, workspace, workspace_bytes, info, S(stream));
+}
+int s3r_poisson_extract_count(int64_t n, int depth, void* workspace, size_t workspace_bytes, int64_t* sizes,
+                              void* stream) {
+  return launch_poisson_extract_count(n, depth, workspace, workspace_bytes, reinterpret_cast<long long*>(sizes),
+                                      S(stream));
+}
+int s3r_poisson_extract(int64_t n, int depth, void* workspace, size_t workspace_bytes, float* vertices, int64_t* faces,
+                        double* densities, void* stream) {
+  return launch_poisson_extract(n, depth, workspace, workspace_bytes, vertices, reinterpret_cast<long long*>(faces),
+                                densities, S(stream));
+}
+int s3r_pcl_quantile(const double* x, int64_t n, double q, void* workspace, double* out, void* stream) {
+  return launch_pcl_quantile(x, n, q, workspace, out, S(stream));
+}
+size_t s3r_mesh_compact_workspace_bytes(int64_t n_verts, int64_t n_faces) {
+  return mesh_compact_workspace_bytes(n_verts, n_faces);
+}
+int s3r_mesh_compact_count(const uint8_t* mask, const int64_t* faces, int64_t n_verts, int64_t n_faces, void* workspace,
+                           size_t workspace_bytes, int64_t* sizes, void* stream) {
+  return launch_mesh_compact_count(mask, reinterpret_cast<const long long*>(faces), n_verts, n_faces, workspace,
+                                   workspace_bytes, reinterpret_cast<long long*>(sizes), S(stream));
+}
+int s3r_mesh_compact(const float* vertices, const int64_t* faces, int64_t n_verts, int64_t n_faces,
+                     const void* workspace, size_t workspace_bytes, float* out_vertices, int64_t* out_faces,
+                     void* stream) {
+  return launch_mesh_compact(vertices, reinterpret_cast<const long long*>(faces), n_verts, n_faces, workspace,
+                             workspace_bytes, out_vertices, reinterpret_cast<long long*>(out_faces), S(stream));
+}
+
 size_t s3r_loss_workspace_bytes(const s3r_loss_desc* d) { return loss_workspace_bytes(d); }
 int s3r_loss_forward(const s3r_loss_desc* d, void* workspace, size_t workspace_bytes, float* gt_out, float* pred_out,
                      uint8_t* valid_out, double* results, void* stream) {

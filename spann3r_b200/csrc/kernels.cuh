@@ -124,6 +124,15 @@ int launch_pcl_icp(const void* src, int f64, long long ns, const void* target_in
 size_t pcl_stats_workspace_bytes();
 int launch_pcl_stats(const double* v, long long n, double threshold, void* workspace, double* out, cudaStream_t st);
 int launch_pcl_abs_dot(const double* a, const double* b, const long long* idx, long long n, double* out, cudaStream_t st);
+// order statistics of ranks r0, r1 of non-negative fp64 values, exact; *picked <- device pointer to the two values
+// inside the workspace (pcl_stats_workspace_bytes())
+int launch_pcl_select_ranks(const double* v, long long n, long long r0, long long r1, void* workspace,
+                            const double** picked, cudaStream_t st);
+// stable LSD radix sort of (key, value) over `passes` 8-bit digits, ping-ponging keys[0] <-> keys[1] (the result is in
+// keys[passes & 1]); hist: pcl_sort_hist_words(n) unsigned words
+long long pcl_sort_hist_words(long long n);
+int launch_pcl_radix_sort(uint64_t* const keys[2], int* const vals[2], long long n, int passes, unsigned* hist,
+                          cudaStream_t st);
 
 // headless point rendering (render.cu): z-buffer of w * h uint64 keys, clear / splat one frame / resolve to RGB
 size_t render_workspace_bytes(int w, int h);
@@ -143,6 +152,23 @@ int launch_raster_triangles(const float* verts, long long n_verts, const int* fa
                             const double* camera, double z_near, double z_far, int w, int h, void* keys,
                             cudaStream_t st);
 int launch_raster_resolve(const void* keys, int w, int h, float* depth, int* face, cudaStream_t st);
+
+// screened Poisson reconstruction (poisson.cu): see include/spann3r_b200.h, s3r_poisson_*
+size_t poisson_workspace_bytes(long long n, int depth);
+size_t poisson_offset(long long n, int depth, int which);
+int launch_poisson_setup(const void* pts, const void* nrm, int f64, long long n, int depth, double scale, void* ws,
+                         size_t ws_bytes, double* info, cudaStream_t st);
+int launch_poisson_solve(long long n, int depth, double tol, int max_iter, void* ws, size_t ws_bytes, double* info,
+                         cudaStream_t st);
+int launch_poisson_extract_count(long long n, int depth, void* ws, size_t ws_bytes, long long* sizes, cudaStream_t st);
+int launch_poisson_extract(long long n, int depth, void* ws, size_t ws_bytes, float* verts, long long* faces,
+                           double* dens, cudaStream_t st);
+int launch_pcl_quantile(const double* x, long long n, double q, void* workspace, double* out, cudaStream_t st);
+size_t mesh_compact_workspace_bytes(long long n_verts, long long n_faces);
+int launch_mesh_compact_count(const uint8_t* mask, const long long* faces, long long n_verts, long long n_faces,
+                              void* ws, size_t ws_bytes, long long* sizes, cudaStream_t st);
+int launch_mesh_compact(const float* verts, const long long* faces, long long n_verts, long long n_faces, const void* ws,
+                        size_t ws_bytes, float* out_verts, long long* out_faces, cudaStream_t st);
 
 // conv backward (conv_wgrad.cu): weight gradient over pixels (split-bf16 wgmma, split contraction + fixed-order reduce)
 // and the col2im of the 3x3 stride-2 conv; both validate their arguments before any CUDA call

@@ -19,6 +19,8 @@
 //   per-pass sums in a fixed block order relative to the target's box centre, the Umeyama update on one thread.
 //   Statistics of an fp64 vector: fixed-order mean, exact median by a 64-bit radix select (8 x 8-bit passes on the bit
 //   pattern, which orders like the value for non-negative doubles once -0.0 is keyed as +0.0), count below a threshold.
+//   The select takes any two ranks (launch_pcl_select_ranks), and the stable radix sort any number of 8-bit passes
+//   (launch_pcl_radix_sort); csrc/poisson.cu uses both.
 #include "kernels.cuh"
 
 #include <climits>
@@ -538,7 +540,8 @@ struct SelectState {
 struct StatsWs {
   double sum[kStatBlocks];
   unsigned long long below[kStatBlocks];
-  SelectState sel[2];   // ranks (n - 1) / 2 and n / 2: np.median's two middle order statistics
+  SelectState sel[2];   // two ranks at once (the median: (n - 1) / 2 and n / 2)
+  double picked[2];     // the two order statistics, after pcl_select_done
 };
 
 __global__ void __launch_bounds__(256) pcl_stats_partial(const double* __restrict__ x, long long n, double thr,
@@ -585,15 +588,19 @@ __global__ void __launch_bounds__(256) pcl_select_hist(const double* __restrict_
   if (h[threadIdx.x]) atomicAdd(&S.hist[threadIdx.x], h[threadIdx.x]);
 }
 
-__global__ void __launch_bounds__(32) pcl_select_pick(long long n, int pass, StatsWs* ws) {
+__global__ void __launch_bounds__(32) pcl_select_pick(long long r0, long long r1, int pass, StatsWs* ws) {
   if (threadIdx.x >= 2) return;
   SelectState& S = ws->sel[threadIdx.x];
-  unsigned long long k = pass == 0 ? (unsigned long long)(threadIdx.x == 0 ? (n - 1) / 2 : n / 2) : S.k;
+  unsigned long long k = pass == 0 ? (unsigned long long)(threadIdx.x == 0 ? r0 : r1) : S.k;
   int bin = 0;
   while (bin < 255 && k >= S.hist[bin]) k -= S.hist[bin++];
   S.prefix = (S.prefix << 8) | (unsigned long long)bin;
   S.k = k;
   for (int i = 0; i < 256; ++i) S.hist[i] = 0;
+}
+
+__global__ void __launch_bounds__(32) pcl_select_done(StatsWs* ws) {
+  if (threadIdx.x < 2) ws->picked[threadIdx.x] = __longlong_as_double((long long)ws->sel[threadIdx.x].prefix);
 }
 
 __global__ void __launch_bounds__(32) pcl_stats_final(long long n, const StatsWs* ws, double* __restrict__ out) {
@@ -623,6 +630,15 @@ __global__ void __launch_bounds__(256) pcl_abs_dot_kernel(const double* __restri
 }
 
 bool n_ok(long long n) { return n >= 1 && n < (1LL << 31); }
+
+// Exact order statistics of ranks r0 and r1 (0-based) into ws->sel[0 / 1].prefix, as bit patterns.
+void select_ranks(const double* v, long long n, long long r0, long long r1, StatsWs* ws, cudaStream_t st) {
+  cudaMemsetAsync(ws->sel, 0, sizeof(ws->sel), st);
+  for (int pass = 0; pass < 8; ++pass) {
+    pcl_select_hist<<<dim3(kStatBlocks, 2), 256, 0, st>>>(v, n, pass, ws);
+    pcl_select_pick<<<1, 32, 0, st>>>(r0, r1, pass, ws);
+  }
+}
 
 // The largest squared distance whose sqrt is <= max_dist: the bound is inclusive on the DISTANCE, as the caller sees it
 // (sqrt rounds, so max_dist * max_dist alone can drop a point at exactly max_dist).
@@ -732,14 +748,41 @@ int launch_pcl_stats(const double* v, long long n, double threshold, void* works
     return -1;
   }
   StatsWs* ws = (StatsWs*)workspace;
-  cudaMemsetAsync(ws->sel, 0, sizeof(ws->sel), st);
   pcl_stats_partial<<<kStatBlocks, 256, 0, st>>>(v, n, threshold, ws);
-  for (int pass = 0; pass < 8; ++pass) {
-    pcl_select_hist<<<dim3(kStatBlocks, 2), 256, 0, st>>>(v, n, pass, ws);
-    pcl_select_pick<<<1, 32, 0, st>>>(n, pass, ws);
-  }
+  select_ranks(v, n, (n - 1) / 2, n / 2, ws, st);
   pcl_stats_final<<<1, 32, 0, st>>>(n, ws, out);
   return launched("pcl_stats");
+}
+
+int launch_pcl_select_ranks(const double* v, long long n, long long r0, long long r1, void* workspace,
+                            const double** picked, cudaStream_t st) {
+  if (!v || !workspace || !picked || !n_ok(n) || r0 < 0 || r1 < 0 || r0 >= n || r1 >= n) {
+    set_error("pcl_select_ranks: bad arguments (n=%lld r0=%lld r1=%lld)", n, r0, r1);
+    return -1;
+  }
+  StatsWs* ws = (StatsWs*)workspace;
+  select_ranks(v, n, r0, r1, ws, st);
+  pcl_select_done<<<1, 32, 0, st>>>(ws);
+  *picked = ws->picked;
+  return launched("pcl_select_ranks");
+}
+
+long long pcl_sort_hist_words(long long n) { return 256LL * ((n + kSortTile - 1) / kSortTile); }
+
+int launch_pcl_radix_sort(uint64_t* const keys[2], int* const vals[2], long long n, int passes, unsigned* hist,
+                          cudaStream_t st) {
+  if (!keys[0] || !keys[1] || !vals[0] || !vals[1] || !hist || !n_ok(n) || passes < 1 || passes > 8) {
+    set_error("pcl_radix_sort: bad arguments (n=%lld passes=%d)", n, passes);
+    return -1;
+  }
+  const int nblk = (int)((n + kSortTile - 1) / kSortTile);
+  for (int pass = 0; pass < passes; ++pass) {
+    const int a = pass & 1;
+    pcl_sort_hist<<<nblk, 256, 0, st>>>(keys[a], n, 8 * pass, nblk, hist);
+    pcl_sort_scan<<<1, 1024, 0, st>>>(hist, 256LL * nblk);
+    pcl_sort_scatter<<<nblk, 256, 0, st>>>(keys[a], vals[a], n, 8 * pass, nblk, hist, keys[a ^ 1], vals[a ^ 1]);
+  }
+  return launched("pcl_radix_sort");
 }
 
 int launch_pcl_abs_dot(const double* a, const double* b, const long long* idx, long long n, double* out, cudaStream_t st) {

@@ -386,13 +386,9 @@ def _ply_type(t, path):
     return _PLY_TYPES[t]
 
 
-def read_ply_mesh(path: str):
-    """A triangle mesh PLY (ASCII or binary little-endian) -> (vertices [N, 3] fp32, faces [F, 3] int64).
-
-    The vertex element needs float or double x, y, z; its other scalar properties are skipped by their declared type.
-    The optional face element holds one list property `vertex_indices` (or `vertex_index`) of three indices per face.
-    Anything else (another format, element or face property, a list on the vertex, a non-triangle, an index out of
-    range, a truncated body) raises ValueError."""
+def _ply_header(path: str):
+    """-> (file bytes, format, [(element name, count, [property tuples])], offset of the body).  ASCII and binary
+    little-endian only; anything else in the header raises ValueError."""
     with open(path, "rb") as fh:
         data = fh.read()
     end = data.find(b"end_header")
@@ -417,6 +413,17 @@ def read_ply_mesh(path: str):
             raise ValueError(f"{path}: malformed header line {line!r}")
     if fmt is None:
         raise ValueError(f"{path}: no format line")
+    return data, fmt, elements, body_at
+
+
+def read_ply_mesh(path: str):
+    """A triangle mesh PLY (ASCII or binary little-endian) -> (vertices [N, 3] fp32, faces [F, 3] int64).
+
+    The vertex element needs float or double x, y, z; its other scalar properties are skipped by their declared type.
+    The optional face element holds one list property `vertex_indices` (or `vertex_index`) of three indices per face.
+    Anything else (another format, element or face property, a list on the vertex, a non-triangle, an index out of
+    range, a truncated body) raises ValueError."""
+    data, fmt, elements, body_at = _ply_header(path)
     names = [e[0] for e in elements]
     if "vertex" not in names or len(set(names)) != len(names) or not set(names) <= {"vertex", "face"}:
         raise ValueError(f"{path}: expected a vertex element and at most a face element, got {names}")
@@ -479,3 +486,206 @@ def read_ply_mesh(path: str):
     if f.size and (f.min() < 0 or f.max() >= len(v)):
         raise ValueError(f"{path}: face indices out of range")
     return v.astype(np.float32), f
+
+
+def read_point_cloud(path: str):
+    """An oriented point cloud PLY (ASCII or binary little-endian), as render_dtu.py's `o3d.io.read_point_cloud` reads
+    DTU's stl*_total.ply -> (points [N, 3] fp64, normals [N, 3] fp64), numpy.
+
+    The vertex element comes first and has float or double x, y, z, nx, ny, nz; its other scalar properties are skipped
+    by their declared type, and elements after it are not read.  A cloud without normals raises ValueError (Open3D's
+    Poisson reconstruction refuses one), as do a list property on the vertex, another format and a truncated body."""
+    data, fmt, elements, body_at = _ply_header(path)
+    if not elements or elements[0][0] != "vertex" or elements[0][1] < 0:
+        raise ValueError(f"{path}: expected the vertex element first, got {[e[0] for e in elements]}")
+    _, count, props = elements[0]
+    if any(p[0] == "list" for p in props):
+        raise ValueError(f"{path}: list properties on vertices are not supported")
+    names = [p[1] for p in props]
+    if len(set(names)) != len(names) or not {"x", "y", "z"} <= set(names) or \
+            any(_ply_type(p[0], path) not in ("f4", "f8") for p in props if p[1] in ("x", "y", "z", "nx", "ny", "nz")):
+        raise ValueError(f"{path}: vertices need float or double x, y, z")
+    if not {"nx", "ny", "nz"} <= set(names):
+        raise ValueError(f"{path}: the point cloud has no normals (nx, ny, nz); Poisson reconstruction needs them")
+    cols = ("x", "y", "z", "nx", "ny", "nz")
+    if fmt == "binary_little_endian":
+        dt = np.dtype([(p[1], "<" + _ply_type(p[0], path)) for p in props])
+        if body_at + count * dt.itemsize > len(data):
+            raise ValueError(f"{path}: truncated vertex data")
+        rec = np.frombuffer(data, dt, count, body_at)
+        out = np.stack([rec[a].astype(np.float64) for a in cols], 1) if count else np.zeros((0, 6))
+    else:
+        rows = [r.split() for r in data[body_at:].decode("ascii", "replace").splitlines() if r.strip()][:count]
+        if len(rows) < count or any(len(r) != len(props) for r in rows):
+            raise ValueError(f"{path}: truncated or malformed vertex data")
+        idx = [names.index(a) for a in cols]
+        try:
+            out = np.array([[float(r[i]) for i in idx] for r in rows], np.float64).reshape(-1, 6)
+        except ValueError as ex:
+            raise ValueError(f"{path}: malformed vertex data: {ex}")
+    return np.ascontiguousarray(out[:, :3]), np.ascontiguousarray(out[:, 3:])
+
+
+def write_ply_mesh(path: str, vertices, faces) -> None:
+    """Binary little-endian PLY of a triangle mesh: `double x y z` (the layout vis.write_point_cloud writes) and faces
+    as `list uchar int vertex_indices`.  read_ply_mesh reads it back exactly.  Tensors on any device or arrays."""
+    v = np.ascontiguousarray(_host(vertices, "vertices"), np.float64).reshape(-1, 3)
+    f = _host(faces, "faces").reshape(-1, 3)
+    if not np.issubdtype(f.dtype, np.integer) or (f.size and (f.min() < 0 or f.max() >= len(v))) or \
+            len(v) >= 2 ** 31 or not np.isfinite(v).all():
+        raise ValueError(f"write_ply_mesh: expected finite vertices and integer faces indexing them, got "
+                         f"{v.shape}, {f.shape} {f.dtype}")
+    rec = np.empty(len(f), np.dtype([("n", "u1"), ("i", "<i4", 3)]))
+    rec["n"] = 3
+    rec["i"] = f
+    header = (f"ply\nformat binary_little_endian 1.0\nelement vertex {len(v)}\n"
+              + "".join(f"property double {a}\n" for a in "xyz")
+              + f"element face {len(f)}\nproperty list uchar int vertex_indices\nend_header\n")
+    with open(path, "wb") as fh:
+        fh.write(header.encode("ascii"))
+        fh.write(v.astype("<f8").tobytes())
+        fh.write(rec.tobytes())
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# Screened Poisson reconstruction (render_dtu.py's get_mesh_from_ply)
+# ----------------------------------------------------------------------------------------------------------------------
+POISSON_TOL = 1e-8          # relative residual |b - A chi| / |b| at which the solve stops
+POISSON_MAX_ITER = 500      # conjugate-gradient iterations before the solve raises
+
+
+class _Poisson:
+    """The device workspace of one reconstruction after setup and solve: the screening blocks, b, chi, the iso value
+    and the density grid stay on the device for extraction (and for the tests)."""
+
+    def __init__(self, points, normals, depth, scale):
+        if isinstance(depth, bool) or not isinstance(depth, (int, np.integer)) or not 1 <= int(depth) <= 10:
+            raise ValueError(f"depth: expected an int in 1..10, got {depth!r}")
+        scale = float(scale)
+        if not (math.isfinite(scale) and scale >= 1.0):
+            raise ValueError(f"scale: expected a finite value >= 1, got {scale}")
+        p = _cuda(points, "points", (torch.float32, torch.float64), 3, 2)
+        n = _cuda(normals, "normals", (torch.float32, torch.float64), 3, 2)
+        if n.shape != p.shape or n.device != p.device:
+            raise ValueError(f"normals {tuple(n.shape)} on {n.device} must match points {tuple(p.shape)} on {p.device}")
+        if p.dtype != n.dtype:
+            p, n = p.double(), n.double()
+        N = len(p)
+        if N < 4 or N >= 2 ** 31:
+            raise ValueError(f"points: expected 4 <= N < 2^31 samples, got {N}")
+        if not bool(torch.isfinite(p).all()) or not bool(torch.isfinite(n).all()):
+            raise ValueError("points / normals: non-finite values")
+        if float((p.amax(0) - p.amin(0)).max()) == 0.0:
+            raise ValueError("points: the bounding box has zero extent")
+        _lib.require_device()
+        L = _lib.lib()
+        self.n, self.depth, self.device = N, int(depth), p.device
+        self.ws_bytes = int(L.s3r_poisson_workspace_bytes(N, self.depth))
+        self.ws = torch.empty(self.ws_bytes, dtype=torch.uint8, device=self.device)
+        info = np.zeros(8, np.float64)
+        out = np.zeros(3, np.float64)
+        with _lib.on_device(self.device):
+            st = _lib.stream_ptr(self.device)
+            _lib.check(L.s3r_poisson_setup(_lib.ptr(p), _lib.ptr(n), int(p.dtype == torch.float64), N, self.depth, scale,
+                                           _lib.ptr(self.ws), self.ws_bytes, C.c_void_p(info.ctypes.data), st),
+                       "s3r_poisson_setup")
+            _lib.check(L.s3r_poisson_solve(N, self.depth, POISSON_TOL, POISSON_MAX_ITER, _lib.ptr(self.ws), self.ws_bytes,
+                                           C.c_void_p(out.ctypes.data), st), "s3r_poisson_solve")
+        self.origin, self.L, self.h = info[:3].copy(), float(info[3]), float(info[4])
+        self.a, self.beta, self.occupied = float(info[5]), float(info[6]), int(info[7])
+        self.iterations, self.residual, self.iso = int(out[0]), float(out[1]), float(out[2])
+
+    def view(self, which: int, dtype, count: int) -> torch.Tensor:
+        """One array of the workspace (s3r_poisson_offset's `which`), as a tensor sharing its memory."""
+        off = int(_lib.lib().s3r_poisson_offset(self.n, self.depth, which))
+        nbytes = count * torch.empty((), dtype=dtype).element_size()
+        return self.ws[off:off + nbytes].view(dtype)
+
+    def extract(self):
+        L = _lib.lib()
+        sizes = np.zeros(2, np.int64)
+        with _lib.on_device(self.device):
+            st = _lib.stream_ptr(self.device)
+            _lib.check(L.s3r_poisson_extract_count(self.n, self.depth, _lib.ptr(self.ws), self.ws_bytes,
+                                                   C.c_void_p(sizes.ctypes.data), st), "s3r_poisson_extract_count")
+            nv, nf = int(sizes[0]), int(sizes[1])
+            v = torch.empty((nv, 3), dtype=torch.float32, device=self.device)
+            f = torch.empty((nf, 3), dtype=torch.int64, device=self.device)
+            d = torch.empty(nv, dtype=torch.float64, device=self.device)
+            _lib.check(L.s3r_poisson_extract(self.n, self.depth, _lib.ptr(self.ws), self.ws_bytes, _lib.ptr(v), _lib.ptr(f),
+                                             _lib.ptr(d), st), "s3r_poisson_extract")
+        return v, f, d
+
+
+def create_from_point_cloud_poisson(points, normals, depth=8, scale=1.1):
+    """Open3D's `TriangleMesh.create_from_point_cloud_poisson(pcd, depth, scale=scale)` on the device, as a dense-grid
+    screened Poisson reconstruction (the problem: csrc/poisson_math.cuh; differences from Open3D: INTEGRATION.md).
+
+    points, normals: CUDA [N, 3] fp32 or fp64 (N >= 4, finite, a bounding box of non-zero extent); depth: 1..10 (a
+    (2^depth + 1)^3 grid); scale >= 1: the cube's side over the bounding box's largest extent.  Returns CUDA tensors
+    (vertices [V, 3] fp32, faces [F, 3] int64 wound outward for outward normals, densities [V] fp64: samples per unit
+    volume on the depth max(depth - 2, 1) grid, interpolated at each vertex).  Bitwise reproducible."""
+    return _Poisson(points, normals, depth, scale).extract()
+
+
+def remove_vertices_by_mask(vertices, faces, mask):
+    """Open3D's `TriangleMesh.remove_vertices_by_mask` on the device: drops the vertices where mask [V] (bool) is true and
+    every face that uses one, renumbering the survivors in their order; faces keep theirs.  vertices [V, 3] fp32,
+    faces [F, 3] int64 CUDA tensors -> (vertices, faces)."""
+    v = _cuda(vertices, "vertices", (torch.float32,), 3, 2)
+    f = _cuda(faces, "faces", (torch.int64,), 3, 2)
+    if not isinstance(mask, torch.Tensor) or mask.dtype != torch.bool or tuple(mask.shape) != (len(v),) or \
+            mask.device != v.device or f.device != v.device:
+        raise ValueError(f"mask: expected a bool tensor ({len(v)},) on {v.device}")
+    if len(v) == 0 or len(v) >= 2 ** 31 or len(f) >= 2 ** 31:
+        raise ValueError(f"expected 1 <= V < 2^31 vertices and F < 2^31 faces, got {len(v)}, {len(f)}")
+    if len(f) and (int(f.min()) < 0 or int(f.max()) >= len(v)):
+        raise ValueError(f"faces: indices must lie in [0, {len(v)})")
+    _lib.require_device()
+    L = _lib.lib()
+    m = mask.contiguous().view(torch.uint8)
+    ws_bytes = int(L.s3r_mesh_compact_workspace_bytes(len(v), len(f)))
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=v.device)
+    sizes = np.zeros(2, np.int64)
+    with _lib.on_device(v.device):
+        st = _lib.stream_ptr(v.device)
+        _lib.check(L.s3r_mesh_compact_count(_lib.ptr(m), _lib.ptr(f), len(v), len(f), _lib.ptr(ws), ws_bytes,
+                                            C.c_void_p(sizes.ctypes.data), st), "s3r_mesh_compact_count")
+        ov = torch.empty((int(sizes[0]), 3), dtype=torch.float32, device=v.device)
+        of = torch.empty((int(sizes[1]), 3), dtype=torch.int64, device=v.device)
+        _lib.check(L.s3r_mesh_compact(_lib.ptr(v), _lib.ptr(f), len(v), len(f), _lib.ptr(ws), ws_bytes, _lib.ptr(ov),
+                                      _lib.ptr(of), st), "s3r_mesh_compact")
+    return ov, of
+
+
+def quantile(x, q) -> torch.Tensor:
+    """np.quantile(x, q) (method 'linear') of a non-negative fp64 CUDA vector, bit for bit, by two exact order
+    statistics on the device -> a 1-element fp64 CUDA tensor."""
+    x = _cuda(x, "x", (torch.float64,), None, 1)
+    q = float(q)
+    if not (0.0 <= q <= 1.0) or len(x) == 0 or len(x) >= 2 ** 31:
+        raise ValueError(f"quantile: need 0 <= q <= 1 and 1 <= len(x) < 2^31, got {q}, {len(x)}")
+    _lib.require_device()
+    L = _lib.lib()
+    ws = torch.empty(int(L.s3r_pcl_stats_workspace_bytes()), dtype=torch.uint8, device=x.device)
+    out = torch.empty(1, dtype=torch.float64, device=x.device)
+    with _lib.on_device(x.device):
+        _lib.check(L.s3r_pcl_quantile(_lib.ptr(x), len(x), q, _lib.ptr(ws), _lib.ptr(out), _lib.stream_ptr(x.device)),
+                   "s3r_pcl_quantile")
+    return out
+
+
+def get_mesh_from_ply(path_to_scan, depth=9, density_thresh=0.1, device="cuda"):
+    """render_dtu.py's `get_mesh_from_ply`: reads the scan's `stl{scan:03d}_total.ply`, reconstructs it at `depth`,
+    removes the vertices whose density is below `np.quantile(densities, density_thresh)` and writes
+    `{scan:03d}_pcd.ply`, the mesh `render_dtu_scenes(path_to_scan, method=None)` renders.  Returns (vertices, faces)
+    of the trimmed mesh as CUDA tensors."""
+    scan_id = int("".join(filter(str.isdigit, os.path.basename(path_to_scan))))
+    pts, nrm = read_point_cloud(os.path.join(path_to_scan, f"stl{scan_id:03d}_total.ply"))
+    _lib.require_device()
+    v, f, dens = create_from_point_cloud_poisson(torch.from_numpy(pts).to(device), torch.from_numpy(nrm).to(device),
+                                                 depth=depth)
+    if len(v):
+        v, f = remove_vertices_by_mask(v, f, dens < quantile(dens, density_thresh))
+    write_ply_mesh(os.path.join(path_to_scan, f"{scan_id:03d}_pcd.ply"), v, f)
+    return v, f
