@@ -208,7 +208,8 @@ int s3r_resample_v_u8_norm(const uint8_t* tmp, int cols, int out_rows, const int
 /* ---- post-path geometry (SURVEY.md section 8f rank 4, first step) ---------------------------------------------------
  * dust3r/post_process.py:12-60 estimate_focal_knowing_depth(pts3d, pp, focal_mode='weiszfeld') as demo.py:148-150 calls
  * it: pts3d [b, h, w, 3] fp32 (device), principal point (ppx, ppy), `iters` re-weighting rounds (the reference: 10),
- * result clipped to [lo, hi] -> focal [b] (device).  scratch: b * 148 * 2 floats.  Deterministic. */
+ * result clipped to [lo, hi] -> focal [b] (device).  scratch: b * 148 * 2 floats.  Deterministic.  A frame with no usable
+ * x / z (every z = 0, every point NaN) gives NaN, as the reference does: the weight floor and the clip keep NaN. */
 int s3r_focal_weiszfeld(const float* pts3d, int b, int h, int w, float ppx, float ppy, int iters, float lo, float hi,
                         float* scratch, float* focal, void* stream);
 
@@ -225,7 +226,8 @@ int s3r_focal_median(const float* pts3d, int b, int h, int w, float ppx, float p
  * (cv2's default 8.0) over all n points, then `refine_iters` damped Gauss-Newton rounds on the best model's inliers
  * (cv2's final SOLVEPNP_ITERATIVE refinement solves the same least-squares problem).
  *   pts3d [b, n, 3] fp32; img_pts [b, n, 2] fp32 or NULL = the dense pixel grid (u = i % width, v = i / width);
- *   out [b, 18] fp64: R (9, row-major, x_cam = R x + t), t (3), rvec (3, Rodrigues), inlier count of the RANSAC model,
+ *   out [b, 18] fp64: R (9, row-major, x_cam = R x + t), t (3), rvec (3, Rodrigues), inlier count of the RANSAC model
+ *   (0 when it fails: the count of the mask returned),
  *   RMS reprojection error after refinement (px), success (1/0);  inlier_mask [b, n] uint8 (cv2's `inliers`, as a mask);
  *   workspace: s3r_pnp_workspace_bytes(b, n_samples) bytes, 16-byte aligned.  Deterministic for a given seed. */
 size_t s3r_pnp_workspace_bytes(int b, int n_samples);

@@ -5,6 +5,8 @@
 //   a = (x/z, y/z) with non-finite values -> 0,  p = (i - ppx, j - ppy)
 //   f0 = sum(a.p) / sum(a.a);   10 x:  w = 1 / max(|p - f a|, 1e-8),  f = sum(w a.p) / sum(w a.a)
 //
+// NaN propagates as in the reference's torch ops: a frame with no usable x / z (every z = 0, every point NaN) gives
+// f0 = 0 / 0 and returns NaN, through the weight floor and the final clip alike.
 // (the reference's means cancel in the ratio).  Each iteration is two fixed-shape launches -- 148 x 256-thread partial
 // sums per image in a fixed order, then one block per image -- so the result is deterministic; the pointmap
 // (2.4 MB at 512 x 384) stays in L2 across the 11 passes and never crosses PCIe.
@@ -38,7 +40,8 @@ __global__ void __launch_bounds__(256) focal_partial_kernel(const float* __restr
     float w = 1.f;
     if (!first) {
       const float du = u - f * ax, dv = v - f * ay;
-      w = 1.0f / fmaxf(sqrtf(du * du + dv * dv), 1e-8f);
+      const float dis = sqrtf(du * du + dv * dv);
+      w = 1.0f / (dis < 1e-8f ? 1e-8f : dis);   // dis.clip(min=1e-8): a NaN distance stays NaN (fmaxf would drop it)
     }
     s_px += w * d_px;
     s_xx += w * d_xx;
@@ -77,7 +80,10 @@ __global__ void __launch_bounds__(256) focal_final_kernel(const float* __restric
   }
   if (threadIdx.x == 0) {
     float f = r0[0] / r1[0];
-    if (last) f = fminf(fmaxf(f, lo), hi);   // focal.clip(min_focal * base, max_focal * base)
+    if (last) {   // focal.clip(min_focal * base, max_focal * base): a NaN focal (no usable x / z) stays NaN
+      f = f < lo ? lo : f;
+      f = f > hi ? hi : f;
+    }
     focal[b] = f;
   }
 }

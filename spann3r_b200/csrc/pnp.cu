@@ -243,7 +243,7 @@ __global__ void __launch_bounds__(32) pnp_gn_update_kernel(const double* __restr
     for (int i = 0; i < 9; ++i) o[i] = G.R[i];
     for (int i = 0; i < 3; ++i) o[9 + i] = G.t[i];
     so3_log(G.R, o + 12);
-    o[15] = (double)st.best_count;
+    o[15] = st.valid ? (double)st.best_count : 0.0;   // the inlier count of the mask returned (empty on failure)
     o[16] = (st.valid && st.good_acc[28] > 0) ? sqrt(st.good_cost / st.good_acc[28]) : 0.0;
     o[17] = st.valid ? 1.0 : 0.0;
   }

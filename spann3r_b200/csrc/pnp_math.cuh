@@ -254,27 +254,33 @@ S3R_HD void so3_exp(const double* w, double* R) {
   R[6] = -A * wy + B * wx * wz;       R[7] = A * wx + B * wy * wz;       R[8] = 1 - B * (wx * wx + wy * wy);
 }
 
-// Rodrigues vector of a rotation matrix (the `rvec` cv2 returns).
+// Rodrigues vector of a rotation matrix (the `rvec` cv2 returns), through the unit quaternion: Shepperd's method takes
+// the largest of |qw|, |qx|, |qy|, |qz| from the diagonal and the rest from the off-diagonal sums / differences, and
+// th = 2 atan2(|q_xyz|, qw).  Accurate to rounding at every angle; acos of the trace with the skew part divided by
+// sin(th) loses digits as th approaches pi (1e-11 at pi - 0.006).
 S3R_HD void so3_log(const double* R, double* w) {
   const double tr = R[0] + R[4] + R[8];
-  double c = 0.5 * (tr - 1);
-  c = c > 1 ? 1 : (c < -1 ? -1 : c);
-  const double th = acos(c);
-  const double ax = R[7] - R[5], ay = R[2] - R[6], az = R[3] - R[1];   // 2 sin(th) * axis
-  if (th < 1e-8) {
-    w[0] = 0.5 * ax; w[1] = 0.5 * ay; w[2] = 0.5 * az;
-    return;
+  double q[4];   // (qw, qx, qy, qz) times 4 * (the largest component)
+  if (tr >= R[0] && tr >= R[4] && tr >= R[8]) {
+    const double s = 1 + tr;
+    q[0] = s; q[1] = R[7] - R[5]; q[2] = R[2] - R[6]; q[3] = R[3] - R[1];
+  } else if (R[0] >= R[4] && R[0] >= R[8]) {
+    const double s = 1 + R[0] - R[4] - R[8];
+    q[0] = R[7] - R[5]; q[1] = s; q[2] = R[1] + R[3]; q[3] = R[2] + R[6];
+  } else if (R[4] >= R[8]) {
+    const double s = 1 + R[4] - R[0] - R[8];
+    q[0] = R[2] - R[6]; q[1] = R[1] + R[3]; q[2] = s; q[3] = R[5] + R[7];
+  } else {
+    const double s = 1 + R[8] - R[0] - R[4];
+    q[0] = R[3] - R[1]; q[1] = R[2] + R[6]; q[2] = R[5] + R[7]; q[3] = s;
   }
-  if (3.141592653589793 - th < 1e-6) {   // near pi: axis from the symmetric part
-    double v[3] = {sqrt(fmax(0.0, 0.5 * (R[0] + 1))), sqrt(fmax(0.0, 0.5 * (R[4] + 1))), sqrt(fmax(0.0, 0.5 * (R[8] + 1)))};
-    if (R[1] + R[3] < 0) v[1] = -v[1];
-    if (R[2] + R[6] < 0) v[2] = -v[2];
-    normalize3(v);
-    w[0] = th * v[0]; w[1] = th * v[1]; w[2] = th * v[2];
-    return;
+  if (q[0] < 0) {   // the quaternion with qw >= 0: th in [0, pi]
+    for (int i = 0; i < 4; ++i) q[i] = -q[i];
   }
-  const double s = th / (2 * sin(th));
-  w[0] = s * ax; w[1] = s * ay; w[2] = s * az;
+  const double n = sqrt(q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
+  // th / |q_xyz| with the common scale divided out; 2 / qw is its limit (to 1e-16 relative) at th < ~1e-8
+  const double k = n > 1e-8 * q[0] ? 2 * atan2(n, q[0]) / n : 2 / q[0];
+  w[0] = k * q[1]; w[1] = k * q[2]; w[2] = k * q[3];
 }
 
 // One damped Gauss-Newton step from the accumulated sums: solve (H + lambda diag(H)) delta = -g by Cholesky, apply

@@ -26,14 +26,13 @@ def estimate_focal_knowing_depth(pts3d: torch.Tensor, pp, focal_mode: str = "med
     ppx, ppy = (float(v) for v in (pp.flatten().tolist() if torch.is_tensor(pp) else pp))
     base = max(H, W) / (2 * math.tan(math.radians(60) / 2))
     lo = min_focal * base
-    hi = max_focal * base if math.isfinite(max_focal) else 3.0e38
+    hi = max_focal * base           # max_focal = inf -> no upper clip; a NaN focal stays NaN in both modes
     focal = torch.empty(B, dtype=torch.float32, device=pts3d.device)
     if focal_mode == "median":      # nanmedian of the per-pixel votes: an exact selection, bit-identical to the reference
         scratch = torch.empty(B * 260, dtype=torch.int32, device=pts3d.device)
         with _lib.on_device(pts3d):
-            _lib.check(_lib.lib().s3r_focal_median(_lib.ptr(pts3d), B, H, W, ppx, ppy, lo,
-                                                   max_focal * base if math.isfinite(max_focal) else float("inf"),
-                                                   _lib.ptr(scratch), _lib.ptr(focal), _lib.stream_ptr(pts3d.device)),
+            _lib.check(_lib.lib().s3r_focal_median(_lib.ptr(pts3d), B, H, W, ppx, ppy, lo, hi, _lib.ptr(scratch),
+                                                   _lib.ptr(focal), _lib.stream_ptr(pts3d.device)),
                        "s3r_focal_median")
         return focal
     scratch = torch.empty(B * 148 * 2, dtype=torch.float32, device=pts3d.device)

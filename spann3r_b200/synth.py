@@ -287,6 +287,218 @@ PNP_CASES = [
 ]
 
 
+# ---- adversarial inputs of the post-path geometry: tests/test_postprocess_adversarial.py ---------------------------
+def _pinhole_map(g, B, H, W, f, noise=0.0):
+    """[B, H, W, 3] fp32 pinhole pointmap with focal f and principal point (W / 2, H / 2), depth in [1, 3]."""
+    jj, ii = torch.meshgrid(torch.arange(H, dtype=torch.float64), torch.arange(W, dtype=torch.float64), indexing="ij")
+    z = 1.0 + 2.0 * torch.rand(B, H, W, generator=g, dtype=torch.float64)
+    x = (ii - W / 2) * z / f
+    y = (jj - H / 2) * z / f
+    if noise:
+        x = x + noise * torch.randn(B, H, W, generator=g, dtype=torch.float64)
+        y = y + noise * torch.randn(B, H, W, generator=g, dtype=torch.float64)
+    return torch.stack((x, y, z), -1).float()
+
+
+def _focal_frame(name: str, g) -> torch.Tensor:
+    nan, inf = float("nan"), float("inf")
+    if name == "all_z0":                  # every x / z is +-inf or NaN -> a = 0 everywhere, f0 = 0 / 0
+        p = _pinhole_map(g, 1, 48, 64, 60.0, 0.01)
+        p[..., 2] = 0.0
+        return p
+    if name == "all_nan":
+        return torch.full((1, 48, 64, 3), nan)
+    if name == "one_finite":
+        p = torch.full((1, 48, 64, 3), nan)
+        p[0, 7, 50] = _pinhole_map(g, 1, 48, 64, 60.0, 0.01)[0, 7, 50]
+        return p
+    if name == "noise_free":              # |p - f a| is fp32 rounding only; 0 at the principal point (weight floor)
+        return _pinhole_map(g, 1, 96, 128, 110.0)
+    if name == "behind_half":             # half the pixels have z < 0 (x, y kept): their a points the wrong way
+        p = _pinhole_map(g, 1, 64, 80, 55.0, 0.01)
+        back = torch.rand(1, 64, 80, generator=g) < 0.5
+        p[..., 2] = torch.where(back, -p[..., 2], p[..., 2])
+        return p
+    if name == "inf_lattice":             # x = +-inf on one lattice of pixels, z = 0 on another
+        p = _pinhole_map(g, 1, 60, 84, 70.0, 0.01)
+        jj, ii = torch.meshgrid(torch.arange(60), torch.arange(84), indexing="ij")
+        lat = (jj % 5 == 0) & (ii % 7 == 0)
+        p[..., 0] = torch.where(lat, torch.where((ii + jj) % 2 == 0, inf, -inf).float(), p[..., 0])
+        p[..., 2] = torch.where((jj % 3 == 1) & (ii % 11 == 3), 0.0, p[..., 2])
+        return p
+    if name == "h1":
+        return _pinhole_map(g, 2, 1, 300, 90.0, 0.01)
+    if name == "w1":
+        return _pinhole_map(g, 2, 300, 1, 90.0, 0.01)
+    if name == "tiny":                    # 120 pixels: fewer than one 256-thread block
+        return _pinhole_map(g, 1, 10, 12, 9.0, 0.001)
+    if name == "hd":                      # 1080 x 1920: many terms per thread
+        return _pinhole_map(g, 1, 1080, 1920, 1400.0, 0.01)
+    if name == "scaled":
+        return _pinhole_map(g, 1, 64, 80, 55.0, 0.01) * 1e-20
+    if name == "underflow":               # a ~ 1e-22: a.a underflows fp32 (subnormal or 0), a.p does not
+        p = _pinhole_map(g, 1, 64, 80, 55.0, 0.01)
+        p[..., :2] = p[..., :2] * 1e-22
+        return p
+    if name == "mixed":                   # valid / all-NaN / all-z=0 / valid
+        p = _pinhole_map(g, 4, 48, 64, 60.0, 0.01)
+        p[1] = nan
+        p[2, ..., 2] = 0.0
+        return p
+    # median-specific frames: votes u z / x and v z / y
+    if name == "med_even":                # a few NaN pixels: an even number of non-NaN votes
+        p = _pinhole_map(g, 1, 31, 37, 40.0, 0.01)
+        p[0, 3:6, 4] = nan
+        return p
+    if name == "med_odd":                 # one NaN x: an odd number of non-NaN votes
+        p = _pinhole_map(g, 1, 31, 37, 40.0, 0.01)
+        p[0, 9, 13, 0] = nan
+        return p
+    if name in ("med_identical", "med_ties"):
+        H, W = 24, 32
+        jj, ii = torch.meshgrid(torch.arange(H), torch.arange(W), indexing="ij")
+        u, v = (ii - W / 2).float(), (jj - H / 2).float()
+        if name == "med_identical":       # x = u / 64, z = 1: every non-NaN vote is exactly 64
+            qx = qy = torch.full((H, W), 64.0)
+        else:                             # votes drawn from {16, 32, 64, 128}: long runs of ties around the median
+            q = torch.tensor([16.0, 32.0, 64.0, 128.0])
+            qx = q[torch.randint(0, 4, (H, W), generator=g)]
+            qy = q[torch.randint(0, 4, (H, W), generator=g)]
+        return torch.stack((u / qx, v / qy, torch.ones(H, W)), -1)[None]
+    if name == "med_inf_mixed":           # x = 0 or y = 0 with u z != 0: +-inf votes among finite ones
+        p = _pinhole_map(g, 1, 40, 50, 45.0, 0.01)
+        sel = torch.rand(1, 40, 50, generator=g)
+        p[..., 0] = torch.where(sel < 0.15, 0.0, p[..., 0])
+        p[..., 1] = torch.where(sel > 0.9, -0.0, p[..., 1])
+        return p
+    if name == "med_plus_inf":            # every x and y is a zero signed like u and v: every non-NaN vote is +inf
+        p = _pinhole_map(g, 1, 40, 50, 45.0)
+        p[..., 0] = p[..., 0] * 0.0
+        p[..., 1] = p[..., 1] * 0.0
+        return p
+    if name == "med_negative":            # z < 0 everywhere: every vote is about -f
+        p = _pinhole_map(g, 1, 40, 50, 45.0, 0.01)
+        p[..., 2] = -p[..., 2]
+        return p
+    if name == "med_one_vote":            # one pixel with a finite x and a NaN y, everything else NaN
+        p = torch.full((1, 40, 50, 3), nan)
+        p[0, 30, 41] = _pinhole_map(g, 1, 40, 50, 45.0, 0.01)[0, 30, 41]
+        p[0, 30, 41, 1] = nan
+        return p
+    raise ValueError(name)
+
+
+# name -> seed of the adversarial focal frames; every frame is run in both focal modes.  `underflow`: a.a underflows fp32,
+# so the reference's fp32 result is NaN while fp64 is finite (a kernel that keeps a subnormal sum may be either).
+FOCAL_ADV_CASES = {name: i + 1 for i, name in enumerate((
+    "all_z0", "all_nan", "one_finite", "noise_free", "behind_half", "inf_lattice", "h1", "w1", "tiny", "hd", "scaled",
+    "underflow", "mixed", "med_even", "med_odd", "med_identical", "med_ties", "med_inf_mixed", "med_plus_inf",
+    "med_negative", "med_one_vote"))}
+
+
+def make_focal_adv_case(name: str) -> torch.Tensor:
+    """Adversarial pointmap `name` of FOCAL_ADV_CASES: [B, H, W, 3] fp32 (CPU); principal point (W / 2, H / 2)."""
+    return _focal_frame(name, torch.Generator().manual_seed(FOCAL_ADV_CASES[name])).contiguous()
+
+
+def _world_from_cam(xc, rvec, tvec):
+    return (xc - np.asarray(tvec, np.float64)) @ _rotation(rvec)
+
+
+def _sparse_exact(rng, n, n_nan, rvec, tvec, K, behind=False):
+    """n exact correspondences of random non-coplanar camera-frame points (plus n_nan NaN image points)."""
+    u = rng.uniform(20, 2 * K[0, 2] - 20, n)
+    v = rng.uniform(20, 2 * K[1, 2] - 20, n)
+    d = rng.uniform(1.5, 4.0, n) * (-1.0 if behind else 1.0)
+    xc = np.stack(((u - K[0, 2]) / K[0, 0] * d, (v - K[1, 2]) / K[1, 1] * d, d), -1)
+    pts = _world_from_cam(xc, rvec, tvec)
+    img = np.stack((u, v), -1)
+    if n_nan:
+        pts = np.concatenate((pts, rng.normal(0, 1, (n_nan, 3))))
+        img = np.concatenate((img, np.full((n_nan, 2), np.nan)))
+    return pts.astype(np.float32), img.astype(np.float32)
+
+
+def make_pnp_adv_case(name: str):
+    """Adversarial PnP frame `name` of PNP_ADV_CASES -> (pts3d, image_points or None, K).  Dense frames: pts3d
+    [H, W, 3] with the pixel grid as image points; sparse frames: pts3d [n, 3], image_points [n, 2].  float32."""
+    rng = np.random.default_rng(PNP_ADV_CASES.index(name) + 100)
+    if name == "nan_inf":                 # 30 % NaN coordinates, 5 % +-inf coordinates
+        pts, K = make_pointmap_case(384, 512, 400.0, (0.1, -0.2, 0.05), (0.3, -0.1, 0.2), 0.002, 0.05, 11)
+        flat = pts.reshape(-1, 3)
+        n = len(flat)
+        bad = rng.choice(n, int(0.35 * n), replace=False)
+        flat[bad[: int(0.30 * n)], rng.integers(0, 3, int(0.30 * n))] = np.nan
+        k = len(bad) - int(0.30 * n)
+        flat[bad[int(0.30 * n):], rng.integers(0, 3, k)] = np.where(rng.random(k) < 0.5, np.inf, -np.inf)
+        return pts, None, K
+    if name == "behind40":                # 40 % of the points moved behind the camera
+        H, W, f, rv, tv = 384, 512, 420.0, (-0.2, 0.4, 0.3), (0.1, 0.6, -0.3)
+        pts, K = make_pointmap_case(H, W, f, rv, tv, 0.002, 0.0, 12)
+        flat = pts.reshape(-1, 3).astype(np.float64)
+        sel = rng.choice(H * W, int(0.4 * H * W), replace=False)
+        xc = flat[sel] @ _rotation(rv).T + np.asarray(tv)
+        xc *= -rng.uniform(0.3, 2.0, (len(sel), 1))
+        flat[sel] = _world_from_cam(xc, rv, tv)
+        return flat.astype(np.float32).reshape(H, W, 3), None, K
+    if name == "planar":                  # a tilted plane
+        H, W, f, rv, tv = 384, 512, 380.0, (0.2, -0.1, 0.3), (-0.2, 0.1, 0.5)
+        K = np.array([[f, 0, W / 2], [0, f, H / 2], [0, 0, 1]])
+        u, v = np.meshgrid(np.arange(W), np.arange(H))
+        ray = np.stack(((u - W / 2) / f, (v - H / 2) / f, np.ones_like(u, np.float64)), -1)
+        d = 2.5 / (1.0 + 0.3 * ray[..., 0] - 0.2 * ray[..., 1])        # plane 0.3 x - 0.2 y + z = 2.5
+        xc = (ray * d[..., None]).reshape(-1, 3) + rng.normal(0, 0.002, (H * W, 3))
+        return _world_from_cam(xc, rv, tv).astype(np.float32).reshape(H, W, 3), None, K
+    if name == "collinear":               # a 4 x 512 strip: the points lie close to one line
+        pts, K = make_pointmap_case(4, 512, 400.0, (0.05, 0.1, -0.05), (0.1, 0.0, 0.3), 0.001, 0.0, 13)
+        return pts, None, K
+    if name in ("sparse4", "sparse5", "sparse8"):
+        K = np.array([[500.0, 0, 320], [0, 500.0, 240], [0, 0, 1]])
+        pts, img = _sparse_exact(rng, int(name[6:]), 3, (0.1, 0.3, -0.2), (0.2, -0.1, 0.4), K)
+        return pts, img, K
+    if name == "three_finite":            # 3 finite correspondences among 12: no model can have 4 inliers
+        K = np.array([[500.0, 0, 320], [0, 500.0, 240], [0, 0, 1]])
+        pts, img = _sparse_exact(rng, 3, 0, (0.1, 0.3, -0.2), (0.2, -0.1, 0.4), K)
+        pts = np.concatenate((pts, np.full((9, 3), np.nan, np.float32)))
+        img = np.concatenate((img, rng.uniform(0, 400, (9, 2)).astype(np.float32)))
+        return pts, img, K
+    if name == "all_behind":              # 6 correspondences, every point behind the camera
+        # A mirror pose (a half turn about the optical axis, then a shift along it) puts behind-camera points of about
+        # one depth in front of the camera on their own pixels, so larger such frames do have 4-inlier models.  These 6
+        # points have none: 4096 samples (many draws of each of their 20 triples) find no model with 4 inliers.
+        K = np.array([[500.0, 0, 320], [0, 500.0, 240], [0, 0, 1]])
+        pts, img = _sparse_exact(np.random.default_rng(0), 6, 0, (0.1, 0.3, -0.2), (0.2, -0.1, 0.4), K, behind=True)
+        return pts, img, K
+    if name == "near_centre":             # identity pose, one exact inlier 2e-3 in front of the camera centre
+        pts, K = make_pointmap_case(384, 512, 400.0, (0.0, 0.0, 0.0), (0.0, 0.0, 0.0), 2e-4, 0.0, 14)
+        z = 2e-3
+        for r, c in ((100, 300), (250, 120)):
+            pts[r, c] = ((c - 256) / 400.0 * z, (r - 192) / 400.0 * z, z)
+        return pts, None, K
+    if name == "hd":
+        pts, K = make_pointmap_case(1080, 1920, 1500.0, (0.1, -0.15, 0.05), (0.2, 0.1, 0.3), 0.002, 0.2, 15)
+        return pts, None, K
+    if name == "all_nan":
+        pts, K = make_pointmap_case(96, 128, 120.0, (0.0, 0.0, 0.0), (0.0, 0.0, 0.0), 0.0, 0.0, 16)
+        return np.full_like(pts, np.nan), None, K
+    if name == "three_finite_dense":
+        pts, K = make_pointmap_case(96, 128, 120.0, (0.1, 0.0, 0.0), (0.0, 0.1, 0.0), 0.001, 0.0, 17)
+        keep = pts[[5, 50, 90], [7, 60, 100]].copy()
+        pts[:] = np.nan
+        pts[[5, 50, 90], [7, 60, 100]] = keep
+        return pts, None, K
+    if name == "valid_small":
+        pts, K = make_pointmap_case(96, 128, 120.0, (0.1, -0.05, 0.02), (0.05, 0.1, 0.2), 0.002, 0.2, 18)
+        return pts, None, K
+    raise ValueError(name)
+
+
+# The adversarial PnP frames; `hd` is GPU-only (the host scoring loop would take minutes).  The last three share one
+# camera (96 x 128, f = 120) so they can form a mixed batch of solvable and unsolvable frames.
+PNP_ADV_CASES = ["nan_inf", "behind40", "planar", "collinear", "sparse4", "sparse5", "sparse8", "three_finite",
+                 "all_behind", "near_centre", "hd", "all_nan", "three_finite_dense", "valid_small"]
+
+
 def make_loss_case(batch: int, frames: int, height: int, width: int, invalid: float = 0.3, seed: int = 0,
                    device="cpu"):
     """Views and `preds_all` for the criteria (spann3r_b200.loss / tests/golden/loss_*.npz): a wavy surface per frame
