@@ -66,6 +66,59 @@ class AttnTrainDesc(C.Structure):
         ("q_stride", _i64 * 3), ("k_stride", _i64 * 3), ("v_stride", _i64 * 3),
     ]
 
+
+# ------------------------------------------------------------------------------------------------
+# model-level structs of include/spann3r_b200.h (s3r_model_w, s3r_bank): the engine's weights and memory bank
+# ------------------------------------------------------------------------------------------------
+class Planes(C.Structure):
+    _fields_ = [("hi", _vp), ("lo", _vp)]
+
+
+class LN(C.Structure):
+    _fields_ = [("w", _vp), ("b", _vp)]
+
+
+class Lin(C.Structure):
+    _fields_ = [("w", Planes), ("b", _vp), ("cs", _vp), ("cs_hi", _vp)]
+
+
+class BlockW(C.Structure):
+    _fields_ = [("norm1", LN), ("qkv", Lin), ("proj", Lin), ("norm2", LN), ("fc1", Lin), ("fc2", Lin)]
+
+
+class DecBlockW(C.Structure):
+    _fields_ = [("norm1", LN), ("qkv", Lin), ("proj", Lin), ("norm_y", LN), ("norm2", LN), ("q", Lin),
+                ("cproj", Lin), ("norm3", LN), ("fc1", Lin), ("fc2", Lin)]
+
+
+class RcuW(C.Structure):
+    _fields_ = [("conv1", Lin), ("conv2", Lin)]
+
+
+class FusionW(C.Structure):
+    _fields_ = [("rcu1", RcuW), ("rcu2", RcuW), ("out_conv", Lin)]
+
+
+class DptW(C.Structure):
+    _fields_ = [("act1_conv", Lin), ("act1_up", Lin), ("act2_conv", Lin), ("act2_up", Lin), ("act3_conv", Lin),
+                ("act4_conv", Lin), ("act4_down", Lin), ("layer_rn", Lin * 4), ("refine", FusionW * 4),
+                ("head0", Lin), ("head2", Lin), ("head4_w", _vp), ("head4_b", _vp)]
+
+
+class ModelW(C.Structure):
+    _fields_ = [("patch_embed", Lin), ("enc", BlockW * 24), ("enc_norm", LN),
+                ("decoder_embed", Lin), ("dec", DecBlockW * 12), ("dec_norm", LN),
+                ("key_fc1", Lin), ("key_fc2", Lin), ("dpt", DptW),
+                ("pos_patch_embed", Lin), ("val", BlockW * 6), ("value_norm", LN), ("value_out", Lin),
+                ("norm_q", LN), ("norm_k", LN), ("norm_v", LN),
+                ("rope_cs", _vp), ("rope_maxpos", _i), ("value_dim", _i), ("rope_cs_v", _vp)]
+
+
+class Bank(C.Structure):
+    _fields_ = [("kn_hi", _vp), ("kn_lo", _vp), ("vnt_hi", _vp), ("vnt_lo", _vp), ("k_raw", _vp), ("v_raw", _vp),
+                ("attn", _vp), ("count", _vp), ("cap", _i), ("len", _i)]
+
+
 _PROTOS = {
     "s3r_version": (_i, []),
     "s3r_abi_sizeof": (_i, [_i]),
@@ -134,6 +187,26 @@ _PROTOS = {
     "s3r_views_resample_v_norm": (_i, [_vp, _i, _i, _i, _vp]),
     "s3r_views_resample_v_u8": (_i, [_vp, _vp, _i, _i, _i, _vp]),
     "s3r_views_color_jitter": (_i, [_vp, _i, _i64, _vp]),
+    "s3r_engine_create": (_vp, [C.POINTER(ModelW), _i, _i, _i, _i]),
+    "s3r_engine_create_ex": (_vp, [C.POINTER(ModelW), _i, _i, _i, _i, _i]),
+    "s3r_engine_destroy": (None, [_vp]),
+    "s3r_engine_encode": (_i, [_vp, _vp, _i, _vp, _vp]),
+    "s3r_engine_decode": (_i, [_vp, _vp, _vp, _vp, _vp]),
+    "s3r_engine_keyheads": (_i, [_vp, _vp, _vp, _vp, _vp, _vp]),
+    "s3r_engine_heads": (_i, [_vp, _vp, _vp, _vp]),
+    "s3r_engine_value": (_i, [_vp, _vp, _vp, _i, _vp, _vp]),
+    "s3r_engine_memory_read": (_i, [_vp, C.POINTER(Bank), _vp, _f, _vp, _vp]),
+    "s3r_engine_memory_read_train": (_i, [_vp, C.POINTER(Bank), _vp, _f, _f, C.c_uint64, _vp, _vp]),
+    "s3r_engine_memory_append": (_i, [_vp, C.POINTER(Bank), _vp, _vp, _vp]),
+    "s3r_engine_check_sim": (_i, [_vp, C.POINTER(Bank), _vp, _i, _vp, _vp]),
+    "s3r_engine_memory_read_slots": (_i, [_vp, C.POINTER(Bank), C.POINTER(_i), _vp, _f, _vp, _vp]),
+    "s3r_engine_memory_append_slots": (_i, [_vp, C.POINTER(Bank), C.POINTER(_i), C.POINTER(_i), _vp, _vp, _vp]),
+    "s3r_engine_check_sim_slots": (_i, [_vp, C.POINTER(Bank), C.POINTER(_i), C.POINTER(_i), _vp, _vp, _vp]),
+    "s3r_engine_take_flops": (C.c_double, [_vp]),
+    "s3r_engine_take_launches": (C.c_longlong, [_vp]),
+    "s3r_engine_profile": (None, [_vp, _i]),
+    "s3r_engine_profile_read": (_i, [_vp, C.POINTER(C.c_double)]),
+    "s3r_engine_profile_list": (_i, [_vp, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(_i), _i]),
 }
 
 
@@ -184,29 +257,12 @@ def lib():
             fn = getattr(L, name)
             fn.restype = res
             fn.argtypes = args
-        _ENGINE_PROTOS_HOOK(L)
         _lib = L
     return _lib
 
 
-def _ENGINE_PROTOS_HOOK(L):  # replaced by engine.py when it defines more entry points
-    for name, (res, args) in _EXTRA_PROTOS.items():
-        fn = getattr(L, name)
-        fn.restype = res
-        fn.argtypes = args
-
-
-_EXTRA_PROTOS: dict = {}
-
-
-def register_protos(protos: dict):
-    _EXTRA_PROTOS.update(protos)
-    if _lib is not None:
-        _ENGINE_PROTOS_HOOK(_lib)
-
-
 def declared_symbols():
-    return list(_PROTOS) + list(_EXTRA_PROTOS)
+    return list(_PROTOS)
 
 
 def check(status: int, what: str = ""):
@@ -237,6 +293,14 @@ def on_device(t_or_dev):
     return torch.cuda.device(dev)
 
 
+def call(name, device, *args):
+    """Call library function `name` with `args` and the current stream of `device` appended, with `device` current
+    (a tensor, a torch.device, or None for the current device); raise S3RError naming `name` on a nonzero status."""
+    dev = device.device if isinstance(device, torch.Tensor) else device
+    with torch.cuda.device(dev):
+        check(getattr(lib(), name)(*args, stream_ptr(dev)), name)
+
+
 # ------------------------------------------------------------------------------------------------
 # tensor-level helpers (op level; the model-level fast path lives in engine.py)
 # ------------------------------------------------------------------------------------------------
@@ -251,8 +315,7 @@ def split(x: torch.Tensor, relu: bool = False, out=None):
     else:
         hi = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
         lo = torch.empty_like(hi)
-    with on_device(x):
-        check(lib().s3r_split(ptr(x), c, ptr(hi), ptr(lo), c, 0, rows, c, int(relu), stream_ptr(x.device)), "s3r_split")
+    call("s3r_split", x, ptr(x), c, ptr(hi), ptr(lo), c, 0, rows, c, int(relu))
     return hi, lo
 
 
@@ -263,18 +326,13 @@ def layernorm(x, w, b, eps, want_f32=True, want_planes=False):
     out = torch.empty_like(x) if want_f32 else None
     hi = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device) if want_planes else None
     lo = torch.empty_like(hi) if want_planes else None
-    with on_device(x):
-        check(lib().s3r_layernorm(ptr(x), c, ptr(w), ptr(b), 0, 0, float(eps), rows, c, ptr(out), c, ptr(hi), ptr(lo), c, 0,
-                                  0, stream_ptr(x.device)), "s3r_layernorm")
+    call("s3r_layernorm", x, ptr(x), c, ptr(w), ptr(b), 0, 0, float(eps), rows, c, ptr(out), c, ptr(hi), ptr(lo), c, 0, 0)
     return out, hi, lo
 
 
 def gemm(desc: GemmDesc, device=None):
     """device: the device the descriptor's pointers live on (default: the current device)."""
-    if device is None:
-        return check(lib().s3r_gemm(C.byref(desc), stream_ptr()), "s3r_gemm")
-    with on_device(device):
-        check(lib().s3r_gemm(C.byref(desc), stream_ptr(device)), "s3r_gemm")
+    call("s3r_gemm", device, C.byref(desc))
 
 
 def linear(x_planes, w_planes, bias=None, act=ACT_NONE, res=None, want_f32=True, want_planes=False, plane_relu=False,
@@ -312,16 +370,13 @@ def conv_wgrad(dy_planes, x_planes, taps: int) -> torch.Tensor:
     nb, h, w, n = yh.shape
     kc = xh.shape[-1]
     assert tuple(xh.shape[:3]) == (nb, h, w) and yh.is_contiguous() and xh.is_contiguous(), (tuple(yh.shape), tuple(xh.shape))
-    L = lib()
-    ws_bytes = L.s3r_conv_wgrad_workspace_bytes(nb, h, w, n, kc, taps)
+    ws_bytes = lib().s3r_conv_wgrad_workspace_bytes(nb, h, w, n, kc, taps)
     if ws_bytes == 0:
         raise S3RError(f"s3r_conv_wgrad: unsupported shape nb={nb} h={h} w={w} n={n} kc={kc} taps={taps}")
     dev = yh.device
     ws = torch.empty(ws_bytes // 4, dtype=torch.float32, device=dev)
     dw = torch.empty((n, taps, kc), dtype=torch.float32, device=dev)
-    with on_device(dev):
-        check(L.s3r_conv_wgrad(ptr(yh), ptr(yl), n, ptr(xh), ptr(xl), kc, nb, h, w, n, kc, taps, ptr(ws), ws_bytes, ptr(dw),
-                               stream_ptr(dev)), "s3r_conv_wgrad")
+    call("s3r_conv_wgrad", dev, ptr(yh), ptr(yl), n, ptr(xh), ptr(xl), kc, nb, h, w, n, kc, taps, ptr(ws), ws_bytes, ptr(dw))
     return dw
 
 
@@ -329,9 +384,7 @@ def col2im_3x3s2(cols: torch.Tensor, nb: int, h: int, w: int, c: int) -> torch.T
     """Adjoint of s3r_im2col_3x3s2: fp32 cols [nb*ho*wo, 9*c] -> fp32 [nb, h, w, c]."""
     assert cols.dtype == torch.float32 and cols.is_cuda and cols.is_contiguous()
     out = torch.empty((nb, h, w, c), dtype=torch.float32, device=cols.device)
-    with on_device(cols):
-        check(lib().s3r_col2im_3x3s2(ptr(cols), nb, h, w, c, (h + 1) // 2, (w + 1) // 2, ptr(out), stream_ptr(cols.device)),
-              "s3r_col2im_3x3s2")
+    call("s3r_col2im_3x3s2", cols, ptr(cols), nb, h, w, c, (h + 1) // 2, (w + 1) // 2, ptr(out))
     return out
 
 
@@ -340,8 +393,7 @@ def conf_score(conf: torch.Tensor) -> torch.Tensor:
     assert conf.is_cuda and conf.dtype == torch.float32 and conf.is_contiguous()
     scratch = torch.empty(256, dtype=torch.float32, device=conf.device)
     out = torch.empty(1, dtype=torch.float32, device=conf.device)
-    with on_device(conf):
-        check(lib().s3r_conf_score(ptr(conf), conf.numel(), ptr(scratch), ptr(out), stream_ptr(conf.device)), "s3r_conf_score")
+    call("s3r_conf_score", conf, ptr(conf), conf.numel(), ptr(scratch), ptr(out))
     return out
 
 
@@ -351,9 +403,7 @@ def conf_score_batched(conf: torch.Tensor) -> torch.Tensor:
     B, hw = conf.shape[1], conf.shape[2] * conf.shape[3]
     scratch = torch.empty(2 * B * 256, dtype=torch.float32, device=conf.device)
     out = torch.empty(2, B, dtype=torch.float32, device=conf.device)
-    with on_device(conf):
-        check(lib().s3r_conf_score_batched(ptr(conf), B, hw, ptr(scratch), ptr(out), stream_ptr(conf.device)),
-              "s3r_conf_score_batched")
+    call("s3r_conf_score_batched", conf, ptr(conf), B, hw, ptr(scratch), ptr(out))
     return out
 
 
@@ -361,7 +411,5 @@ def dropout_mask(shape, seed: int, p: float, device) -> torch.Tensor:
     """Keep-scale (0 or 1 / (1 - p)) of every element of a [..., len] attention tensor under the Philox mask the
     training-mode memory read applies for `seed` (s3r_engine_memory_read_train); flat index = row-major position."""
     out = torch.empty(shape, dtype=torch.float32, device=device)
-    with on_device(out):
-        check(lib().s3r_dropout_mask(ptr(out), out.numel(), int(seed) & 0xFFFFFFFFFFFFFFFF, float(p), stream_ptr(out.device)),
-              "s3r_dropout_mask")
+    call("s3r_dropout_mask", out, ptr(out), out.numel(), int(seed) & 0xFFFFFFFFFFFFFFFF, float(p))
     return out

@@ -56,9 +56,7 @@ def _forward(q, k, v, scale: float):
     d = _desc(q, k, v, scale)
     o = torch.empty((B, nq, H * dh), dtype=torch.float32, device=q.device)
     lse = torch.empty((B * H, nq), dtype=torch.float32, device=q.device)
-    with _lib.on_device(q):
-        _lib.check(_lib.lib().s3r_attn_train_forward(C.byref(d), _lib.ptr(o), _lib.ptr(lse), _lib.stream_ptr(q.device)),
-                   "s3r_attn_train_forward")
+    _lib.call("s3r_attn_train_forward", q, C.byref(d), _lib.ptr(o), _lib.ptr(lse))
     return q, k, v, o, lse
 
 
@@ -75,16 +73,13 @@ class _Attention(torch.autograd.Function):
         q, k, v, o, lse = ctx.saved_tensors
         go = go.float().contiguous()
         d = _desc(q, k, v, ctx.scale)
-        L = _lib.lib()
-        ws_bytes = L.s3r_attn_train_workspace_bytes(C.byref(d))
+        ws_bytes = _lib.lib().s3r_attn_train_workspace_bytes(C.byref(d))
         ws = torch.empty(ws_bytes // 4, dtype=torch.float32, device=q.device)
         dq = torch.empty(q.shape, dtype=torch.float32, device=q.device)
         dk = torch.empty(k.shape, dtype=torch.float32, device=q.device)
         dv = torch.empty(v.shape, dtype=torch.float32, device=q.device)
-        with _lib.on_device(q):
-            _lib.check(L.s3r_attn_train_backward(C.byref(d), _lib.ptr(o), _lib.ptr(lse), _lib.ptr(go), _lib.ptr(ws), ws_bytes,
-                                                 _lib.ptr(dq), _lib.ptr(dk), _lib.ptr(dv), _lib.stream_ptr(q.device)),
-                       "s3r_attn_train_backward")
+        _lib.call("s3r_attn_train_backward", q, C.byref(d), _lib.ptr(o), _lib.ptr(lse), _lib.ptr(go), _lib.ptr(ws),
+                  ws_bytes, _lib.ptr(dq), _lib.ptr(dk), _lib.ptr(dv))
         return dq, dk, dv, None
 
 

@@ -123,9 +123,7 @@ class _Conv3x3s2(torch.autograd.Function):
         xh, xl = _planes(_nhwc(x))
         ch = torch.empty((nb, ho, wo, 9 * c), dtype=torch.bfloat16, device=x.device)
         cl = torch.empty_like(ch)
-        with _lib.on_device(x):
-            _lib.check(_lib.lib().s3r_im2col_3x3s2(_lib.ptr(xh), _lib.ptr(xl), nb, h, wd, c, ho, wo, _lib.ptr(ch), _lib.ptr(cl),
-                                                   _lib.stream_ptr(x.device)), "s3r_im2col_3x3s2")
+        _lib.call("s3r_im2col_3x3s2", x, _lib.ptr(xh), _lib.ptr(xl), nb, h, wd, c, ho, wo, _lib.ptr(ch), _lib.ptr(cl))
         ctx.cols, ctx.in_shape, ctx.has_bias = (ch, cl), (nb, h, wd, c), b is not None
         ctx.save_for_backward(w)
         return _nchw(_gemm((ch, cl), nb, ho, wo, _planes(w.permute(0, 2, 3, 1).reshape(w.shape[0], 9 * c)), w.shape[0], 1, b))
@@ -157,9 +155,7 @@ class _PatchConv(torch.autograd.Function):
         ch = torch.empty((nb, gh, gw_, 768), dtype=torch.bfloat16, device=x.device)
         cl = torch.empty_like(ch)
         sb, sc, sy, sx = xf.stride()
-        with _lib.on_device(x):
-            _lib.check(_lib.lib().s3r_im2col_patch16(_lib.ptr(xf), sb, sc, sy, sx, nb, gh, gw_, _lib.ptr(ch), _lib.ptr(cl),
-                                                     _lib.stream_ptr(x.device)), "s3r_im2col_patch16")
+        _lib.call("s3r_im2col_patch16", x, _lib.ptr(xf), sb, sc, sy, sx, nb, gh, gw_, _lib.ptr(ch), _lib.ptr(cl))
         ctx.cols, ctx.in_shape, ctx.has_bias = (ch, cl), x.shape, b is not None
         ctx.save_for_backward(w)
         return _nchw(_gemm((ch, cl), nb, gh, gw_, _planes(w.reshape(w.shape[0], 768)), w.shape[0], 1, b))

@@ -19,6 +19,7 @@
 // (bits + 0x1000) & ~0x1fff; l = l * al + sum P (per-thread partials, quad-reduced at the end); O = O * al + P V on tf32
 // wgmma with P as the register A operand; out = O * (1.0f / l), the division correctly rounded, written as fp32 and/or
 // split2_bf16 planes at [b * nq + q, h * 64 + c] with row stride ldo.
+#include "../../include/spann3r_b200.h"
 #include "common.cuh"
 #include "kernels.cuh"
 #include "wgmma.cuh"
@@ -298,3 +299,18 @@ int attn_launch(const AttnPlan& plan, cudaStream_t st) {
 }
 
 }  // namespace s3r
+
+using namespace s3r;
+
+extern "C" {
+
+int s3r_attention(const float* q, const float* k, const float* vt, int bh, int heads, int nq, int nk, int nk_pad,
+                  void* o_hi, void* o_lo, float* o_f32, int64_t ldo, void* stream) {
+  const AttnDesc d = {q, k, vt, bh, heads, nq, nk, nk_pad, static_cast<__nv_bfloat16*>(o_hi),
+                      static_cast<__nv_bfloat16*>(o_lo), o_f32, ldo};
+  AttnPlan plan;
+  if (int r = attn_plan(d, &plan)) return r;
+  return attn_launch(plan, static_cast<cudaStream_t>(stream));
+}
+
+}  // extern "C"

@@ -35,7 +35,6 @@
 #include "../../include/spann3r_b200.h"
 #include "common.cuh"
 #include "gemm.cuh"
-#include "kernels.cuh"
 
 namespace s3r {
 namespace {
@@ -520,13 +519,20 @@ Src token_major(const float* x, const s3r_attn_train_desc* d) {
 
 }  // namespace
 
-size_t attn_train_workspace_bytes(const s3r_attn_train_desc* d) {
+}  // namespace s3r
+
+using namespace s3r;
+
+extern "C" {
+
+size_t s3r_attn_train_workspace_bytes(const s3r_attn_train_desc* d) {
   if (check_desc(d, "s3r_attn_train_workspace_bytes")) return 0;
   const size_t rows = (size_t)d->batch * d->heads * d->nq;
   return (rows * sizeof(float) + 255) / 256 * 256;
 }
 
-int launch_attn_train_forward(const s3r_attn_train_desc* d, float* o, float* lse, cudaStream_t st) {
+int s3r_attn_train_forward(const s3r_attn_train_desc* d, float* o, float* lse, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (int r = check_desc(d, "s3r_attn_train_forward")) return r;
   if (misaligned(o) || misaligned(lse)) {
     set_error("s3r_attn_train_forward: null or not 16-byte aligned pointer (o, lse)");
@@ -545,15 +551,16 @@ int launch_attn_train_forward(const s3r_attn_train_desc* d, float* o, float* lse
   return 0;
 }
 
-int launch_attn_train_backward(const s3r_attn_train_desc* d, const float* o, const float* lse, const float* d_o,
-                               void* workspace, size_t workspace_bytes, float* dq, float* dk, float* dv, cudaStream_t st) {
+int s3r_attn_train_backward(const s3r_attn_train_desc* d, const float* o, const float* lse, const float* d_o,
+                            void* workspace, size_t workspace_bytes, float* dq, float* dk, float* dv, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (int r = check_desc(d, "s3r_attn_train_backward")) return r;
   if (misaligned(o) || misaligned(lse) || misaligned(d_o) || misaligned(dq) || misaligned(dk) || misaligned(dv) ||
       misaligned(workspace)) {
     set_error("s3r_attn_train_backward: null or not 16-byte aligned pointer (o, lse, d_o, workspace, dq, dk, dv)");
     return -1;
   }
-  const size_t need = attn_train_workspace_bytes(d);
+  const size_t need = s3r_attn_train_workspace_bytes(d);
   if (workspace_bytes < need) {
     set_error("s3r_attn_train_backward: workspace of %zu bytes, %zu needed (s3r_attn_train_workspace_bytes)",
               workspace_bytes, need);
@@ -592,4 +599,4 @@ int launch_attn_train_backward(const s3r_attn_train_desc* d, const float* o, con
   return 0;
 }
 
-}  // namespace s3r
+}  // extern "C"

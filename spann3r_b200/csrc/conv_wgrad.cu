@@ -22,9 +22,9 @@
 //                 3 wgmma (hi*lo, lo*hi, hi*hi) per 64-channel X box into 64 x 64 fp32 register accumulators.
 #include <cstring>
 
+#include "../../include/spann3r_b200.h"
 #include "common.cuh"
 #include "gemm.cuh"
-#include "kernels.cuh"
 #include "wgmma.cuh"
 
 namespace s3r {
@@ -97,13 +97,6 @@ static void wgrad_plan(int NB, int H, int W, int N, int Kc, int taps, WgradPlan*
 static bool valid_shape(int NB, int H, int W, int N, int Kc, int taps) {
   return NB >= 1 && H >= 1 && W >= 1 && N >= 8 && N % 8 == 0 && Kc >= 8 && Kc % 8 == 0 && (taps == 1 || taps == 9) &&
          (long long)NB * H * W < (1LL << 31);
-}
-
-size_t conv_wgrad_workspace_bytes(int NB, int H, int W, int N, int Kc, int taps) {
-  if (!valid_shape(NB, H, W, N, Kc, taps)) return 0;
-  WgradPlan p;
-  wgrad_plan(NB, H, W, N, Kc, taps, &p);
-  return (size_t)p.splits * N * taps * Kc * sizeof(float);
 }
 
 // wgmma shared-memory descriptor of an MN-major operand stored as TMA SWIZZLE_128B wrote it: 128-byte rows along the
@@ -307,9 +300,60 @@ static int encode_nhwc(CUtensorMap* m, const void* base, int NB, int H, int W, i
 
 static bool misaligned(const void* p) { return p == nullptr || (reinterpret_cast<uintptr_t>(p) & 15) != 0; }
 
-int launch_conv_wgrad(const __nv_bfloat16* dy_hi, const __nv_bfloat16* dy_lo, long long ldy, const __nv_bfloat16* x_hi,
-                      const __nv_bfloat16* x_lo, long long ldx, int NB, int H, int W, int N, int Kc, int taps,
-                      void* workspace, size_t workspace_bytes, float* dw, cudaStream_t st) {
+// ------------------------------------------------------------------------------------------------
+// col2im of Conv2d(C, C, 3, stride 2, pad 1): the adjoint of im2col_3x3s2 (elementwise.cu).
+//   cols fp32 [NB*Ho*Wo, 9*C] (k = tap*C + c)  ->  out fp32 [NB, H, W, C]
+// Gather form: each input pixel sums the (at most 4) output pixel / tap pairs that read it, taps in ascending order, so the
+// result is deterministic without atomics.
+// ------------------------------------------------------------------------------------------------
+__global__ void col2im_3x3s2_kernel(const float* __restrict__ cols, int NB, int H, int W, int C, int Ho, int Wo,
+                                    float* __restrict__ out) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int c4 = C >> 2;
+  const long long total = (long long)NB * H * W * c4;
+  for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
+       idx += (long long)gridDim.x * blockDim.x) {
+    const int cc = (int)(idx % c4);
+    const long long t = idx / c4;
+    const int x = (int)(t % W);
+    const int y = (int)((t / W) % H);
+    const int nb = (int)(t / ((long long)W * H));
+    float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+    for (int ky = 0; ky < 3; ++ky) {
+      const int ty = y + 1 - ky;                 // = 2 * oy
+      if (ty < 0 || (ty & 1) || (ty >> 1) >= Ho) continue;
+#pragma unroll
+      for (int kx = 0; kx < 3; ++kx) {
+        const int tx = x + 1 - kx;
+        if (tx < 0 || (tx & 1) || (tx >> 1) >= Wo) continue;
+        const long long row = ((long long)nb * Ho + (ty >> 1)) * Wo + (tx >> 1);
+        const float4 v = *reinterpret_cast<const float4*>(cols + row * 9 * C + (ky * 3 + kx) * C + cc * 4);
+        s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
+      }
+    }
+    *reinterpret_cast<float4*>(out + t * C + cc * 4) = s;
+  }
+}
+
+}  // namespace s3r
+
+using namespace s3r;
+
+extern "C" {
+
+size_t s3r_conv_wgrad_workspace_bytes(int NB, int H, int W, int N, int Kc, int taps) {
+  if (!valid_shape(NB, H, W, N, Kc, taps)) return 0;
+  WgradPlan p;
+  wgrad_plan(NB, H, W, N, Kc, taps, &p);
+  return (size_t)p.splits * N * taps * Kc * sizeof(float);
+}
+
+int s3r_conv_wgrad(const void* dy_hi, const void* dy_lo, int64_t ldy, const void* x_hi, const void* x_lo, int64_t ldx,
+                   int NB, int H, int W, int N, int Kc, int taps, void* workspace, size_t workspace_bytes, float* dw,
+                   void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (!valid_shape(NB, H, W, N, Kc, taps)) {
     set_error("s3r_conv_wgrad: unsupported shape nb=%d h=%d w=%d n=%d kc=%d taps=%d (n, kc multiples of 8, taps in {1,9}, "
               "nb*h*w < 2^31)", NB, H, W, N, Kc, taps);
@@ -325,7 +369,7 @@ int launch_conv_wgrad(const __nv_bfloat16* dy_hi, const __nv_bfloat16* dy_lo, lo
     set_error("s3r_conv_wgrad: null or not 16-byte aligned pointer");
     return -1;
   }
-  const size_t need = conv_wgrad_workspace_bytes(NB, H, W, N, Kc, taps);
+  const size_t need = s3r_conv_wgrad_workspace_bytes(NB, H, W, N, Kc, taps);
   if (workspace_bytes < need) {
     set_error("s3r_conv_wgrad: workspace of %zu bytes, %zu needed (s3r_conv_wgrad_workspace_bytes)", workspace_bytes, need);
     return -1;
@@ -372,44 +416,8 @@ int launch_conv_wgrad(const __nv_bfloat16* dy_hi, const __nv_bfloat16* dy_lo, lo
   return 0;
 }
 
-// ------------------------------------------------------------------------------------------------
-// col2im of Conv2d(C, C, 3, stride 2, pad 1): the adjoint of im2col_3x3s2 (elementwise.cu).
-//   cols fp32 [NB*Ho*Wo, 9*C] (k = tap*C + c)  ->  out fp32 [NB, H, W, C]
-// Gather form: each input pixel sums the (at most 4) output pixel / tap pairs that read it, taps in ascending order, so the
-// result is deterministic without atomics.
-// ------------------------------------------------------------------------------------------------
-__global__ void col2im_3x3s2_kernel(const float* __restrict__ cols, int NB, int H, int W, int C, int Ho, int Wo,
-                                    float* __restrict__ out) {
-  pdl_launch_dependents();
-  pdl_wait();
-  const int c4 = C >> 2;
-  const long long total = (long long)NB * H * W * c4;
-  for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
-       idx += (long long)gridDim.x * blockDim.x) {
-    const int cc = (int)(idx % c4);
-    const long long t = idx / c4;
-    const int x = (int)(t % W);
-    const int y = (int)((t / W) % H);
-    const int nb = (int)(t / ((long long)W * H));
-    float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-    for (int ky = 0; ky < 3; ++ky) {
-      const int ty = y + 1 - ky;                 // = 2 * oy
-      if (ty < 0 || (ty & 1) || (ty >> 1) >= Ho) continue;
-#pragma unroll
-      for (int kx = 0; kx < 3; ++kx) {
-        const int tx = x + 1 - kx;
-        if (tx < 0 || (tx & 1) || (tx >> 1) >= Wo) continue;
-        const long long row = ((long long)nb * Ho + (ty >> 1)) * Wo + (tx >> 1);
-        const float4 v = *reinterpret_cast<const float4*>(cols + row * 9 * C + (ky * 3 + kx) * C + cc * 4);
-        s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
-      }
-    }
-    *reinterpret_cast<float4*>(out + t * C + cc * 4) = s;
-  }
-}
-
-int launch_col2im_3x3s2(const float* cols, int NB, int H, int W, int C, int Ho, int Wo, float* out, cudaStream_t st) {
+int s3r_col2im_3x3s2(const float* cols, int NB, int H, int W, int C, int Ho, int Wo, float* out, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (NB < 1 || H < 1 || W < 1 || C < 8 || C % 8 != 0 || Ho != (H + 1) / 2 || Wo != (W + 1) / 2 ||
       (long long)NB * H * W * C >= (1LL << 40)) {
     set_error("s3r_col2im_3x3s2: unsupported shape nb=%d h=%d w=%d c=%d ho=%d wo=%d (c a multiple of 8, ho = (h+1)/2, "
@@ -431,4 +439,4 @@ int launch_col2im_3x3s2(const float* cols, int NB, int H, int W, int C, int Ho, 
   return 0;
 }
 
-}  // namespace s3r
+}  // extern "C"

@@ -3,6 +3,7 @@
 // and the curope-compatible in-place RoPE shim.  All are plain coalesced / 128-bit vectorised
 // CUDA-core kernels: the data they touch (<= a few MB per call, except the DPT upsamples) lives in
 // the 126 MB L2 between the tensor-core kernels that produce and consume it.
+#include "../../include/spann3r_b200.h"
 #include "kernels.cuh"
 
 #include "common.cuh"
@@ -402,8 +403,19 @@ __global__ void rope2d_kernel(float* __restrict__ tokens, const long long* __res
   }
 }
 
-int launch_rope2d(float* tokens, const long long* pos, long long BN, int H, int D, long long stride_tok,
-                  long long stride_head, float base, float fwd, cudaStream_t st) {
+}  // namespace s3r
+
+using namespace s3r;
+
+static __nv_bfloat16* B(void* p) { return static_cast<__nv_bfloat16*>(p); }
+static const __nv_bfloat16* B(const void* p) { return static_cast<const __nv_bfloat16*>(p); }
+
+extern "C" {
+
+int s3r_rope2d_inplace(float* tokens, const int64_t* pos_, int64_t BN, int H, int D, int64_t stride_tok,
+                       int64_t stride_head, float base, float fwd, void* stream) {
+  const long long* pos = reinterpret_cast<const long long*>(pos_);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (D % 4) { set_error("rope2d: D %% 4 != 0"); return -1; }
   const long long total = BN * H * (D / 2);
   if (total == 0) return 0;
@@ -413,4 +425,30 @@ int launch_rope2d(float* tokens, const long long* pos, long long BN, int H, int 
   return cudaGetLastError() == cudaSuccess ? 0 : -6;
 }
 
-}  // namespace s3r
+int s3r_split(const float* x, int64_t ldx, void* hi, void* lo, int64_t ldp, int col0, int64_t rows, int c, int relu,
+              void* stream) {
+  return launch_split(x, ldx, B(hi), B(lo), ldp, col0, rows, c, relu, static_cast<cudaStream_t>(stream));
+}
+
+int s3r_layernorm(const float* x, int64_t ldx, const float* w, const float* b, int64_t wb_group_stride,
+                  int64_t rows_per_group, float eps, int64_t rows, int c, float* out, int64_t ldo, void* hi, void* lo,
+                  int64_t ldp, int col0, int64_t swap_rows, void* stream) {
+  return launch_layernorm(x, ldx, w, b, wb_group_stride, rows_per_group, eps, rows, c, out, ldo, B(hi), B(lo), ldp,
+                          col0, swap_rows, static_cast<cudaStream_t>(stream));
+}
+
+int s3r_im2col_patch16(const float* img, int64_t sb, int64_t sc, int64_t sy, int64_t sx, int b, int gh, int gw,
+                       void* hi, void* lo, void* stream) {
+  return launch_im2col_patch16(img, sb, sc, sy, sx, b, gh, gw, B(hi), B(lo), static_cast<cudaStream_t>(stream));
+}
+
+int s3r_im2col_3x3s2(const void* ihi, const void* ilo, int nb, int h, int w, int c, int ho, int wo, void* ohi,
+                     void* olo, void* stream) {
+  return launch_im2col_3x3s2(B(ihi), B(ilo), nb, h, w, c, ho, wo, B(ohi), B(olo), static_cast<cudaStream_t>(stream));
+}
+
+int s3r_upsample2x(const float* x, int nb, int h, int w, int c, float* out, void* hi, void* lo, void* stream) {
+  return launch_upsample2x(x, nb, h, w, c, out, B(hi), B(lo), static_cast<cudaStream_t>(stream));
+}
+
+}  // extern "C"

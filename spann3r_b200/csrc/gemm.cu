@@ -706,3 +706,30 @@ int gemm_launch(const GemmPlan& plan, cudaStream_t stream) {
 }
 
 }  // namespace s3r
+
+using namespace s3r;
+
+extern "C" {
+
+int s3r_gemm(const s3r_gemm_desc* d, void* stream) {
+  GemmPlan plan;
+  if (int r = gemm_plan(*d, &plan)) return r;
+  return gemm_launch(plan, static_cast<cudaStream_t>(stream));
+}
+
+int s3r_gemm_tile_n(const s3r_gemm_desc* d) {
+  GemmPlan plan;
+  if (int r = gemm_plan(*d, &plan)) return r;
+  return plan.bn;
+}
+
+int s3r_gemm_plan_bn(int64_t m_tiles, int n, int sms, int col_align, int force_bn) {
+  if (m_tiles < 1 || n < 1 || sms < 1 || col_align < 0) {
+    set_error("s3r_gemm_plan_bn: m_tiles=%lld n=%d sms=%d col_align=%d (positive; col_align >= 0)", (long long)m_tiles,
+              n, sms, col_align);
+    return -1;
+  }
+  return gemm_choose_bn(m_tiles, n, sms, col_align, force_bn);
+}
+
+}  // extern "C"

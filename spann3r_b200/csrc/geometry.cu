@@ -10,7 +10,8 @@
 // (the reference's means cancel in the ratio).  Each iteration is two fixed-shape launches -- 148 x 256-thread partial
 // sums per image in a fixed order, then one block per image -- so the result is deterministic; the pointmap
 // (2.4 MB at 512 x 384) stays in L2 across the 11 passes and never crosses PCIe.
-#include "kernels.cuh"
+#include "../../include/spann3r_b200.h"
+#include "gemm.cuh"
 
 #include "common.cuh"
 #include "focal_math.cuh"
@@ -88,21 +89,6 @@ __global__ void __launch_bounds__(256) focal_final_kernel(const float* __restric
   }
 }
 
-int launch_focal_weiszfeld(const float* pts3d, int B, int H, int W, float ppx, float ppy, int iters, float lo, float hi,
-                           float* scratch, float* focal, cudaStream_t st) {
-  if (B <= 0 || H <= 0 || W <= 0 || iters < 0) {
-    set_error("focal_weiszfeld: bad arguments");
-    return -1;
-  }
-  for (int it = 0; it <= iters; ++it) {
-    launch_pdl(focal_partial_kernel, dim3(kFocalBlocks, B), dim3(256), 0, st, pts3d, H, W, ppx, ppy, (const float*)focal,
-               it == 0 ? 1 : 0, scratch);
-    launch_pdl(focal_final_kernel, dim3(B), dim3(256), 0, st, (const float*)scratch, lo, hi, it == iters ? 1 : 0, focal);
-  }
-  return cudaGetLastError() == cudaSuccess ? 0 : -6;
-}
-
-
 // ------------------------------------------------------------------------------------------------------------------
 // focal_mode='median' (dust3r/post_process.py:26-36): nanmedian over the 2*H*W votes (u z / x, v z / y) of an image.
 // The median is an ELEMENT of the vote set, so it is selected, not averaged: 4 passes of an 8-bit radix select on the
@@ -168,8 +154,30 @@ __global__ void __launch_bounds__(32) focal_median_pick_kernel(int* __restrict__
   }
 }
 
-int launch_focal_median(const float* pts3d, int B, int H, int W, float ppx, float ppy, float lo, float hi, int* scratch,
-                        float* focal, cudaStream_t st) {
+}  // namespace s3r
+
+using namespace s3r;
+
+extern "C" {
+
+int s3r_focal_weiszfeld(const float* pts3d, int B, int H, int W, float ppx, float ppy, int iters, float lo, float hi,
+                        float* scratch, float* focal, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (B <= 0 || H <= 0 || W <= 0 || iters < 0) {
+    set_error("focal_weiszfeld: bad arguments");
+    return -1;
+  }
+  for (int it = 0; it <= iters; ++it) {
+    launch_pdl(focal_partial_kernel, dim3(kFocalBlocks, B), dim3(256), 0, st, pts3d, H, W, ppx, ppy, (const float*)focal,
+               it == 0 ? 1 : 0, scratch);
+    launch_pdl(focal_final_kernel, dim3(B), dim3(256), 0, st, (const float*)scratch, lo, hi, it == iters ? 1 : 0, focal);
+  }
+  return cudaGetLastError() == cudaSuccess ? 0 : -6;
+}
+
+int s3r_focal_median(const float* pts3d, int B, int H, int W, float ppx, float ppy, float lo, float hi, int32_t* scratch,
+                     float* focal, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (!pts3d || !scratch || !focal || B <= 0 || H <= 0 || W <= 0) {
     set_error("focal_median: bad arguments");
     return -1;
@@ -182,4 +190,4 @@ int launch_focal_median(const float* pts3d, int B, int H, int W, float ppx, floa
   return cudaGetLastError() == cudaSuccess ? 0 : -6;
 }
 
-}  // namespace s3r
+}  // extern "C"

@@ -18,7 +18,7 @@
 // No float atomics anywhere: results are bitwise reproducible.
 #include "../../include/spann3r_b200.h"
 #include "common.cuh"
-#include "kernels.cuh"
+#include "gemm.cuh"
 #include "loss_math.cuh"
 
 #include <vector>
@@ -595,14 +595,21 @@ Ws bind(const Cfg& c, void* ws) {
 
 }  // namespace
 
-size_t loss_workspace_bytes(const s3r_loss_desc* d) {
+}  // namespace s3r
+
+using namespace s3r;
+
+extern "C" {
+
+size_t s3r_loss_workspace_bytes(const s3r_loss_desc* d) {
   Cfg c;
   if (check_desc(d, "loss_workspace_bytes", c)) return 0;
   return layout(c.F, c.B, c.P, c.nblk).total;
 }
 
-int launch_loss_forward(const s3r_loss_desc* d, void* ws, size_t ws_bytes, float* gt_out, float* pred_out,
-                        uint8_t* valid_out, double* results, cudaStream_t st) {
+int s3r_loss_forward(const s3r_loss_desc* d, void* ws, size_t ws_bytes, float* gt_out, float* pred_out,
+                     uint8_t* valid_out, double* results, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
   Cfg c;
   if (check_desc(d, "loss_forward", c)) return -1;
   const Layout L = layout(c.F, c.B, c.P, c.nblk);
@@ -647,8 +654,9 @@ int launch_loss_forward(const s3r_loss_desc* d, void* ws, size_t ws_bytes, float
   return 0;
 }
 
-int launch_loss_backward(const s3r_loss_desc* d, const void* ws, size_t ws_bytes, const float* upstream,
-                         float* grad_pred, float* grad_conf, cudaStream_t st) {
+int s3r_loss_backward(const s3r_loss_desc* d, const void* ws, size_t ws_bytes, const float* upstream,
+                      float* grad_pred, float* grad_conf, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
   Cfg c;
   if (check_desc(d, "loss_backward", c)) return -1;
   const Layout L = layout(c.F, c.B, c.P, c.nblk);
@@ -668,4 +676,4 @@ int launch_loss_backward(const s3r_loss_desc* d, const void* ws, size_t ws_bytes
   return 0;
 }
 
-}  // namespace s3r
+}  // extern "C"

@@ -6,6 +6,7 @@
 // write time; LayerNorm is per token, so this equals normalising the whole bank on every read as the
 // reference does) as split-bf16 planes: K_n [B, Mcap, 1024] (GEMM B operand of S = Q K^T) and V_n^T
 // [B, 1024, Mcap] (K-major B operand of O = P V).  Both are streamed by TMA in 128-byte rows.
+#include "../../include/spann3r_b200.h"
 #include "common.cuh"
 #include "kernels.cuh"
 
@@ -161,18 +162,6 @@ __global__ void __launch_bounds__(256) mem_softmax_kernel(const float* __restric
     *reinterpret_cast<uint2*>(ph + 4 * i) = make_uint2(h01, h23);
     *reinterpret_cast<uint2*>(pl + 4 * i) = make_uint2(l01, l23);
   }
-}
-
-int launch_dropout_mask(float* out, long long n, unsigned long long seed, float p, cudaStream_t st) {
-  if (n <= 0) return 0;
-  if (!(p >= 0.f && p < 1.f)) {
-    set_error("dropout_mask: p=%g outside [0, 1)", (double)p);
-    return -1;
-  }
-  const long long blocks = (n + 255) / 256;
-  dropout_mask_kernel<<<(unsigned)(blocks < 2048 ? blocks : 2048), 256, 0, st>>>(out, n, seed, p,
-                                                                                  (float)(1.0 / (1.0 - (double)p)));
-  return cudaGetLastError() == cudaSuccess ? 0 : -6;
 }
 
 int launch_mem_softmax(const float* S, long long ldS, long long rows, int nq, const SlotInts& lens, int Mmax, int Mpad,
@@ -431,14 +420,39 @@ __global__ void __launch_bounds__(256) conf_final_kernel(const float* __restrict
   if (threadIdx.x == 0) out[blockIdx.x] = red[0] / (float)n;
 }
 
-int launch_conf_score(const float* conf, long long n, float* scratch256, float* out, cudaStream_t st) {
+}  // namespace s3r
+
+using namespace s3r;
+
+extern "C" {
+
+int s3r_dropout_mask(float* out, int64_t n, uint64_t seed, float p, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (!out && n > 0) {
+    set_error("s3r_dropout_mask: null output");
+    return -1;
+  }
+  if (n <= 0) return 0;
+  if (!(p >= 0.f && p < 1.f)) {
+    set_error("dropout_mask: p=%g outside [0, 1)", (double)p);
+    return -1;
+  }
+  const long long blocks = (n + 255) / 256;
+  dropout_mask_kernel<<<(unsigned)(blocks < 2048 ? blocks : 2048), 256, 0, st>>>(out, n, seed, p,
+                                                                                  (float)(1.0 / (1.0 - (double)p)));
+  return cudaGetLastError() == cudaSuccess ? 0 : -6;
+}
+
+int s3r_conf_score(const float* conf, int64_t n, float* scratch256, float* out, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (n <= 0) { set_error("conf_score: empty input"); return -1; }
   launch_pdl(conf_partial_kernel, dim3(256), dim3(256), 0, st, conf, n, scratch256);
   launch_pdl(conf_final_kernel, dim3(1), dim3(256), 0, st, (const float*)scratch256, 256, n, out);
   return cudaGetLastError() == cudaSuccess ? 0 : -6;
 }
 
-int launch_conf_score_batched(const float* conf, int batch, long long hw, float* scratch, float* out, cudaStream_t st) {
+int s3r_conf_score_batched(const float* conf, int batch, int64_t hw, float* scratch, float* out, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (batch < 1 || batch > 32767) { set_error("conf_score_batched: batch %d outside [1, 32767]", batch); return -1; }
   if (hw < 1) { set_error("conf_score_batched: H*W = %lld must be >= 1", hw); return -1; }
   if (!conf || !scratch || !out) { set_error("conf_score_batched: null pointer"); return -1; }
@@ -448,4 +462,4 @@ int launch_conf_score_batched(const float* conf, int batch, long long hw, float*
   return cudaGetLastError() == cudaSuccess ? 0 : -6;
 }
 
-}  // namespace s3r
+}  // extern "C"

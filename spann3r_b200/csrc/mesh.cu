@@ -13,7 +13,8 @@
 //                           CTA's threads stride over that one triangle's box.  The minimum does not depend on the order
 //                           the atomics land in, so the result depends neither on scheduling nor on the pass.
 //   raster_resolve_kernel   one thread per pixel: fp32 depth (0 where empty) and int32 face id (-1 where empty).
-#include "kernels.cuh"
+#include "../../include/spann3r_b200.h"
+#include "gemm.cuh"
 
 #include <math.h>
 
@@ -169,14 +170,21 @@ int launched(const char* what) {
 
 }  // namespace
 
-size_t mesh_grid_workspace_bytes(int T, int H, int W) {
+}  // namespace s3r
+
+using namespace s3r;
+
+extern "C" {
+
+size_t s3r_mesh_grid_workspace_bytes(int T, int H, int W) {
   return grid_ok(T, H, W) ? sizeof(long long) * (size_t)(grid_tiles(T, H, W) + 1) : 0;
 }
 
-int launch_mesh_grid_count(const uint8_t* valid, int T, int H, int W, void* workspace, size_t workspace_bytes,
-                           long long* n_faces, cudaStream_t st) {
+int s3r_mesh_grid_count(const uint8_t* valid, int T, int H, int W, void* workspace, size_t workspace_bytes,
+                        int64_t* n_faces, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (!grid_ok(T, H, W) || !valid || !workspace || (uintptr_t)workspace % 8 || !n_faces ||
-      workspace_bytes < mesh_grid_workspace_bytes(T, H, W)) {
+      workspace_bytes < s3r_mesh_grid_workspace_bytes(T, H, W)) {
     set_error("mesh_grid_count: bad arguments (T=%d H=%d W=%d workspace_bytes=%zu; need T, H, W >= 1, T * H * W < 2^31, "
               "an 8-byte aligned workspace of mesh_grid_workspace_bytes and non-null pointers)", T, H, W, workspace_bytes);
     return -1;
@@ -195,10 +203,11 @@ int launch_mesh_grid_count(const uint8_t* valid, int T, int H, int W, void* work
   return 0;
 }
 
-int launch_mesh_grid_faces(const uint8_t* valid, const float* images, int T, int H, int W, const void* workspace,
-                           size_t workspace_bytes, int* faces, float* colors, cudaStream_t st) {
+int s3r_mesh_grid_faces(const uint8_t* valid, const float* images, int T, int H, int W, const void* workspace,
+                        size_t workspace_bytes, int32_t* faces, float* colors, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (!grid_ok(T, H, W) || !valid || !images || !workspace || (uintptr_t)workspace % 8 ||
-      workspace_bytes < mesh_grid_workspace_bytes(T, H, W)) {
+      workspace_bytes < s3r_mesh_grid_workspace_bytes(T, H, W)) {
     set_error("mesh_grid_faces: bad arguments (T=%d H=%d W=%d workspace_bytes=%zu; need T, H, W >= 1, T * H * W < 2^31, "
               "the workspace mesh_grid_count filled and non-null pointers)", T, H, W, workspace_bytes);
     return -1;
@@ -214,9 +223,9 @@ int launch_mesh_grid_faces(const uint8_t* valid, const float* images, int T, int
   return launched("mesh_grid_faces");
 }
 
-int launch_raster_triangles(const float* verts, long long n_verts, const int* faces, long long n_faces, long long id0,
-                            const double* camera, double z_near, double z_far, int w, int h, void* keys,
-                            cudaStream_t st) {
+int s3r_raster_triangles(const float* verts, int64_t n_verts, const int32_t* faces, int64_t n_faces, int64_t id0,
+                         const double* camera, double z_near, double z_far, int w, int h, void* keys, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (!verts || !faces || !camera || !keys || (uintptr_t)keys % 8 || !raster_size_ok(w, h) || n_verts < 0 ||
       n_verts >= (1LL << 31) || n_faces < 0 || id0 < 0 || id0 + n_faces >= (1LL << 31)) {
     set_error("raster_triangles: bad arguments (n_verts=%lld n_faces=%lld id0=%lld w=%d h=%d; need n_verts < 2^31, "
@@ -243,7 +252,8 @@ int launch_raster_triangles(const float* verts, long long n_verts, const int* fa
   return launched("raster_triangles");
 }
 
-int launch_raster_resolve(const void* keys, int w, int h, float* depth, int* face, cudaStream_t st) {
+int s3r_raster_resolve(const void* keys, int w, int h, float* depth, int32_t* face, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (!keys || (uintptr_t)keys % 8 || !depth || !face || !raster_size_ok(w, h)) {
     set_error("raster_resolve: bad arguments (w=%d h=%d; need w, h >= 1, w * h < 2^31, an 8-byte aligned key buffer and "
               "non-null pointers)", w, h);
@@ -255,4 +265,4 @@ int launch_raster_resolve(const void* keys, int w, int h, float* depth, int* fac
   return launched("raster_resolve");
 }
 
-}  // namespace s3r
+}  // extern "C"

@@ -18,7 +18,8 @@
 // HBM-bound point work (12 B per point per pass, the 2.4 MB pointmap stays in L2); the result is the least-squares
 // optimum on the inlier set, so it agrees with cv2 to ~1e-14 on clean data and to the few-inlier difference of two
 // RANSAC runs (~1e-4) otherwise -- tests/test_pnp.py.
-#include "kernels.cuh"
+#include "../../include/spann3r_b200.h"
+#include "gemm.cuh"
 
 #include "common.cuh"
 #include "pnp_math.cuh"
@@ -62,8 +63,6 @@ static PnpWorkspace carve(void* base, int B, int Hn) {
   w.bytes = o;
   return w;
 }
-
-size_t pnp_workspace_bytes(int B, int n_samples) { return carve(nullptr, B, 4 * n_samples).bytes; }
 
 __global__ void __launch_bounds__(64) pnp_hyp_kernel(const float* __restrict__ pts, const float* __restrict__ img,
                                                      long long n, int width, Cam k, unsigned long long seed,
@@ -249,9 +248,21 @@ __global__ void __launch_bounds__(32) pnp_gn_update_kernel(const double* __restr
   }
 }
 
-int launch_pnp_ransac(const float* pts3d, const float* img_pts, int B, long long n, int width, double fx, double fy,
-                      double cx, double cy, float reproj_err, int n_samples, int refine_iters, unsigned long long seed,
-                      void* workspace, double* out, unsigned char* inlier_mask, cudaStream_t st) {
+}  // namespace s3r
+
+using namespace s3r;
+
+extern "C" {
+
+size_t s3r_pnp_workspace_bytes(int B, int n_samples) {
+  if (B <= 0 || n_samples <= 0) return 0;
+  return carve(nullptr, B, 4 * n_samples).bytes;
+}
+
+int s3r_pnp_ransac(const float* pts3d, const float* img_pts, int B, int64_t n, int width, double fx, double fy, double cx,
+                   double cy, float reproj_err, int n_samples, int refine_iters, uint64_t seed, void* workspace,
+                   double* out, uint8_t* inlier_mask, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (!pts3d || !workspace || !out || !inlier_mask || B <= 0 || n < 4 || n_samples <= 0 || n_samples > 4096 ||
       refine_iters < 0 || refine_iters > 100 || !(reproj_err > 0) || !(fx > 0) || !(fy > 0) || (!img_pts && width <= 0)) {
     set_error("pnp_ransac: bad arguments (b=%d n=%lld width=%d samples=%d iters=%d)", B, n, width, n_samples, refine_iters);
@@ -283,4 +294,4 @@ int launch_pnp_ransac(const float* pts3d, const float* img_pts, int B, long long
   return 0;
 }
 
-}  // namespace s3r
+}  // extern "C"

@@ -21,6 +21,7 @@
 //   pattern, which orders like the value for non-negative doubles once -0.0 is keyed as +0.0), count below a threshold.
 //   The select takes any two ranks (launch_pcl_select_ranks), and the stable radix sort any number of 8-bit passes
 //   (launch_pcl_radix_sort); csrc/poisson.cu uses both.
+#include "../../include/spann3r_b200.h"
 #include "kernels.cuh"
 
 #include <climits>
@@ -661,99 +662,6 @@ int launched(const char* what) {
 
 }  // namespace
 
-size_t pcl_index_bytes(long long n) { return n_ok(n) ? carve_index(nullptr, n).bytes : 0; }
-
-int launch_pcl_index_build(const void* pts, int f64, long long n, const double* T, void* index, cudaStream_t st) {
-  if (!pts || !index || !n_ok(n)) {
-    set_error("pcl_index_build: bad arguments (n=%lld; need 1 <= n < 2^31 and non-null pointers)", n);
-    return -1;
-  }
-  if ((uintptr_t)index % 16 != 0) {
-    set_error("pcl_index_build: index workspace must be 16-byte aligned");
-    return -1;
-  }
-  Index x = carve_index(index, n);
-  pcl_box_partial<<<kBoxBlocks, 256, 0, st>>>(pts, f64, n, T, x.part);
-  pcl_box_final<<<1, 32, 0, st>>>(x.part, x.meta);
-  const int g = (int)((n + 255) / 256);
-  pcl_keys_kernel<<<g, 256, 0, st>>>(pts, f64, n, T, x.meta, x.keys[0], x.vals[0]);
-  for (int pass = 0; pass < 8; ++pass) {
-    const int a = pass & 1;
-    pcl_sort_hist<<<x.nblk, 256, 0, st>>>(x.keys[a], n, 8 * pass, x.nblk, x.hist);
-    pcl_sort_scan<<<1, 1024, 0, st>>>(x.hist, 256LL * x.nblk);
-    pcl_sort_scatter<<<x.nblk, 256, 0, st>>>(x.keys[a], x.vals[a], n, 8 * pass, x.nblk, x.hist, x.keys[a ^ 1],
-                                             x.vals[a ^ 1]);
-  }
-  pcl_gather_kernel<<<g, 256, 0, st>>>(pts, f64, n, T, x.vals[0], x.pts, x.orig);
-  pcl_leaf_kernel<<<(x.L + 255) / 256, 256, 0, st>>>(x.pts, n, x.L, x.box);
-  for (int first = x.L / 2; first >= 1; first /= 2)
-    pcl_level_kernel<<<(first + 255) / 256, 256, 0, st>>>(first, first, x.box);
-  return launched("pcl_index_build");
-}
-
-int launch_pcl_nearest(const void* index, long long n, const void* q, int f64, long long nq, const double* T,
-                       double max_dist, double* dist, long long* idx, cudaStream_t st) {
-  if (!index || !q || !dist || !idx || !n_ok(n) || !n_ok(nq) || !(max_dist >= 0)) {
-    set_error("pcl_nearest: bad arguments (n=%lld nq=%lld max_dist=%g)", n, nq, max_dist);
-    return -1;
-  }
-  const Index x = carve_index(const_cast<void*>(index), n);
-  const double max_d2 = bound2(max_dist);
-  pcl_nn_kernel<<<(int)((nq + 127) / 128), 128, 0, st>>>(view_of(x), q, f64, nq, T, max_d2, dist, idx);
-  return launched("pcl_nearest");
-}
-
-int launch_pcl_normals(const void* index, long long n, int k, double* normals, cudaStream_t st) {
-  if (!index || !normals || !n_ok(n) || k < 1 || k > 32) {
-    set_error("pcl_normals: bad arguments (n=%lld k=%d; need 1 <= k <= 32)", n, k);
-    return -1;
-  }
-  const Index x = carve_index(const_cast<void*>(index), n);
-  const int ke = (long long)k < n ? k : (int)n;
-  pcl_normals_kernel<<<(int)((n + 127) / 128), 128, 0, st>>>(view_of(x), ke, normals);
-  return launched("pcl_normals");
-}
-
-size_t pcl_icp_workspace_bytes() { return align256(sizeof(IcpState)) + align256(sizeof(double) * kIcpBlocks * kAccN); }
-
-int launch_pcl_icp(const void* src, int f64, long long ns, const void* target_index, long long nt, double max_corr,
-                   const double* init, int max_iteration, double rel_fitness, double rel_rmse, void* workspace,
-                   double* out, cudaStream_t st) {
-  if (!src || !target_index || !workspace || !out || !n_ok(ns) || !n_ok(nt) || !(max_corr >= 0) || max_iteration < 0 ||
-      max_iteration > 10000 || !(rel_fitness >= 0) || !(rel_rmse >= 0)) {
-    set_error("pcl_icp: bad arguments (ns=%lld nt=%lld max_corr=%g max_iteration=%d)", ns, nt, max_corr, max_iteration);
-    return -1;
-  }
-  if ((uintptr_t)workspace % 16 != 0) {
-    set_error("pcl_icp: workspace must be 16-byte aligned");
-    return -1;
-  }
-  const Index x = carve_index(const_cast<void*>(target_index), nt);
-  IcpState* state = (IcpState*)workspace;
-  double* part = (double*)((uintptr_t)workspace + align256(sizeof(IcpState)));
-  const double max_d2 = bound2(max_corr);
-  pcl_icp_init<<<1, 32, 0, st>>>(init, max_iteration, state, out);
-  for (int j = 0; j <= max_iteration; ++j) {
-    pcl_icp_corr_kernel<<<kIcpBlocks, kIcpThreads, 0, st>>>(view_of(x), x.meta, src, f64, ns, max_d2, state, part);
-    pcl_icp_update_kernel<<<1, 32, 0, st>>>(part, x.meta, ns, max_iteration, rel_fitness, rel_rmse, state, out);
-  }
-  return launched("pcl_icp");
-}
-
-size_t pcl_stats_workspace_bytes() { return align256(sizeof(StatsWs)); }
-
-int launch_pcl_stats(const double* v, long long n, double threshold, void* workspace, double* out, cudaStream_t st) {
-  if (!v || !workspace || !out || !n_ok(n)) {
-    set_error("pcl_stats: bad arguments (n=%lld)", n);
-    return -1;
-  }
-  StatsWs* ws = (StatsWs*)workspace;
-  pcl_stats_partial<<<kStatBlocks, 256, 0, st>>>(v, n, threshold, ws);
-  select_ranks(v, n, (n - 1) / 2, n / 2, ws, st);
-  pcl_stats_final<<<1, 32, 0, st>>>(n, ws, out);
-  return launched("pcl_stats");
-}
-
 int launch_pcl_select_ranks(const double* v, long long n, long long r0, long long r1, void* workspace,
                             const double** picked, cudaStream_t st) {
   if (!v || !workspace || !picked || !n_ok(n) || r0 < 0 || r1 < 0 || r0 >= n || r1 >= n) {
@@ -785,7 +693,116 @@ int launch_pcl_radix_sort(uint64_t* const keys[2], int* const vals[2], long long
   return launched("pcl_radix_sort");
 }
 
-int launch_pcl_abs_dot(const double* a, const double* b, const long long* idx, long long n, double* out, cudaStream_t st) {
+}  // namespace s3r
+
+using namespace s3r;
+
+extern "C" {
+
+size_t s3r_pcl_index_bytes(int64_t n) { return n_ok(n) ? carve_index(nullptr, n).bytes : 0; }
+
+int s3r_pcl_index_build(const void* pts, int f64, int64_t n, const double* T, void* index, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (!pts || !index || !n_ok(n)) {
+    set_error("pcl_index_build: bad arguments (n=%lld; need 1 <= n < 2^31 and non-null pointers)", n);
+    return -1;
+  }
+  if ((uintptr_t)index % 16 != 0) {
+    set_error("pcl_index_build: index workspace must be 16-byte aligned");
+    return -1;
+  }
+  Index x = carve_index(index, n);
+  pcl_box_partial<<<kBoxBlocks, 256, 0, st>>>(pts, f64, n, T, x.part);
+  pcl_box_final<<<1, 32, 0, st>>>(x.part, x.meta);
+  const int g = (int)((n + 255) / 256);
+  pcl_keys_kernel<<<g, 256, 0, st>>>(pts, f64, n, T, x.meta, x.keys[0], x.vals[0]);
+  for (int pass = 0; pass < 8; ++pass) {
+    const int a = pass & 1;
+    pcl_sort_hist<<<x.nblk, 256, 0, st>>>(x.keys[a], n, 8 * pass, x.nblk, x.hist);
+    pcl_sort_scan<<<1, 1024, 0, st>>>(x.hist, 256LL * x.nblk);
+    pcl_sort_scatter<<<x.nblk, 256, 0, st>>>(x.keys[a], x.vals[a], n, 8 * pass, x.nblk, x.hist, x.keys[a ^ 1],
+                                             x.vals[a ^ 1]);
+  }
+  pcl_gather_kernel<<<g, 256, 0, st>>>(pts, f64, n, T, x.vals[0], x.pts, x.orig);
+  pcl_leaf_kernel<<<(x.L + 255) / 256, 256, 0, st>>>(x.pts, n, x.L, x.box);
+  for (int first = x.L / 2; first >= 1; first /= 2)
+    pcl_level_kernel<<<(first + 255) / 256, 256, 0, st>>>(first, first, x.box);
+  return launched("pcl_index_build");
+}
+
+int s3r_pcl_nearest(const void* index, int64_t n, const void* q, int f64, int64_t nq, const double* T, double max_dist,
+                    double* dist, int64_t* idx_, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  long long* idx = reinterpret_cast<long long*>(idx_);
+  if (!index || !q || !dist || !idx || !n_ok(n) || !n_ok(nq) || !(max_dist >= 0)) {
+    set_error("pcl_nearest: bad arguments (n=%lld nq=%lld max_dist=%g)", n, nq, max_dist);
+    return -1;
+  }
+  const Index x = carve_index(const_cast<void*>(index), n);
+  const double max_d2 = bound2(max_dist);
+  pcl_nn_kernel<<<(int)((nq + 127) / 128), 128, 0, st>>>(view_of(x), q, f64, nq, T, max_d2, dist, idx);
+  return launched("pcl_nearest");
+}
+
+int s3r_pcl_normals(const void* index, int64_t n, int k, double* normals, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (!index || !normals || !n_ok(n) || k < 1 || k > 32) {
+    set_error("pcl_normals: bad arguments (n=%lld k=%d; need 1 <= k <= 32)", n, k);
+    return -1;
+  }
+  const Index x = carve_index(const_cast<void*>(index), n);
+  const int ke = (long long)k < n ? k : (int)n;
+  pcl_normals_kernel<<<(int)((n + 127) / 128), 128, 0, st>>>(view_of(x), ke, normals);
+  return launched("pcl_normals");
+}
+
+size_t s3r_pcl_icp_workspace_bytes(void) {
+  return align256(sizeof(IcpState)) + align256(sizeof(double) * kIcpBlocks * kAccN);
+}
+
+int s3r_pcl_icp(const void* src, int f64, int64_t ns, const void* target_index, int64_t nt, double max_corr,
+                const double* init, int max_iteration, double rel_fitness, double rel_rmse, void* workspace, double* out,
+                void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (!src || !target_index || !workspace || !out || !n_ok(ns) || !n_ok(nt) || !(max_corr >= 0) || max_iteration < 0 ||
+      max_iteration > 10000 || !(rel_fitness >= 0) || !(rel_rmse >= 0)) {
+    set_error("pcl_icp: bad arguments (ns=%lld nt=%lld max_corr=%g max_iteration=%d)", ns, nt, max_corr, max_iteration);
+    return -1;
+  }
+  if ((uintptr_t)workspace % 16 != 0) {
+    set_error("pcl_icp: workspace must be 16-byte aligned");
+    return -1;
+  }
+  const Index x = carve_index(const_cast<void*>(target_index), nt);
+  IcpState* state = (IcpState*)workspace;
+  double* part = (double*)((uintptr_t)workspace + align256(sizeof(IcpState)));
+  const double max_d2 = bound2(max_corr);
+  pcl_icp_init<<<1, 32, 0, st>>>(init, max_iteration, state, out);
+  for (int j = 0; j <= max_iteration; ++j) {
+    pcl_icp_corr_kernel<<<kIcpBlocks, kIcpThreads, 0, st>>>(view_of(x), x.meta, src, f64, ns, max_d2, state, part);
+    pcl_icp_update_kernel<<<1, 32, 0, st>>>(part, x.meta, ns, max_iteration, rel_fitness, rel_rmse, state, out);
+  }
+  return launched("pcl_icp");
+}
+
+size_t s3r_pcl_stats_workspace_bytes(void) { return align256(sizeof(StatsWs)); }
+
+int s3r_pcl_stats(const double* v, int64_t n, double threshold, void* workspace, double* out, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (!v || !workspace || !out || !n_ok(n)) {
+    set_error("pcl_stats: bad arguments (n=%lld)", n);
+    return -1;
+  }
+  StatsWs* ws = (StatsWs*)workspace;
+  pcl_stats_partial<<<kStatBlocks, 256, 0, st>>>(v, n, threshold, ws);
+  select_ranks(v, n, (n - 1) / 2, n / 2, ws, st);
+  pcl_stats_final<<<1, 32, 0, st>>>(n, ws, out);
+  return launched("pcl_stats");
+}
+
+int s3r_pcl_abs_dot(const double* a, const double* b, const int64_t* idx_, int64_t n, double* out, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const long long* idx = reinterpret_cast<const long long*>(idx_);
   if (!a || !b || !idx || !out || !n_ok(n)) {
     set_error("pcl_abs_dot: bad arguments (n=%lld)", n);
     return -1;
@@ -794,4 +811,4 @@ int launch_pcl_abs_dot(const double* a, const double* b, const long long* idx, l
   return launched("pcl_abs_dot");
 }
 
-}  // namespace s3r
+}  // extern "C"

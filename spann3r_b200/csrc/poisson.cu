@@ -26,6 +26,7 @@
 //            poisson_vertex_density_kernel interpolates the density grid at every vertex.
 //   trim     pcl_quantile: two exact order statistics (pointcloud.cu's radix select) and numpy's lerp;
 //            mesh_compact_*: remove masked vertices and the faces that use them, renumbering in order.
+#include "../../include/spann3r_b200.h"
 #include "kernels.cuh"
 
 #include <math.h>
@@ -781,7 +782,7 @@ int launched(const char* what) {
 }
 
 int check_ws(const char* what, long long n, int depth, const void* ws, size_t ws_bytes) {
-  if (!args_ok(n, depth) || !ws || (uintptr_t)ws % 256 || ws_bytes < poisson_workspace_bytes(n, depth)) {
+  if (!args_ok(n, depth) || !ws || (uintptr_t)ws % 256 || ws_bytes < s3r_poisson_workspace_bytes(n, depth)) {
     set_error("%s: bad arguments (n=%lld depth=%d workspace_bytes=%zu; need 4 <= n < 2^31, 1 <= depth <= 10 and a "
               "256-byte aligned workspace of s3r_poisson_workspace_bytes(n, depth) bytes)", what, n, depth, ws_bytes);
     return -1;
@@ -853,9 +854,18 @@ struct Solver {
 
 }  // namespace
 
-size_t poisson_workspace_bytes(long long n, int depth) { return args_ok(n, depth) ? carve(nullptr, n, depth).bytes : 0; }
+// After the solve, r / p / q / z are free: node counts in q, node offsets in r, cell counts in z, cell offsets in p.
+}  // namespace s3r
 
-size_t poisson_offset(long long n, int depth, int which) {
+using namespace s3r;
+
+extern "C" {
+
+size_t s3r_poisson_workspace_bytes(int64_t n, int depth) {
+  return args_ok(n, depth) ? carve(nullptr, n, depth).bytes : 0;
+}
+
+size_t s3r_poisson_offset(int64_t n, int depth, int which) {
   if (!args_ok(n, depth) || which < 0 || which > 7) return (size_t)-1;
   const Layout w = carve(nullptr, n, depth);
   // 0: sorted sample order: the sort's final value buffer
@@ -863,8 +873,9 @@ size_t poisson_offset(long long n, int depth, int which) {
   return w.offset[which];
 }
 
-int launch_poisson_setup(const void* pts, const void* nrm, int f64, long long n, int depth, double scale, void* ws,
-                         size_t ws_bytes, double* info, cudaStream_t st) {
+int s3r_poisson_setup(const void* pts, const void* nrm, int f64, int64_t n, int depth, double scale, void* ws,
+                      size_t ws_bytes, double* info, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (int e = check_ws("poisson_setup", n, depth, ws, ws_bytes)) return e;
   if (!pts || !nrm || !info || !(scale >= 1.0) || !isfinite(scale)) {
     set_error("poisson_setup: points, normals and info must be non-null and scale finite and >= 1 (got %g)", scale);
@@ -901,8 +912,9 @@ int launch_poisson_setup(const void* pts, const void* nrm, int f64, long long n,
   return 0;
 }
 
-int launch_poisson_solve(long long n, int depth, double tol, int max_iter, void* ws, size_t ws_bytes, double* info,
-                         cudaStream_t st) {
+int s3r_poisson_solve(int64_t n, int depth, double tol, int max_iter, void* ws, size_t ws_bytes, double* info,
+                      void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (int e = check_ws("poisson_solve", n, depth, ws, ws_bytes)) return e;
   if (!info || !(tol > 0.0) || max_iter < 1) {
     set_error("poisson_solve: info must be non-null, tol > 0 and max_iter >= 1 (got tol=%g max_iter=%d)", tol, max_iter);
@@ -966,8 +978,8 @@ int launch_poisson_solve(long long n, int depth, double tol, int max_iter, void*
   return 0;
 }
 
-// After the solve, r / p / q / z are free: node counts in q, node offsets in r, cell counts in z, cell offsets in p.
-int launch_poisson_extract_count(long long n, int depth, void* ws, size_t ws_bytes, long long* sizes, cudaStream_t st) {
+int s3r_poisson_extract_count(int64_t n, int depth, void* ws, size_t ws_bytes, int64_t* sizes, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (int e = check_ws("poisson_extract_count", n, depth, ws, ws_bytes)) return e;
   if (!sizes) {
     set_error("poisson_extract_count: sizes must be non-null");
@@ -990,8 +1002,10 @@ int launch_poisson_extract_count(long long n, int depth, void* ws, size_t ws_byt
   return launched("poisson_extract_count");
 }
 
-int launch_poisson_extract(long long n, int depth, void* ws, size_t ws_bytes, float* verts, long long* faces,
-                           double* dens, cudaStream_t st) {
+int s3r_poisson_extract(int64_t n, int depth, void* ws, size_t ws_bytes, float* verts, int64_t* faces_, double* dens,
+                        void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  long long* faces = reinterpret_cast<long long*>(faces_);
   if (int e = check_ws("poisson_extract", n, depth, ws, ws_bytes)) return e;
   Meta m;
   const Layout w = carve(ws, n, depth);
@@ -1013,7 +1027,8 @@ int launch_poisson_extract(long long n, int depth, void* ws, size_t ws_bytes, fl
   return launched("poisson_extract");
 }
 
-int launch_pcl_quantile(const double* x, long long n, double q, void* workspace, double* out, cudaStream_t st) {
+int s3r_pcl_quantile(const double* x, int64_t n, double q, void* workspace, double* out, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (!x || !workspace || !out || n < 1 || n >= (1LL << 31) || !(q >= 0.0 && q <= 1.0)) {
     set_error("pcl_quantile: bad arguments (n=%lld q=%g; need 1 <= n < 2^31, 0 <= q <= 1, non-null pointers)", n, q);
     return -1;
@@ -1027,14 +1042,16 @@ int launch_pcl_quantile(const double* x, long long n, double q, void* workspace,
   return launched("pcl_quantile");
 }
 
-size_t mesh_compact_workspace_bytes(long long nv, long long nf) {
+size_t s3r_mesh_compact_workspace_bytes(int64_t nv, int64_t nf) {
   return nv >= 1 && nv < (1LL << 31) && nf >= 0 && nf < (1LL << 31) ? carve_compact(nullptr, nv, nf).bytes : 0;
 }
 
-int launch_mesh_compact_count(const uint8_t* mask, const long long* faces, long long nv, long long nf, void* ws,
-                              size_t ws_bytes, long long* sizes, cudaStream_t st) {
-  if (!mask || !ws || !sizes || (nf && !faces) || (uintptr_t)ws % 256 || mesh_compact_workspace_bytes(nv, nf) == 0 ||
-      ws_bytes < mesh_compact_workspace_bytes(nv, nf)) {
+int s3r_mesh_compact_count(const uint8_t* mask, const int64_t* faces_, int64_t nv, int64_t nf, void* ws,
+                           size_t ws_bytes, int64_t* sizes, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const long long* faces = reinterpret_cast<const long long*>(faces_);
+  if (!mask || !ws || !sizes || (nf && !faces) || (uintptr_t)ws % 256 || s3r_mesh_compact_workspace_bytes(nv, nf) == 0 ||
+      ws_bytes < s3r_mesh_compact_workspace_bytes(nv, nf)) {
     set_error("mesh_compact_count: bad arguments (n_verts=%lld n_faces=%lld workspace_bytes=%zu; need 1 <= n_verts, "
               "n_faces < 2^31, a 256-byte aligned workspace of s3r_mesh_compact_workspace_bytes and non-null pointers)",
               nv, nf, ws_bytes);
@@ -1057,10 +1074,13 @@ int launch_mesh_compact_count(const uint8_t* mask, const long long* faces, long 
   return launched("mesh_compact_count");
 }
 
-int launch_mesh_compact(const float* verts, const long long* faces, long long nv, long long nf, const void* ws,
-                        size_t ws_bytes, float* out_verts, long long* out_faces, cudaStream_t st) {
+int s3r_mesh_compact(const float* verts, const int64_t* faces_, int64_t nv, int64_t nf, const void* ws,
+                     size_t ws_bytes, float* out_verts, int64_t* out_faces_, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const long long* faces = reinterpret_cast<const long long*>(faces_);
+  long long* out_faces = reinterpret_cast<long long*>(out_faces_);
   if (!verts || !ws || !out_verts || (nf && (!faces || !out_faces)) || (uintptr_t)ws % 256 ||
-      mesh_compact_workspace_bytes(nv, nf) == 0 || ws_bytes < mesh_compact_workspace_bytes(nv, nf)) {
+      s3r_mesh_compact_workspace_bytes(nv, nf) == 0 || ws_bytes < s3r_mesh_compact_workspace_bytes(nv, nf)) {
     set_error("mesh_compact: bad arguments (n_verts=%lld n_faces=%lld workspace_bytes=%zu; need the workspace "
               "s3r_mesh_compact_count filled and non-null pointers)", nv, nf, ws_bytes);
     return -1;
@@ -1071,4 +1091,4 @@ int launch_mesh_compact(const float* verts, const long long* faces, long long nv
   return launched("mesh_compact");
 }
 
-}  // namespace s3r
+}  // extern "C"

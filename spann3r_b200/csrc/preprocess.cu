@@ -8,7 +8,8 @@
 // columns that survive the final crop are ever computed.
 //
 // HBM-bound byte work: one read of the crop of the source image, one small uint8 intermediate, one fp32 write.
-#include "kernels.cuh"
+#include "../../include/spann3r_b200.h"
+#include "gemm.cuh"
 
 #include "common.cuh"
 #include "resample_u8.cuh"
@@ -45,8 +46,15 @@ __global__ void __launch_bounds__(256) resample_v_u8_norm_kernel(const uint8_t* 
   dst[((long long)c * out_rows + y) * cols + x] = resample_v_u8_norm_value(tmp, cols, j, y, bounds, kk, ksize);
 }
 
-int launch_resample_h_u8(const uint8_t* src, long long row_stride, int rows, int out_cols, const int* bounds,
-                         const int* kk, int ksize, int max_span, uint8_t* dst, cudaStream_t st) {
+}  // namespace s3r
+
+using namespace s3r;
+
+extern "C" {
+
+int s3r_resample_h_u8(const uint8_t* src, int64_t row_stride, int rows, int out_cols, const int32_t* bounds,
+                      const int32_t* kk, int ksize, int max_span, uint8_t* dst, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (rows <= 0 || out_cols <= 0) return 0;
   const size_t smem = (size_t)3 * max_span;
   if (smem > 160 * 1024) {
@@ -63,12 +71,13 @@ int launch_resample_h_u8(const uint8_t* src, long long row_stride, int rows, int
   return cudaGetLastError() == cudaSuccess ? 0 : -6;
 }
 
-int launch_resample_v_u8_norm(const uint8_t* tmp, int cols, int out_rows, const int* bounds, const int* kk, int ksize,
-                              float* dst, cudaStream_t st) {
+int s3r_resample_v_u8_norm(const uint8_t* tmp, int cols, int out_rows, const int32_t* bounds, const int32_t* kk,
+                           int ksize, float* dst, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (out_rows <= 0 || cols <= 0) return 0;
   launch_pdl(resample_v_u8_norm_kernel, dim3((cols * 3 + 255) / 256, out_rows), dim3(256), 0, st, tmp, cols, out_rows,
              bounds, kk, ksize, dst);
   return cudaGetLastError() == cudaSuccess ? 0 : -6;
 }
 
-}  // namespace s3r
+}  // extern "C"

@@ -10,7 +10,8 @@
 //
 // The key buffer (w * h uint64) is the only state.  Static mode keeps it across frames and splats only the new frame's
 // points, so frame i equals a from-scratch render of frames 0..i at O(H W) work per frame; dynamic mode clears it first.
-#include "kernels.cuh"
+#include "../../include/spann3r_b200.h"
+#include "gemm.cuh"
 
 #include <math.h>
 
@@ -65,20 +66,30 @@ int launched(const char* what) {
 
 }  // namespace
 
-size_t render_workspace_bytes(int w, int h) { return size_ok(w, h) ? sizeof(unsigned long long) * (size_t)w * h : 0; }
+}  // namespace s3r
 
-int launch_render_clear(void* keys, int w, int h, cudaStream_t st) {
+using namespace s3r;
+
+extern "C" {
+
+size_t s3r_render_workspace_bytes(int w, int h) {
+  return size_ok(w, h) ? sizeof(unsigned long long) * (size_t)w * h : 0;
+}
+
+int s3r_render_clear(void* keys, int w, int h, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (!keys_ok(keys) || !size_ok(w, h)) {
     set_error("render_clear: bad arguments (w=%d h=%d; need w, h >= 1, w * h < 2^31 and an 8-byte aligned key buffer)",
               w, h);
     return -1;
   }
-  if (cudaMemsetAsync(keys, 0xff, render_workspace_bytes(w, h), st) != cudaSuccess) return launched("render_clear");
+  if (cudaMemsetAsync(keys, 0xff, s3r_render_workspace_bytes(w, h), st) != cudaSuccess) return launched("render_clear");
   return 0;
 }
 
-int launch_render_splat(const float* pts, const uint8_t* mask, long long n, long long id0, const double* camera,
-                        double z_near, int w, int h, void* keys, cudaStream_t st) {
+int s3r_render_splat(const float* pts, const uint8_t* mask, int64_t n, int64_t id0, const double* camera, double z_near,
+                     int w, int h, void* keys, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (!pts || !camera || !keys_ok(keys) || !size_ok(w, h) || n < 0 || id0 < 0 || id0 + n >= (1LL << 32)) {
     set_error("render_splat: bad arguments (n=%lld id0=%lld w=%d h=%d; need id0 + n < 2^32, w, h >= 1, w * h < 2^31 and "
               "non-null pointers)", n, id0, w, h);
@@ -104,7 +115,8 @@ int launch_render_splat(const float* pts, const uint8_t* mask, long long n, long
   return launched("render_splat");
 }
 
-int launch_render_resolve(const void* keys, const float* colors, int w, int h, uint8_t* out, cudaStream_t st) {
+int s3r_render_resolve(const void* keys, const float* colors, int w, int h, uint8_t* out, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (!keys_ok(keys) || !colors || !out || !size_ok(w, h)) {
     set_error("render_resolve: bad arguments (w=%d h=%d; need w, h >= 1, w * h < 2^31, an 8-byte aligned key buffer and "
               "non-null pointers)", w, h);
@@ -116,4 +128,4 @@ int launch_render_resolve(const void* keys, const float* colors, int w, int h, u
   return launched("render_resolve");
 }
 
-}  // namespace s3r
+}  // extern "C"

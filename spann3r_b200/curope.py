@@ -22,16 +22,13 @@ from . import _lib
 def _launch(tokens: torch.Tensor, positions: torch.Tensor, base: float, fwd: float) -> None:
     B, N, H, D = tokens.shape
     st = tokens.stride()
-    L = _lib.lib()
-    with _lib.on_device(tokens):                # the tokens' device, not whatever device happens to be current
-        sp = _lib.stream_ptr(tokens.device)
-        if B == 1 or st[0] == N * st[1]:        # one uniform token stride across the batch: a single launch
-            _lib.check(L.s3r_rope2d_inplace(_lib.ptr(tokens), _lib.ptr(positions), B * N, H, D, st[1], st[2], float(base),
-                                            float(fwd), sp), "s3r_rope2d_inplace")
-            return
-        for b in range(B):
-            _lib.check(L.s3r_rope2d_inplace(_lib.ptr(tokens[b]), _lib.ptr(positions[b]), N, H, D, st[1], st[2], float(base),
-                                            float(fwd), sp), "s3r_rope2d_inplace")
+    if B == 1 or st[0] == N * st[1]:            # one uniform token stride across the batch: a single launch
+        _lib.call("s3r_rope2d_inplace", tokens, _lib.ptr(tokens), _lib.ptr(positions), B * N, H, D, st[1], st[2],
+                  float(base), float(fwd))
+        return
+    for b in range(B):
+        _lib.call("s3r_rope2d_inplace", tokens, _lib.ptr(tokens[b]), _lib.ptr(positions[b]), N, H, D, st[1], st[2],
+                  float(base), float(fwd))
 
 
 def rope_2d(tokens: torch.Tensor, positions: torch.Tensor, base: float, fwd: float) -> None:

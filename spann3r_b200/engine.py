@@ -14,82 +14,8 @@ import torch
 
 from . import _lib
 from ._lib import _f, _i, _i64, _vp  # noqa: F401
+from ._lib import Bank, BlockW, DecBlockW, DptW, FusionW, Lin, LN, ModelW, Planes, RcuW  # noqa: F401
 
-
-# ------------------------------------------------------------------------------------------------
-# ctypes mirrors of the structs in include/spann3r_b200.h
-# ------------------------------------------------------------------------------------------------
-class Planes(C.Structure):
-    _fields_ = [("hi", _vp), ("lo", _vp)]
-
-
-class LN(C.Structure):
-    _fields_ = [("w", _vp), ("b", _vp)]
-
-
-class Lin(C.Structure):
-    _fields_ = [("w", Planes), ("b", _vp), ("cs", _vp), ("cs_hi", _vp)]
-
-
-class BlockW(C.Structure):
-    _fields_ = [("norm1", LN), ("qkv", Lin), ("proj", Lin), ("norm2", LN), ("fc1", Lin), ("fc2", Lin)]
-
-
-class DecBlockW(C.Structure):
-    _fields_ = [("norm1", LN), ("qkv", Lin), ("proj", Lin), ("norm_y", LN), ("norm2", LN), ("q", Lin),
-                ("cproj", Lin), ("norm3", LN), ("fc1", Lin), ("fc2", Lin)]
-
-
-class RcuW(C.Structure):
-    _fields_ = [("conv1", Lin), ("conv2", Lin)]
-
-
-class FusionW(C.Structure):
-    _fields_ = [("rcu1", RcuW), ("rcu2", RcuW), ("out_conv", Lin)]
-
-
-class DptW(C.Structure):
-    _fields_ = [("act1_conv", Lin), ("act1_up", Lin), ("act2_conv", Lin), ("act2_up", Lin), ("act3_conv", Lin),
-                ("act4_conv", Lin), ("act4_down", Lin), ("layer_rn", Lin * 4), ("refine", FusionW * 4),
-                ("head0", Lin), ("head2", Lin), ("head4_w", _vp), ("head4_b", _vp)]
-
-
-class ModelW(C.Structure):
-    _fields_ = [("patch_embed", Lin), ("enc", BlockW * 24), ("enc_norm", LN),
-                ("decoder_embed", Lin), ("dec", DecBlockW * 12), ("dec_norm", LN),
-                ("key_fc1", Lin), ("key_fc2", Lin), ("dpt", DptW),
-                ("pos_patch_embed", Lin), ("val", BlockW * 6), ("value_norm", LN), ("value_out", Lin),
-                ("norm_q", LN), ("norm_k", LN), ("norm_v", LN),
-                ("rope_cs", _vp), ("rope_maxpos", _i), ("value_dim", _i), ("rope_cs_v", _vp)]
-
-
-class Bank(C.Structure):
-    _fields_ = [("kn_hi", _vp), ("kn_lo", _vp), ("vnt_hi", _vp), ("vnt_lo", _vp), ("k_raw", _vp), ("v_raw", _vp),
-                ("attn", _vp), ("count", _vp), ("cap", _i), ("len", _i)]
-
-
-_lib.register_protos({
-    "s3r_engine_create": (_vp, [C.POINTER(ModelW), _i, _i, _i, _i]),
-    "s3r_engine_create_ex": (_vp, [C.POINTER(ModelW), _i, _i, _i, _i, _i]),
-    "s3r_engine_destroy": (None, [_vp]),
-    "s3r_engine_encode": (_i, [_vp, _vp, _i, _vp, _vp]),
-    "s3r_engine_decode": (_i, [_vp, _vp, _vp, _vp, _vp]),
-    "s3r_engine_keyheads": (_i, [_vp, _vp, _vp, _vp, _vp, _vp]),
-    "s3r_engine_heads": (_i, [_vp, _vp, _vp, _vp]),
-    "s3r_engine_value": (_i, [_vp, _vp, _vp, _i, _vp, _vp]),
-    "s3r_engine_memory_read": (_i, [_vp, C.POINTER(Bank), _vp, _f, _vp, _vp]),
-    "s3r_engine_memory_read_train": (_i, [_vp, C.POINTER(Bank), _vp, _f, _f, C.c_uint64, _vp, _vp]),
-    "s3r_engine_memory_append": (_i, [_vp, C.POINTER(Bank), _vp, _vp, _vp]),
-    "s3r_engine_check_sim": (_i, [_vp, C.POINTER(Bank), _vp, _i, _vp, _vp]),
-    "s3r_engine_memory_read_slots": (_i, [_vp, C.POINTER(Bank), C.POINTER(_i), _vp, _f, _vp, _vp]),
-    "s3r_engine_memory_append_slots": (_i, [_vp, C.POINTER(Bank), C.POINTER(_i), C.POINTER(_i), _vp, _vp, _vp]),
-    "s3r_engine_check_sim_slots": (_i, [_vp, C.POINTER(Bank), C.POINTER(_i), C.POINTER(_i), _vp, _vp, _vp]),
-    "s3r_engine_take_flops": (C.c_double, [_vp]),
-    "s3r_engine_take_launches": (C.c_longlong, [_vp]),
-    "s3r_engine_profile": (None, [_vp, _i]),
-    "s3r_engine_profile_read": (_i, [_vp, C.POINTER(C.c_double)]),
-    "s3r_engine_profile_list": (_i, [_vp, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(_i), _i]),
-})
 
 ROPE_MAXPOS = 64
 MAX_SLOTS = 64      # include/spann3r_b200.h: S3R_MAX_SLOTS, the batch limit of the per-slot memory stages
@@ -443,11 +369,10 @@ class Engine:
         if not self._h:
             raise _lib.S3RError("s3r_engine_create failed: " + L.s3r_last_error().decode())
 
-    def _call(self, name, what, *args):
+    def _call(self, name, *args):
         """One engine stage on the engine's own device and that device's current stream (the library launches on the
         current device; the C side refuses a call made while another device is current)."""
-        with torch.cuda.device(self.device):
-            _lib.check(getattr(_lib.lib(), name)(self._h, *args, _lib.stream_ptr(self.device)), what)
+        _lib.call(name, self.device, self._h, *args)
 
     def __del__(self):
         h, self._h = getattr(self, "_h", None), None
@@ -471,25 +396,25 @@ class Engine:
         nimg = img.shape[0]
         self._chk(img, (nimg, 3, self.H, self.W))
         feat = self._new(nimg, self.N, 1024)
-        self._call("s3r_engine_encode", "encode", _lib.ptr(img), nimg, _lib.ptr(feat))
+        self._call("s3r_engine_encode", _lib.ptr(img), nimg, _lib.ptr(feat))
         return feat
 
     def decode(self, f1, f2, want_all=False):
         self._chk(f1, (self.B, self.N, 1024)); self._chk(f2, (self.B, self.N, 1024))
         dec_all = self._new(12, 2, self.B, self.N, 768) if want_all else None
-        self._call("s3r_engine_decode", "decode", _lib.ptr(f1), _lib.ptr(f2), _lib.ptr(dec_all))
+        self._call("s3r_engine_decode", _lib.ptr(f1), _lib.ptr(f2), _lib.ptr(dec_all))
         return dec_all
 
     def keyheads(self, feat1, feat2):
         self._chk(feat1, (self.B, self.N, 1024)); self._chk(feat2, (self.B, self.N, 1024))
         k1, k2 = self._new(self.B, self.N, 1024), self._new(self.B, self.N, 1024)
-        self._call("s3r_engine_keyheads", "keyheads", _lib.ptr(feat1), _lib.ptr(feat2), _lib.ptr(k1), _lib.ptr(k2))
+        self._call("s3r_engine_keyheads", _lib.ptr(feat1), _lib.ptr(feat2), _lib.ptr(k1), _lib.ptr(k2))
         return k1, k2
 
     def heads(self):
         pts = self._new(2, self.B, self.H, self.W, 3)
         conf = self._new(2, self.B, self.H, self.W)
-        self._call("s3r_engine_heads", "heads", _lib.ptr(pts), _lib.ptr(conf))
+        self._call("s3r_engine_heads", _lib.ptr(pts), _lib.ptr(conf))
         return pts, conf
 
     def value(self, pts3d, feat_k1, transposed: bool = False, rope: bool = False, tokens: bool = False):
@@ -505,7 +430,7 @@ class Engine:
         self._chk(feat_k1, (self.B, self.N, 1024))
         out = self._new(self.B, self.N, 1024)
         flags = (VALUE_PTS_TRANSPOSED if transposed else 0) | (VALUE_ROPE if rope else 0) | (VALUE_DEC_TOKENS if tokens else 0)
-        self._call("s3r_engine_value", "value", _lib.ptr(pts3d), _lib.ptr(feat_k1), flags, _lib.ptr(out))
+        self._call("s3r_engine_value", _lib.ptr(pts3d), _lib.ptr(feat_k1), flags, _lib.ptr(out))
         return out
 
     def memory_read(self, bank: MemoryBank, feat, thresh: float, drop_p: float = 0.0, seed: int = 0):
@@ -514,22 +439,22 @@ class Engine:
         out = self._new(self.B, self.N, 1024)
         bs = bank.struct()
         if drop_p > 0.0:
-            self._call("s3r_engine_memory_read_train", "memory_read", C.byref(bs), _lib.ptr(feat), float(thresh), float(drop_p),
+            self._call("s3r_engine_memory_read_train", C.byref(bs), _lib.ptr(feat), float(thresh), float(drop_p),
                        int(seed) & 0xFFFFFFFFFFFFFFFF, _lib.ptr(out))
         else:
-            self._call("s3r_engine_memory_read", "memory_read", C.byref(bs), _lib.ptr(feat), float(thresh), _lib.ptr(out))
+            self._call("s3r_engine_memory_read", C.byref(bs), _lib.ptr(feat), float(thresh), _lib.ptr(out))
         return out
 
     def memory_append(self, bank: MemoryBank, feat_k, feat_v):
         self._chk(feat_k, (self.B, self.N, 1024)); self._chk(feat_v, (self.B, self.N, 1024))
         bs = bank.struct()
-        self._call("s3r_engine_memory_append", "memory_append", C.byref(bs), _lib.ptr(feat_k), _lib.ptr(feat_v))
+        self._call("s3r_engine_memory_append", C.byref(bs), _lib.ptr(feat_k), _lib.ptr(feat_v))
         bank.len += self.N
 
     def check_sim(self, bank: MemoryBank, feat_k, wm: int) -> torch.Tensor:
         out = self._new(self.B, wm)
         bs = bank.struct()
-        self._call("s3r_engine_check_sim", "check_sim", C.byref(bs), _lib.ptr(feat_k), wm, _lib.ptr(out))
+        self._call("s3r_engine_check_sim", C.byref(bs), _lib.ptr(feat_k), wm, _lib.ptr(out))
         return out
 
     # -- per-slot memory stages (independent sequences, one per batch item) ------------------------------------
@@ -543,21 +468,21 @@ class Engine:
         """memory_read with slot b reading its first lens[b] tokens; a slot of length 0 returns its feat row unchanged."""
         self._chk(feat, (self.B, self.N, 1024))
         out = self._new(self.B, self.N, 1024)
-        self._call("s3r_engine_memory_read_slots", "memory_read_slots", C.byref(bank.struct()), self._slot_ints(lens),
+        self._call("s3r_engine_memory_read_slots", C.byref(bank.struct()), self._slot_ints(lens),
                    _lib.ptr(feat), float(thresh), _lib.ptr(out))
         return out
 
     def memory_append_slots(self, bank: MemoryBank, lens, append, feat_k, feat_v):
         """Slot b with append[b] takes its N tokens at offset lens[b]; the caller tracks the lengths."""
         self._chk(feat_k, (self.B, self.N, 1024)); self._chk(feat_v, (self.B, self.N, 1024))
-        self._call("s3r_engine_memory_append_slots", "memory_append_slots", C.byref(bank.struct()), self._slot_ints(lens),
+        self._call("s3r_engine_memory_append_slots", C.byref(bank.struct()), self._slot_ints(lens),
                    self._slot_ints(append), _lib.ptr(feat_k), _lib.ptr(feat_v))
 
     def check_sim_slots(self, bank: MemoryBank, lens, wm, feat_k) -> torch.Tensor:
         """[B, 8]: slot b's gate values against its last wm[b] frames ending at lens[b]; -inf past wm[b]."""
         self._chk(feat_k, (self.B, self.N, 1024))
         out = self._new(self.B, 8)
-        self._call("s3r_engine_check_sim_slots", "check_sim_slots", C.byref(bank.struct()), self._slot_ints(lens),
+        self._call("s3r_engine_check_sim_slots", C.byref(bank.struct()), self._slot_ints(lens),
                    self._slot_ints(wm), _lib.ptr(feat_k), _lib.ptr(out))
         return out
 

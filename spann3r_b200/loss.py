@@ -151,20 +151,16 @@ class _Call:
             gt_out = torch.empty((F, B, H, W, 3), dtype=torch.float32, device=self.dev)
             pred_out = torch.empty((2 * (F - 1), B, H, W, 3), dtype=torch.float32, device=self.dev)
             valid_out = torch.empty((F, B, H, W), dtype=torch.uint8, device=self.dev)
-        with _lib.on_device(self.dev):
-            _lib.check(_lib.lib().s3r_loss_forward(C.byref(self.desc), _lib.ptr(self.ws), self.ws_bytes, _lib.ptr(gt_out),
-                                                   _lib.ptr(pred_out), _lib.ptr(valid_out), _lib.ptr(self.results),
-                                                   _lib.stream_ptr(self.dev)), "s3r_loss_forward")
+        _lib.call("s3r_loss_forward", self.dev, C.byref(self.desc), _lib.ptr(self.ws), self.ws_bytes, _lib.ptr(gt_out),
+                  _lib.ptr(pred_out), _lib.ptr(valid_out), _lib.ptr(self.results))
         return gt_out, pred_out, valid_out
 
     def backward(self, upstream):
         B, H, W, S = self.B, self.H, self.W, 2 * (self.F - 1)
         gp = torch.empty((S, B, H, W, 3), dtype=torch.float32, device=self.dev)
         gc = torch.empty((S, B, H, W), dtype=torch.float32, device=self.dev) if self.desc.conf_loss else None
-        with _lib.on_device(self.dev):
-            _lib.check(_lib.lib().s3r_loss_backward(C.byref(self.desc), _lib.ptr(self.ws), self.ws_bytes,
-                                                    _lib.ptr(upstream), _lib.ptr(gp), _lib.ptr(gc),
-                                                    _lib.stream_ptr(self.dev)), "s3r_loss_backward")
+        _lib.call("s3r_loss_backward", self.dev, C.byref(self.desc), _lib.ptr(self.ws), self.ws_bytes, _lib.ptr(upstream),
+                  _lib.ptr(gp), _lib.ptr(gc))
         return gp, gc
 
     def per_b(self, i):

@@ -68,21 +68,17 @@ def pts3d_to_mesh(pts_all, images_all, mask=None):
     if not bool((finite | ~mask).all()):
         raise ValueError("pts_all / images_all: non-finite values at valid pixels")
     _lib.require_device()
-    L = _lib.lib()
     dev = pts_all.device
     valid = mask.view(torch.uint8)
-    ws_bytes = int(L.s3r_mesh_grid_workspace_bytes(T, H, W))
+    ws_bytes = int(_lib.lib().s3r_mesh_grid_workspace_bytes(T, H, W))
     ws = torch.empty(ws_bytes // 8, dtype=torch.int64, device=dev)
     n = C.c_int64(0)
-    with _lib.on_device(dev):
-        st = _lib.stream_ptr(dev)
-        _lib.check(L.s3r_mesh_grid_count(_lib.ptr(valid), T, H, W, _lib.ptr(ws), ws_bytes, C.byref(n), st),
-                   "s3r_mesh_grid_count")
-        faces = torch.empty((n.value, 3), dtype=torch.int32, device=dev)
-        colors = torch.empty((n.value, 3), dtype=torch.float32, device=dev)
-        if n.value:
-            _lib.check(L.s3r_mesh_grid_faces(_lib.ptr(valid), _lib.ptr(images_all), T, H, W, _lib.ptr(ws), ws_bytes,
-                                             _lib.ptr(faces), _lib.ptr(colors), st), "s3r_mesh_grid_faces")
+    _lib.call("s3r_mesh_grid_count", dev, _lib.ptr(valid), T, H, W, _lib.ptr(ws), ws_bytes, C.byref(n))
+    faces = torch.empty((n.value, 3), dtype=torch.int32, device=dev)
+    colors = torch.empty((n.value, 3), dtype=torch.float32, device=dev)
+    if n.value:
+        _lib.call("s3r_mesh_grid_faces", dev, _lib.ptr(valid), _lib.ptr(images_all), T, H, W, _lib.ptr(ws), ws_bytes,
+                  _lib.ptr(faces), _lib.ptr(colors))
     return pts_all.reshape(-1, 3), faces, colors
 
 
@@ -218,15 +214,15 @@ def _planes(z_near, z_far):
     return z_near, z_far
 
 
-def _draw(L, keys, v, f, cam, z_near, z_far, w, h, st, id0=0):
+def _draw(keys, v, f, cam, z_near, z_far, w, h, id0=0):
     if len(f) == 0:
         return
-    _lib.check(L.s3r_raster_triangles(_lib.ptr(v), len(v), _lib.ptr(f), len(f), id0, C.c_void_p(cam.ctypes.data),
-                                      z_near, z_far, w, h, _lib.ptr(keys), st), "s3r_raster_triangles")
+    _lib.call("s3r_raster_triangles", keys, _lib.ptr(v), len(v), _lib.ptr(f), len(f), id0, C.c_void_p(cam.ctypes.data),
+              z_near, z_far, w, h, _lib.ptr(keys))
 
 
-def _resolve(L, keys, w, h, depth, face, st):
-    _lib.check(L.s3r_raster_resolve(_lib.ptr(keys), w, h, _lib.ptr(depth), _lib.ptr(face), st), "s3r_raster_resolve")
+def _resolve(keys, w, h, depth, face):
+    _lib.call("s3r_raster_resolve", keys, _lib.ptr(keys), w, h, _lib.ptr(depth), _lib.ptr(face))
 
 
 def rasterize(vertices, faces, camera, w, h, z_near=0.0, z_far=math.inf):
@@ -241,16 +237,13 @@ def rasterize(vertices, faces, camera, w, h, z_near=0.0, z_far=math.inf):
     w, h = _size(w, h)
     z_near, z_far = _planes(z_near, z_far)
     _lib.require_device()
-    L = _lib.lib()
     dev = v.device
-    keys = torch.empty(int(L.s3r_render_workspace_bytes(w, h)) // 8, dtype=torch.int64, device=dev)
+    keys = torch.empty(int(_lib.lib().s3r_render_workspace_bytes(w, h)) // 8, dtype=torch.int64, device=dev)
     depth = torch.empty((h, w), dtype=torch.float32, device=dev)
     face = torch.empty((h, w), dtype=torch.int32, device=dev)
-    with _lib.on_device(dev):
-        st = _lib.stream_ptr(dev)
-        _lib.check(L.s3r_render_clear(_lib.ptr(keys), w, h, st), "s3r_render_clear")
-        _draw(L, keys, v, f, cam, z_near, z_far, w, h, st)
-        _resolve(L, keys, w, h, depth, face, st)
+    _lib.call("s3r_render_clear", keys, _lib.ptr(keys), w, h)
+    _draw(keys, v, f, cam, z_near, z_far, w, h)
+    _resolve(keys, w, h, depth, face)
     return depth, face
 
 
@@ -291,17 +284,14 @@ def _to_device_mesh(mesh, device):
 
 def _depth_maps(v, f, cams, H, W, near, far):
     """[len(cams), H, W] fp32 CUDA: one draw per camera against the same device mesh."""
-    L = _lib.lib()
     dev = v.device
-    keys = torch.empty(int(L.s3r_render_workspace_bytes(W, H)) // 8, dtype=torch.int64, device=dev)
+    keys = torch.empty(int(_lib.lib().s3r_render_workspace_bytes(W, H)) // 8, dtype=torch.int64, device=dev)
     depth = torch.empty((len(cams), H, W), dtype=torch.float32, device=dev)
     face = torch.empty((H, W), dtype=torch.int32, device=dev)
-    with _lib.on_device(dev):
-        st = _lib.stream_ptr(dev)
-        for i, cam in enumerate(cams):
-            _lib.check(L.s3r_render_clear(_lib.ptr(keys), W, H, st), "s3r_render_clear")
-            _draw(L, keys, v, f, cam, near, far, W, H, st)
-            _resolve(L, keys, W, H, depth[i], face, st)
+    for i, cam in enumerate(cams):
+        _lib.call("s3r_render_clear", keys, _lib.ptr(keys), W, H)
+        _draw(keys, v, f, cam, near, far, W, H)
+        _resolve(keys, W, H, depth[i], face)
     return depth
 
 
@@ -578,19 +568,15 @@ class _Poisson:
         if float((p.amax(0) - p.amin(0)).max()) == 0.0:
             raise ValueError("points: the bounding box has zero extent")
         _lib.require_device()
-        L = _lib.lib()
         self.n, self.depth, self.device = N, int(depth), p.device
-        self.ws_bytes = int(L.s3r_poisson_workspace_bytes(N, self.depth))
+        self.ws_bytes = int(_lib.lib().s3r_poisson_workspace_bytes(N, self.depth))
         self.ws = torch.empty(self.ws_bytes, dtype=torch.uint8, device=self.device)
         info = np.zeros(8, np.float64)
         out = np.zeros(3, np.float64)
-        with _lib.on_device(self.device):
-            st = _lib.stream_ptr(self.device)
-            _lib.check(L.s3r_poisson_setup(_lib.ptr(p), _lib.ptr(n), int(p.dtype == torch.float64), N, self.depth, scale,
-                                           _lib.ptr(self.ws), self.ws_bytes, C.c_void_p(info.ctypes.data), st),
-                       "s3r_poisson_setup")
-            _lib.check(L.s3r_poisson_solve(N, self.depth, POISSON_TOL, POISSON_MAX_ITER, _lib.ptr(self.ws), self.ws_bytes,
-                                           C.c_void_p(out.ctypes.data), st), "s3r_poisson_solve")
+        _lib.call("s3r_poisson_setup", self.device, _lib.ptr(p), _lib.ptr(n), int(p.dtype == torch.float64), N, self.depth,
+                  scale, _lib.ptr(self.ws), self.ws_bytes, C.c_void_p(info.ctypes.data))
+        _lib.call("s3r_poisson_solve", self.device, N, self.depth, POISSON_TOL, POISSON_MAX_ITER, _lib.ptr(self.ws),
+                  self.ws_bytes, C.c_void_p(out.ctypes.data))
         self.origin, self.L, self.h = info[:3].copy(), float(info[3]), float(info[4])
         self.a, self.beta, self.occupied = float(info[5]), float(info[6]), int(info[7])
         self.iterations, self.residual, self.iso = int(out[0]), float(out[1]), float(out[2])
@@ -602,18 +588,15 @@ class _Poisson:
         return self.ws[off:off + nbytes].view(dtype)
 
     def extract(self):
-        L = _lib.lib()
         sizes = np.zeros(2, np.int64)
-        with _lib.on_device(self.device):
-            st = _lib.stream_ptr(self.device)
-            _lib.check(L.s3r_poisson_extract_count(self.n, self.depth, _lib.ptr(self.ws), self.ws_bytes,
-                                                   C.c_void_p(sizes.ctypes.data), st), "s3r_poisson_extract_count")
-            nv, nf = int(sizes[0]), int(sizes[1])
-            v = torch.empty((nv, 3), dtype=torch.float32, device=self.device)
-            f = torch.empty((nf, 3), dtype=torch.int64, device=self.device)
-            d = torch.empty(nv, dtype=torch.float64, device=self.device)
-            _lib.check(L.s3r_poisson_extract(self.n, self.depth, _lib.ptr(self.ws), self.ws_bytes, _lib.ptr(v), _lib.ptr(f),
-                                             _lib.ptr(d), st), "s3r_poisson_extract")
+        _lib.call("s3r_poisson_extract_count", self.device, self.n, self.depth, _lib.ptr(self.ws), self.ws_bytes,
+                  C.c_void_p(sizes.ctypes.data))
+        nv, nf = int(sizes[0]), int(sizes[1])
+        v = torch.empty((nv, 3), dtype=torch.float32, device=self.device)
+        f = torch.empty((nf, 3), dtype=torch.int64, device=self.device)
+        d = torch.empty(nv, dtype=torch.float64, device=self.device)
+        _lib.call("s3r_poisson_extract", self.device, self.n, self.depth, _lib.ptr(self.ws), self.ws_bytes, _lib.ptr(v),
+                  _lib.ptr(f), _lib.ptr(d))
         return v, f, d
 
 
@@ -642,19 +625,16 @@ def remove_vertices_by_mask(vertices, faces, mask):
     if len(f) and (int(f.min()) < 0 or int(f.max()) >= len(v)):
         raise ValueError(f"faces: indices must lie in [0, {len(v)})")
     _lib.require_device()
-    L = _lib.lib()
     m = mask.contiguous().view(torch.uint8)
-    ws_bytes = int(L.s3r_mesh_compact_workspace_bytes(len(v), len(f)))
+    ws_bytes = int(_lib.lib().s3r_mesh_compact_workspace_bytes(len(v), len(f)))
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device=v.device)
     sizes = np.zeros(2, np.int64)
-    with _lib.on_device(v.device):
-        st = _lib.stream_ptr(v.device)
-        _lib.check(L.s3r_mesh_compact_count(_lib.ptr(m), _lib.ptr(f), len(v), len(f), _lib.ptr(ws), ws_bytes,
-                                            C.c_void_p(sizes.ctypes.data), st), "s3r_mesh_compact_count")
-        ov = torch.empty((int(sizes[0]), 3), dtype=torch.float32, device=v.device)
-        of = torch.empty((int(sizes[1]), 3), dtype=torch.int64, device=v.device)
-        _lib.check(L.s3r_mesh_compact(_lib.ptr(v), _lib.ptr(f), len(v), len(f), _lib.ptr(ws), ws_bytes, _lib.ptr(ov),
-                                      _lib.ptr(of), st), "s3r_mesh_compact")
+    _lib.call("s3r_mesh_compact_count", v, _lib.ptr(m), _lib.ptr(f), len(v), len(f), _lib.ptr(ws), ws_bytes,
+              C.c_void_p(sizes.ctypes.data))
+    ov = torch.empty((int(sizes[0]), 3), dtype=torch.float32, device=v.device)
+    of = torch.empty((int(sizes[1]), 3), dtype=torch.int64, device=v.device)
+    _lib.call("s3r_mesh_compact", v, _lib.ptr(v), _lib.ptr(f), len(v), len(f), _lib.ptr(ws), ws_bytes, _lib.ptr(ov),
+              _lib.ptr(of))
     return ov, of
 
 
@@ -666,12 +646,9 @@ def quantile(x, q) -> torch.Tensor:
     if not (0.0 <= q <= 1.0) or len(x) == 0 or len(x) >= 2 ** 31:
         raise ValueError(f"quantile: need 0 <= q <= 1 and 1 <= len(x) < 2^31, got {q}, {len(x)}")
     _lib.require_device()
-    L = _lib.lib()
-    ws = torch.empty(int(L.s3r_pcl_stats_workspace_bytes()), dtype=torch.uint8, device=x.device)
+    ws = torch.empty(int(_lib.lib().s3r_pcl_stats_workspace_bytes()), dtype=torch.uint8, device=x.device)
     out = torch.empty(1, dtype=torch.float64, device=x.device)
-    with _lib.on_device(x.device):
-        _lib.check(L.s3r_pcl_quantile(_lib.ptr(x), len(x), q, _lib.ptr(ws), _lib.ptr(out), _lib.stream_ptr(x.device)),
-                   "s3r_pcl_quantile")
+    _lib.call("s3r_pcl_quantile", x, _lib.ptr(x), len(x), q, _lib.ptr(ws), _lib.ptr(out))
     return out
 
 

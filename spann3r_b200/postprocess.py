@@ -30,15 +30,10 @@ def estimate_focal_knowing_depth(pts3d: torch.Tensor, pp, focal_mode: str = "med
     focal = torch.empty(B, dtype=torch.float32, device=pts3d.device)
     if focal_mode == "median":      # nanmedian of the per-pixel votes: an exact selection, bit-identical to the reference
         scratch = torch.empty(B * 260, dtype=torch.int32, device=pts3d.device)
-        with _lib.on_device(pts3d):
-            _lib.check(_lib.lib().s3r_focal_median(_lib.ptr(pts3d), B, H, W, ppx, ppy, lo, hi, _lib.ptr(scratch),
-                                                   _lib.ptr(focal), _lib.stream_ptr(pts3d.device)),
-                       "s3r_focal_median")
+        _lib.call("s3r_focal_median", pts3d, _lib.ptr(pts3d), B, H, W, ppx, ppy, lo, hi, _lib.ptr(scratch), _lib.ptr(focal))
         return focal
     scratch = torch.empty(B * 148 * 2, dtype=torch.float32, device=pts3d.device)
-    with _lib.on_device(pts3d):
-        _lib.check(_lib.lib().s3r_focal_weiszfeld(_lib.ptr(pts3d), B, H, W, ppx, ppy, 10, lo, hi, _lib.ptr(scratch),
-                                                  _lib.ptr(focal), _lib.stream_ptr(pts3d.device)), "s3r_focal_weiszfeld")
+    _lib.call("s3r_focal_weiszfeld", pts3d, _lib.ptr(pts3d), B, H, W, ppx, ppy, 10, lo, hi, _lib.ptr(scratch), _lib.ptr(focal))
     return focal
 
 
@@ -75,12 +70,10 @@ def solve_pnp_ransac(pts3d: torch.Tensor, camera_matrix, image_points: torch.Ten
             raise ValueError("image_points must be float32 on the GPU")
         image_points = image_points.contiguous()
         n, width, out_shape = pts3d.shape[1], 0, tuple(pts3d.shape[:2])
-    L = _lib.lib()
-    ws = torch.empty(int(L.s3r_pnp_workspace_bytes(B, int(iterations_count))), dtype=torch.uint8, device=pts3d.device)
+    ws = torch.empty(int(_lib.lib().s3r_pnp_workspace_bytes(B, int(iterations_count))), dtype=torch.uint8, device=pts3d.device)
     out = torch.empty(B, 18, dtype=torch.float64, device=pts3d.device)
     mask = torch.empty(B, n, dtype=torch.uint8, device=pts3d.device)
-    with _lib.on_device(pts3d):
-        _lib.check(L.s3r_pnp_ransac(_lib.ptr(pts3d), _lib.ptr(image_points), B, n, width, fx, fy, cx, cy,
-                                    float(reprojection_error), int(iterations_count), int(refine_iters), int(seed),
-                                    _lib.ptr(ws), _lib.ptr(out), _lib.ptr(mask), _lib.stream_ptr(pts3d.device)), "s3r_pnp_ransac")
+    _lib.call("s3r_pnp_ransac", pts3d, _lib.ptr(pts3d), _lib.ptr(image_points), B, n, width, fx, fy, cx, cy,
+              float(reprojection_error), int(iterations_count), int(refine_iters), int(seed), _lib.ptr(ws), _lib.ptr(out),
+              _lib.ptr(mask))
     return out[:, 17] > 0.5, out[:, 12:15], out[:, 9:12], mask.view(out_shape).bool()

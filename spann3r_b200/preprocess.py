@@ -153,14 +153,11 @@ class FrameAdapter:
         p = self._plan(h, w, square_flip)
         src = rgb.to(self.device, non_blocking=True).contiguous()
         out = torch.empty((1, 3, p["out_h"], p["out_w"]), dtype=torch.float32, device=self.device)
-        L = _lib.lib()
         src_ptr = src.data_ptr() + (p["src_row0"] * w + p["src_col0"]) * 3
-        with _lib.on_device(out):
-            sp = _lib.stream_ptr(out.device)
-            _lib.check(L.s3r_resample_h_u8(src_ptr, w * 3, p["rows"], p["out_w"], _lib.ptr(p["bh"]), _lib.ptr(p["kh"]), p["ksh"],
-                                           p["span"], _lib.ptr(p["tmp"]), sp), "s3r_resample_h_u8")
-            _lib.check(L.s3r_resample_v_u8_norm(_lib.ptr(p["tmp"]), p["out_w"], p["out_h"], _lib.ptr(p["bv"]), _lib.ptr(p["kv"]),
-                                                p["ksv"], _lib.ptr(out), sp), "s3r_resample_v_u8_norm")
+        _lib.call("s3r_resample_h_u8", out, src_ptr, w * 3, p["rows"], p["out_w"], _lib.ptr(p["bh"]), _lib.ptr(p["kh"]),
+                  p["ksh"], p["span"], _lib.ptr(p["tmp"]))
+        _lib.call("s3r_resample_v_u8_norm", out, _lib.ptr(p["tmp"]), p["out_w"], p["out_h"], _lib.ptr(p["bv"]),
+                  _lib.ptr(p["kv"]), p["ksv"], _lib.ptr(out))
         return out
 
 

@@ -65,11 +65,8 @@ class PointIndex:
         self.n = points.shape[0]
         # _device_rt: a [3, 4] fp64 transform this module computed on the device (the ICP result), used as is
         T = _device_rt if _device_rt is not None else _rigid(transform, self.device, "transform")
-        L = _lib.lib()
-        self.ws = torch.empty(int(L.s3r_pcl_index_bytes(self.n)), dtype=torch.uint8, device=self.device)
-        with _lib.on_device(points):
-            _lib.check(L.s3r_pcl_index_build(_lib.ptr(points), _is_f64(points), self.n, _lib.ptr(T), _lib.ptr(self.ws),
-                                             _lib.stream_ptr(self.device)), "s3r_pcl_index_build")
+        self.ws = torch.empty(int(_lib.lib().s3r_pcl_index_bytes(self.n)), dtype=torch.uint8, device=self.device)
+        _lib.call("s3r_pcl_index_build", points, _lib.ptr(points), _is_f64(points), self.n, _lib.ptr(T), _lib.ptr(self.ws))
 
     def query(self, queries: torch.Tensor, max_dist: float = math.inf, transform=None):
         """1-NN of every query (each first mapped by `transform` if given) -> (dist [Q] fp64, idx [Q] int64).  Nothing within
@@ -83,10 +80,8 @@ class PointIndex:
         nq = queries.shape[0]
         dist = torch.empty(nq, dtype=torch.float64, device=self.device)
         idx = torch.empty(nq, dtype=torch.int64, device=self.device)
-        with _lib.on_device(queries):
-            _lib.check(_lib.lib().s3r_pcl_nearest(_lib.ptr(self.ws), self.n, _lib.ptr(queries), _is_f64(queries), nq,
-                                                  _lib.ptr(T), float(max_dist), _lib.ptr(dist), _lib.ptr(idx),
-                                                  _lib.stream_ptr(self.device)), "s3r_pcl_nearest")
+        _lib.call("s3r_pcl_nearest", self.device, _lib.ptr(self.ws), self.n, _lib.ptr(queries), _is_f64(queries), nq,
+                  _lib.ptr(T), float(max_dist), _lib.ptr(dist), _lib.ptr(idx))
         return dist, idx
 
     def normals(self, knn: int = 30) -> torch.Tensor:
@@ -94,9 +89,7 @@ class PointIndex:
         if not 1 <= int(knn) <= 32:
             raise ValueError(f"knn must be in 1..32, got {knn}")
         out = torch.empty(self.n, 3, dtype=torch.float64, device=self.device)
-        with _lib.on_device(self.device):
-            _lib.check(_lib.lib().s3r_pcl_normals(_lib.ptr(self.ws), self.n, int(knn), _lib.ptr(out),
-                                                  _lib.stream_ptr(self.device)), "s3r_pcl_normals")
+        _lib.call("s3r_pcl_normals", self.device, _lib.ptr(self.ws), self.n, int(knn), _lib.ptr(out))
         return out
 
 
@@ -132,14 +125,11 @@ def _icp(source: torch.Tensor, target: PointIndex, max_correspondence_distance, 
     if not 0 <= int(max_iteration) <= 10000:
         raise ValueError(f"max_iteration must be in 0..10000, got {max_iteration}")
     T0 = _rigid(init, target.device, "init")
-    L = _lib.lib()
-    ws = torch.empty(int(L.s3r_pcl_icp_workspace_bytes()), dtype=torch.uint8, device=target.device)
+    ws = torch.empty(int(_lib.lib().s3r_pcl_icp_workspace_bytes()), dtype=torch.uint8, device=target.device)
     out = torch.empty(19 + 2 * (int(max_iteration) + 1), dtype=torch.float64, device=target.device)
-    with _lib.on_device(source):
-        _lib.check(L.s3r_pcl_icp(_lib.ptr(source), _is_f64(source), source.shape[0], _lib.ptr(target.ws), target.n,
-                                 float(max_correspondence_distance), _lib.ptr(T0), int(max_iteration),
-                                 float(relative_fitness), float(relative_rmse), _lib.ptr(ws), _lib.ptr(out),
-                                 _lib.stream_ptr(target.device)), "s3r_pcl_icp")
+    _lib.call("s3r_pcl_icp", target.device, _lib.ptr(source), _is_f64(source), source.shape[0], _lib.ptr(target.ws),
+              target.n, float(max_correspondence_distance), _lib.ptr(T0), int(max_iteration), float(relative_fitness),
+              float(relative_rmse), _lib.ptr(ws), _lib.ptr(out))
     return out
 
 
@@ -159,18 +149,13 @@ def registration_icp(source: torch.Tensor, target: torch.Tensor, max_corresponde
 
 def _stats_into(x: torch.Tensor, out: torch.Tensor, threshold: float = 0.0):
     """out[0:3] = mean, median, count(x < threshold) of the fp64 vector x (device, no synchronisation)."""
-    L = _lib.lib()
-    ws = torch.empty(int(L.s3r_pcl_stats_workspace_bytes()), dtype=torch.uint8, device=x.device)
-    with _lib.on_device(x):
-        _lib.check(L.s3r_pcl_stats(_lib.ptr(x), x.numel(), float(threshold), _lib.ptr(ws), _lib.ptr(out),
-                                   _lib.stream_ptr(x.device)), "s3r_pcl_stats")
+    ws = torch.empty(int(_lib.lib().s3r_pcl_stats_workspace_bytes()), dtype=torch.uint8, device=x.device)
+    _lib.call("s3r_pcl_stats", x, _lib.ptr(x), x.numel(), float(threshold), _lib.ptr(ws), _lib.ptr(out))
 
 
 def _abs_dot(a: torch.Tensor, b: torch.Tensor, idx: torch.Tensor) -> torch.Tensor:
     out = torch.empty(a.shape[0], dtype=torch.float64, device=a.device)
-    with _lib.on_device(a):
-        _lib.check(_lib.lib().s3r_pcl_abs_dot(_lib.ptr(a), _lib.ptr(b), _lib.ptr(idx), a.shape[0], _lib.ptr(out),
-                                              _lib.stream_ptr(a.device)), "s3r_pcl_abs_dot")
+    _lib.call("s3r_pcl_abs_dot", a, _lib.ptr(a), _lib.ptr(b), _lib.ptr(idx), a.shape[0], _lib.ptr(out))
     return out
 
 
@@ -190,10 +175,8 @@ def _one_direction(index: PointIndex, queries, idx_normals, q_normals, query_rt=
         nq = queries.shape[0]
         dist = torch.empty(nq, dtype=torch.float64, device=index.device)
         idx = torch.empty(nq, dtype=torch.int64, device=index.device)
-        with _lib.on_device(queries):
-            _lib.check(_lib.lib().s3r_pcl_nearest(_lib.ptr(index.ws), index.n, _lib.ptr(queries), _is_f64(queries), nq,
-                                                  _lib.ptr(query_rt), math.inf, _lib.ptr(dist), _lib.ptr(idx),
-                                                  _lib.stream_ptr(index.device)), "s3r_pcl_nearest")
+        _lib.call("s3r_pcl_nearest", index.device, _lib.ptr(index.ws), index.n, _lib.ptr(queries), _is_f64(queries), nq,
+                  _lib.ptr(query_rt), math.inf, _lib.ptr(dist), _lib.ptr(idx))
     res = torch.empty(6, dtype=torch.float64, device=index.device)
     _stats_into(dist, res[0:3])
     if idx_normals is None:

@@ -357,23 +357,18 @@ class ViewBuilder:
         if jitter is not None:
             hb[jd_off:jd_off + C.sizeof(jds)] = np.frombuffer(bytes(jds), dtype=np.uint8)
         buf.copy_(host, non_blocking=True)
-        L = _lib.lib()
         max_pix = max(p["out"][0] * p["out"][1] for (_, _, _, p, _, _) in views)
         max_rows = max(g["rows"] for (*_, g) in views)
         max_cols = max(p["out"][0] for (_, _, _, p, _, _) in views)
         max_out_rows = max(p["out"][1] for (_, _, _, p, _, _) in views)
         max_span = max(g["span"] for (*_, g) in views)
-        with _lib.on_device(buf):
-            sp = _lib.stream_ptr(dev)
-            _lib.check(L.s3r_views_depth(base + dd_off, n, max_pix, sp), "s3r_views_depth")
-            _lib.check(L.s3r_views_resample_h(base + id_off, n, max_rows, max_cols, max_span, sp), "s3r_views_resample_h")
-            if jitter is None:
-                _lib.check(L.s3r_views_resample_v_norm(base + id_off, n, max_out_rows, max_cols, sp),
-                           "s3r_views_resample_v_norm")
-            else:
-                _lib.check(L.s3r_views_resample_v_u8(base + id_off, base + jd_off, n, max_out_rows, max_cols, sp),
-                           "s3r_views_resample_v_u8")
-                _lib.check(L.s3r_views_color_jitter(base + jd_off, n, max_pix, sp), "s3r_views_color_jitter")
+        _lib.call("s3r_views_depth", buf, base + dd_off, n, max_pix)
+        _lib.call("s3r_views_resample_h", buf, base + id_off, n, max_rows, max_cols, max_span)
+        if jitter is None:
+            _lib.call("s3r_views_resample_v_norm", buf, base + id_off, n, max_out_rows, max_cols)
+        else:
+            _lib.call("s3r_views_resample_v_u8", buf, base + id_off, base + jd_off, n, max_out_rows, max_cols)
+            _lib.call("s3r_views_color_jitter", buf, base + jd_off, n, max_pix)
         bad = nonfinite.cpu().nonzero().flatten().tolist()     # waits for the launches
         if bad:
             raise ValueError(f"NaN / inf in the cropped depth map of view(s) {bad}")

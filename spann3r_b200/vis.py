@@ -148,22 +148,18 @@ def render_frames(pts_all, image_all, camera_parameters, output_dir=None, mask=N
     if not (math.isfinite(z_near) and z_near >= 0):
         raise ValueError(f"z_near must be finite and >= 0, got {z_near}")
     _lib.require_device()
-    L = _lib.lib()
     T, H, W, _ = pts_all.shape
     per = H * W
     dev = pts_all.device
-    keys = torch.empty(int(L.s3r_render_workspace_bytes(w, h)) // 8, dtype=torch.int64, device=dev)
+    keys = torch.empty(int(_lib.lib().s3r_render_workspace_bytes(w, h)) // 8, dtype=torch.int64, device=dev)
     frames = torch.empty((T, h, w, 3), dtype=torch.uint8, device=dev)
     cam_p = C.c_void_p(cam.ctypes.data)
-    with _lib.on_device(dev):
-        st = _lib.stream_ptr(dev)
-        for i in range(T):
-            if dynamic or i == 0:
-                _lib.check(L.s3r_render_clear(_lib.ptr(keys), w, h, st), "s3r_render_clear")
-            _lib.check(L.s3r_render_splat(_lib.ptr(pts_all[i]), _lib.ptr(None if mask is None else mask[i]), per, i * per,
-                                          cam_p, float(z_near), w, h, _lib.ptr(keys), st), "s3r_render_splat")
-            _lib.check(L.s3r_render_resolve(_lib.ptr(keys), _lib.ptr(image_all), w, h, _lib.ptr(frames[i]), st),
-                       "s3r_render_resolve")
+    for i in range(T):
+        if dynamic or i == 0:
+            _lib.call("s3r_render_clear", dev, _lib.ptr(keys), w, h)
+        _lib.call("s3r_render_splat", dev, _lib.ptr(pts_all[i]), _lib.ptr(None if mask is None else mask[i]), per, i * per,
+                  cam_p, float(z_near), w, h, _lib.ptr(keys))
+        _lib.call("s3r_render_resolve", dev, _lib.ptr(keys), _lib.ptr(image_all), w, h, _lib.ptr(frames[i]))
     if output_dir is not None:
         write_frames(frames, output_dir, camera_parameters if save_camera else None, save_video)
     return frames
@@ -190,24 +186,19 @@ def render_mesh_frames(pts_all, image_all, camera_parameters, output_dir=None, m
                                 torch.arange(T + 1, dtype=torch.int32, device=faces.device)).cpu().tolist()
     if len(colors) == 0:
         colors = torch.zeros((1, 3), dtype=torch.float32, device=pts_all.device)   # never read: no face is drawn
-    L = _lib.lib()
     dev = pts_all.device
-    keys = torch.empty(int(L.s3r_render_workspace_bytes(w, h)) // 8, dtype=torch.int64, device=dev)
+    keys = torch.empty(int(_lib.lib().s3r_render_workspace_bytes(w, h)) // 8, dtype=torch.int64, device=dev)
     frames = torch.empty((T, h, w, 3), dtype=torch.uint8, device=dev)
     cam_p = C.c_void_p(cam.ctypes.data)
-    with _lib.on_device(dev):
-        st = _lib.stream_ptr(dev)
-        for i in range(T):
-            if dynamic or i == 0:
-                _lib.check(L.s3r_render_clear(_lib.ptr(keys), w, h, st), "s3r_render_clear")
-            f = faces[bounds[i]:bounds[i + 1]]
-            if len(f):
-                _lib.check(L.s3r_raster_triangles(_lib.ptr(verts), len(verts), _lib.ptr(f), len(f), bounds[i], cam_p,
-                                                  float(z_near), math.inf, w, h, _lib.ptr(keys), st),
-                           "s3r_raster_triangles")
-            # the keys hold face ids: the render resolve gathers the face colours
-            _lib.check(L.s3r_render_resolve(_lib.ptr(keys), _lib.ptr(colors), w, h, _lib.ptr(frames[i]), st),
-                       "s3r_render_resolve")
+    for i in range(T):
+        if dynamic or i == 0:
+            _lib.call("s3r_render_clear", dev, _lib.ptr(keys), w, h)
+        f = faces[bounds[i]:bounds[i + 1]]
+        if len(f):
+            _lib.call("s3r_raster_triangles", dev, _lib.ptr(verts), len(verts), _lib.ptr(f), len(f), bounds[i], cam_p,
+                      float(z_near), math.inf, w, h, _lib.ptr(keys))
+        # the keys hold face ids: the render resolve gathers the face colours
+        _lib.call("s3r_render_resolve", dev, _lib.ptr(keys), _lib.ptr(colors), w, h, _lib.ptr(frames[i]))
     if output_dir is not None:
         write_frames(frames, output_dir, camera_parameters if save_camera else None, save_video)
     return frames

@@ -56,7 +56,7 @@ def test_no_cpu_fallback(spec):
 
 
 def test_library_exports_every_declared_symbol():
-    from spann3r_b200 import _lib, engine  # noqa: F401  (engine registers the model-level prototypes)
+    from spann3r_b200 import _lib
     if not os.path.exists(_lib.LIB_PATH):
         import __graft_entry__
         __graft_entry__.build()
@@ -242,15 +242,15 @@ def test_pairwise_and_offline_control_flow_on_a_fake_engine(monkeypatch):
     assert all(c == ("value", True, False) for c in eng.calls if c[0] == "value")
 
 
-def test_ctypes_prototypes_match_the_header():
+def test_prototype_table_matches_the_header():
     """Every function declared in include/spann3r_b200.h is bound in Python with the same number of arguments and the same
     scalar kinds (pointer / int / int64 / uint64 / float / double / size_t) -- guards the ctypes layer against ABI drift."""
     import ctypes as C
-    from spann3r_b200 import _lib, engine  # noqa: F401
+    from spann3r_b200 import _lib
     header = open(os.path.join(ROOT, "include", "spann3r_b200.h")).read()
     header = re.sub(r"/\*.*?\*/", " ", header, flags=re.S)
     header = re.sub(r"^\s*#.*$", " ", header, flags=re.M)
-    protos = {**_lib._PROTOS, **_lib._EXTRA_PROTOS}
+    protos = _lib._PROTOS
 
     def kind_c(t):
         t = t.strip()

@@ -211,8 +211,8 @@ def test_run_sharded_independent_passes_the_ranks_sequences():
 SLOT_SYMBOLS = {"s3r_engine_memory_read_slots": 7, "s3r_engine_memory_append_slots": 7, "s3r_engine_check_sim_slots": 7}
 
 
-def test_slot_symbols_are_exported_with_their_declared_arity():
-    from spann3r_b200 import _lib, engine  # noqa: F401  (engine registers the model-level prototypes)
+def test_slot_symbols_are_exported_and_bound_with_their_declared_arity():
+    from spann3r_b200 import _lib, engine
     if not os.path.exists(_lib.LIB_PATH):
         import __graft_entry__
         __graft_entry__.build()
@@ -222,4 +222,4 @@ def test_slot_symbols_are_exported_with_their_declared_arity():
     for name, arity in SLOT_SYMBOLS.items():
         assert hasattr(L, name), name
         assert name + "(" in header, name
-        assert len(_lib._EXTRA_PROTOS[name][1]) == arity, name
+        assert len(_lib._PROTOS[name][1]) == arity, name
